@@ -9,8 +9,7 @@ import shutil
 import subprocess
 
 _HERE = os.path.dirname(os.path.realpath(__file__))
-# PYFLYT_B200_LIB: development override used by tools/ to time experimental builds of the SAME library (lib/variants/...)
-LIB_PATH = os.environ.get("PYFLYT_B200_LIB") or os.path.join(_HERE, "lib", "libpyflyt_b200.so")
+LIB_PATH = os.path.join(_HERE, "lib", "libpyflyt_b200.so")
 _lib = None
 
 

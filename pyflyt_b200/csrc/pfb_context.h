@@ -62,29 +62,23 @@ struct PfbContext {
   cudaEvent_t ev_step;     // recorded on the caller's stream after a step launch; the side stream waits on it
   cudaEvent_t ev_spare[4]; // ev_spare[k % 4]: spares consumed by step k are rebuilt; step k + 2 waits on it
   int64_t side_launches;
-  // optional per-step CUDA-event pairs around the dominant kernel (bench.py's roofline leg)
-  int mapped_dyn_smem;    // dynamic shared memory requested by the step launch of pfb_env_step_mapped (bounds the CTAs resident per SM: several waves)
-  int step_dyn_smem;      // what the next QuadX-Hover step launch requests (0 = everything resident in one wave)
   float* noise_dump;      // optional [substeps per env step][N] device buffer: the step kernel writes every noise draw it hands out (tests)
+  // optional per-step CUDA-event pairs around the dominant kernel (bench.py's roofline leg)
   cudaEvent_t* prof_ev;   // [2 * prof_cap]
   int prof_cap;
   int prof_n;
 };
 
 // One warp per CTA: a CTA retires as soon as its own warp is done, so the SM back-fills sooner and the single wave has a
-// shorter tail (PFB_BLOCK: A/B knob).  448 threads per SM resident (<= 146 regs/thread) for the generic kernels.
-#ifndef PFB_BLOCK  // A/B knob (per translation unit): threads per CTA
-#define PFB_BLOCK 32
-#endif
-constexpr int kBlock = PFB_BLOCK;
-constexpr int kMinBlocks = 448 / kBlock > 0 ? 448 / kBlock : 1;
+// shorter tail.  448 threads per SM resident (<= 146 regs/thread) for the generic kernels.  The warp-tiled QuadX-Hover
+// kernels index their 32-env tile by threadIdx.x and ballot over the full warp, so they depend on this being one warp.
+constexpr int kBlock = 32;
+static_assert(kBlock == pfb::kTileLanes, "one warp per CTA: the Hover kernels map lane threadIdx.x onto a 32-env tile");
+constexpr int kMinBlocks = 448 / kBlock;
 // the step kernels of the aerodynamic-surface vehicles (Fixedwing-Waypoints, Dogfight): the batch sizes they run at leave
 // < 4 warps per SM, so registers are better spent on interleaving the surfaces than on residency (8 CTAs / SM, up to
-// 255 registers, rather than 14 CTAs / SM at 128).  PFB_AERO_MIN_BLOCKS: A/B knob
-#ifndef PFB_AERO_MIN_BLOCKS
-#define PFB_AERO_MIN_BLOCKS 8
-#endif
-constexpr int kAeroBlocks = PFB_AERO_MIN_BLOCKS;
+// 255 registers, rather than 14 CTAs / SM at 128)
+constexpr int kAeroBlocks = 8;
 
 static inline int grid_for(int64_t n) { return (int)((n + kBlock - 1) / kBlock); }
 

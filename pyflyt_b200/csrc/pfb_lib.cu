@@ -132,13 +132,10 @@ __global__ void __launch_bounds__(kBlock) k_quadx_observe(const float* __restric
 // ---------------------------------------------------------------------------------------------------
 // kernels — QuadX-Hover env (warp-tiled state)
 // ---------------------------------------------------------------------------------------------------
-// 512 threads per SM resident (<= 128 registers), so that the 2048 CTAs of a 65 536-env step and the builder CTAs of the spare
-// rebuild (two per SM) are resident at once or nearly so.  On an H100 a small second wave remains; capping the builders to remove
-// it was measured slower, because each builder then carries more of the serial warm-up chains (DESIGN.md §4)
-#ifndef PFB_HOVER_THREADS
-#define PFB_HOVER_THREADS 512
-#endif
-constexpr int kHoverBlocks = PFB_HOVER_THREADS / kBlock;
+// 16 one-warp CTAs (512 threads) per SM resident (<= 128 registers), so that the 2048 CTAs of a 65 536-env step and the builder
+// CTAs of the spare rebuild (two per SM) are resident at once or nearly so.  On an H100 a small second wave remains; capping the
+// builders to remove it was measured slower, because each builder then carries more of the serial warm-up chains (DESIGN.md §4)
+constexpr int kHoverBlocks = 16;
 constexpr int kObsMax = 24;  // floats per observation row (20 / 21, + 3 for MAQuadXHover)
 
 // ---- spare post-reset states (DESIGN.md §4, "reset pipeline") ---------------------------------------
@@ -163,10 +160,7 @@ enum { SP_POSE = QX_ROWS, SP_VALID = QX_ROWS + 6, SP_FLAGS = QX_ROWS + 7, SP_EPI
 static_assert(QX_ROWS % 4 == 0 && QX_ROWS + 16 <= SP_ROWS && SP_ROWS % 4 == 0, "spare record layout");
 constexpr int kSpareBufs = 4;  // records per env, buffer = episode & 3: the step pipeline uses two neighbours (one being consumed, one being built);
 constexpr uint32_t kSpareMask = kSpareBufs - 1;  // the fused rollout keeps three spares ahead (k_hover_rollout)
-#ifndef PFB_WARM_SPLIT
-#define PFB_WARM_SPLIT 5
-#endif
-constexpr int kWarmSplit = PFB_WARM_SPLIT;  // Aviary steps integrated by the first builder phase; every warm-up requantizes its state there
+constexpr int kWarmSplit = 5;  // Aviary steps integrated by the first builder phase; every warm-up requantizes its state there
 
 // cp.async.bulk (TMA, 1-D) shared -> global: one instruction moves a warp's whole observation tile
 __device__ __forceinline__ void bulk_store_s2g(void* gdst, const void* ssrc, uint32_t bytes) {
@@ -200,18 +194,6 @@ __device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity, float 
 }
 __device__ __forceinline__ void bulk_store_wait_read() { asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory"); }
 __device__ __forceinline__ void fence_async_smem() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
-#ifdef PFB_TIMELINE
-// experiment build (tools/exp_timeline.py): every warp of the step launch stamps %globaltimer at four points into the buffer
-// that normally receives the noise dump: [warp][4] uint64 = entry, inputs landed, integration done, exit
-__device__ __forceinline__ unsigned long long gtimer() {
-  unsigned long long t;
-  asm volatile("mov.u64 %0, %globaltimer;" : "=l"(t));
-  return t;
-}
-#define PFB_TL(slot) do { if (noise_dump && threadIdx.x == 0) reinterpret_cast<unsigned long long*>(noise_dump)[(size_t)blockIdx.x * 4 + (slot)] = gtimer(); } while (0)
-#else
-#define PFB_TL(slot) do { } while (0)
-#endif
 __device__ __forceinline__ void prefetch_l1(const void* p) { asm volatile("prefetch.global.L1 [%0];" ::"l"(p)); }
 // per-thread asynchronous copies global -> shared (LDGSTS): issued and forgotten, complete in the background, waited for with
 // cp_async_wait_all() by the issuing thread, which may then read what it copied
@@ -271,7 +253,7 @@ __device__ __forceinline__ void hover_build(const QuadXParams& p, const HoverPar
                                             const int32_t* __restrict__ b1_count, const int32_t* __restrict__ b1_list,
                                             uint32_t* __restrict__ b0_elist, const uint32_t* __restrict__ b1_elist,
                                             const float* __restrict__ start_pos, const float* __restrict__ start_orn,
-                                            float* __restrict__ spare, uint32_t* __restrict__ episode, int64_t N, float* noise_dump = nullptr) {
+                                            float* __restrict__ spare, uint32_t* __restrict__ episode, int64_t N) {
   const int phase = b >= builders ? 1 : 0;
   const int slot = b - phase * builders;
   const int32_t* __restrict__ list = phase ? b1_list : b0_list;
@@ -303,12 +285,7 @@ __device__ __forceinline__ void hover_build(const QuadXParams& p, const HoverPar
       const F4 sp = ld_f4(rec + SP_SETPOINT);
       s.sp[0] = sp.x; s.sp[1] = sp.y; s.sp[2] = sp.z; s.sp[3] = sp.w;
     }
-#ifdef PFB_TIMELINE
-    if (s.flags == 0xffffffffu) return;  // consume the loaded state before the stamp
-#endif
-    PFB_TL(1);
     hover_warmup_inline<MODE, false>(p, s, phase ? split : 0, phase ? h.warmup_steps : split, rng, nullptr, N, i, e);
-    PFB_TL(2);
     quadx_store_tile<7, 4>(rec, s, 0);
     if (phase == 0) {
       st_f4(rec + SP_POSE, px, py, pz, ox);
@@ -347,18 +324,12 @@ __global__ void __launch_bounds__(kBlock, kHoverBlocks)
   // builder CTAs come FIRST in the grid: their serial warm-up chain is the longest thing in the launch, so they must be
   // dispatched at t = 0, not behind the ~2000 step CTAs
   const int n_build = AUTORESET ? 2 * builders : 0;
-  PFB_TL(0);
   if (AUTORESET && (int)blockIdx.x < n_build) {  // builder CTA (CTA-uniform role)
     hover_build<MODE>(p, h, rng, (int)blockIdx.x, builders, b0_count, b0_list, b1_count, b1_list, b0_elist, b1_elist, start_pos, start_orn, spare,
-                      episode, N, noise_dump);
-    PFB_TL(3);
+                      episode, N);
     return;
   }
   const int tile = (int)blockIdx.x - n_build;
-  if (h.stagger_ns > 0) {  // experiment: de-synchronise the memory phases of the single wave
-    const int late = tile % h.stagger_mod;
-    if (late) __nanosleep((unsigned)(late * h.stagger_ns));
-  }
   __shared__ __align__(128) float smem[kBlock * kObsMax];
   const int O = (h.angle_representation == 0 ? 20 : 21) + (MA ? 3 : 0);
   const int lane = threadIdx.x;
@@ -382,9 +353,7 @@ __global__ void __launch_bounds__(kBlock, kHoverBlocks)
   float past[4] = {0.f, 0.f, 0.f, 0.f};
   auto nz = make_noise<INJECT>(noise, N, active ? i : 0, rng, step_seq, TAG_ENV_STEP, p.noise_loc, p.ratio);
   nz.prefetch4();
-#ifndef PFB_TIMELINE
   if (!INJECT && noise_dump && active) nz.set_dump(noise_dump + i, N);
-#endif
   if (RANDACT) {
     uint64_t g = ((uint64_t)rng.env_offset_hi << 32 | rng.env_offset_lo) + (uint64_t)i;
     U4 r = philox4x32_10(U4{(uint32_t)g, (uint32_t)(g >> 32), step_seq, (uint32_t)TAG_ACTION << 24}, rng.k0, rng.k1);
@@ -408,7 +377,6 @@ __global__ void __launch_bounds__(kBlock, kHoverBlocks)
   int step_count;
   mbar_wait(&mbar, 0, nz.dep(0), nz.dep(1), nz.dep(2), nz.dep(3), nz.dep(4), nz.dep(5), nz.dep(6), nz.dep(7));  // the tile has landed
   quadx_load_tile<MODE, kTileGroupStride>(stile + lane * 4, s, step_count);  // LDS.128, conflict-free (lane-contiguous vectors)
-  PFB_TL(1);
   // an env that finished on the previous call: this call is its reset (NEXT_STEP)
   const bool resetting = AUTORESET && active && (s.flags & (FLAG_TERM | FLAG_TRUNC)) != 0;
   const float* staged = nullptr;  // this lane's spare record + start pose in shared memory (see kStageFloats)
@@ -457,7 +425,6 @@ __global__ void __launch_bounds__(kBlock, kHoverBlocks)
     else hover_term_trunc_reward(h, s, step_count, rew);
   }
   step_count += 1;
-  PFB_TL(2);
   if (AUTORESET && __any_sync(0xffffffffu, resetting)) {
     if (resetting) {
       // env.reset(): begin_reset + end_reset (quadx_base_env.py:149-212) — normally a copy of the env's spare
@@ -532,7 +499,6 @@ __global__ void __launch_bounds__(kBlock, kHoverBlocks)
     }
   }
   if (bulk && lane == 0) bulk_store_wait_read();  // the CTA's shared memory must outlive the engine's reads
-  PFB_TL(3);
 }
 
 // ---------------------------------------------------------------------------------------------------
@@ -921,12 +887,6 @@ int pfb_create(const PfbModel* model, const PfbEnvConfig* env, int64_t n_envs, i
     c->hover.dome2 = (float)(dome * dome);
   }
   c->hover.ma = (env && env->env_kind == PFB_ENV_MA_QUADX_HOVER) ? 1 : 0;
-  c->hover.stagger_ns = 0;
-  c->hover.stagger_mod = 1;
-  if (const char* e = getenv("PFB_HOVER_STAGGER")) {
-    int ns = 0, mod = 2;
-    if (sscanf(e, "%d,%d", &ns, &mod) >= 1 && ns >= 0 && ns <= 20000 && mod >= 1 && mod <= 8) { c->hover.stagger_ns = ns; c->hover.stagger_mod = mod; }
-  }
   if (c->hover.ma && env->autoreset) {
     delete c;
     return fail("MAQuadXHover is a per-agent epilogue: arenas are reset by the caller (pfb_env_reset with a mask), autoreset must be 0");
@@ -966,15 +926,6 @@ int pfb_create(const PfbModel* model, const PfbEnvConfig* env, int64_t n_envs, i
   cudaDeviceProp prop;
   CUDA_OK(cudaGetDeviceProperties(&prop, device));
   c->sm_count = prop.multiProcessorCount;
-  // pfb_env_step_mapped: the kernel reads / writes host memory over PCIe, which is the bottleneck by 10x; with every CTA resident
-  // in one wave the bus idles while all warps compute and then takes the whole output at once.  Requesting dynamic shared
-  // memory the kernel never touches caps the CTAs resident per SM, so the step runs as several waves and the output of a wave
-  // crosses the bus while the next one computes.  PFB_MAPPED_DYN_SMEM overrides (bytes, <= 48 KB; 0 = one wave).
-  c->mapped_dyn_smem = 12 * 1024;  // tools/exp_mapped_waves.py sweeps it
-  if (const char* e = getenv("PFB_MAPPED_DYN_SMEM")) {
-    const int v = atoi(e);
-    if (v >= 0 && v <= 40 * 1024) c->mapped_dyn_smem = v;
-  }
   CUDA_OK(cudaMalloc(&c->d_counters, 8 * sizeof(int32_t)));  // [0..3] rotating autoreset counters, [4] ticket of the split dogfight
   CUDA_OK(cudaMemset(c->d_counters, 0, 8 * sizeof(int32_t)));
   CUDA_OK(cudaMalloc(&c->d_done_list, 4 * (size_t)n_envs * sizeof(int32_t)));
@@ -1171,7 +1122,9 @@ int pfb_env_reset(PfbHandle h, const uint8_t* mask, const float* noise, void* st
   return 0;
 }
 
-static int env_step_impl(PfbHandle h, float* actions, const float* noise, bool randact, cudaStream_t s) {
+// `dyn_smem`: dynamic shared memory the QuadX-Hover step launch requests and never touches (pfb_env_step_mapped; 0 = every CTA
+// resident in one wave)
+static int env_step_impl(PfbHandle h, float* actions, const float* noise, bool randact, size_t dyn_smem, cudaStream_t s) {
   if (is_df(h)) return df_env_step(h, actions, noise, randact, s);
   if (is_fw(h)) return fw_env_step(h, actions, noise, randact, s);
   if (is_rk(h)) return rk_env_step(h, actions, noise, randact, s);
@@ -1197,7 +1150,6 @@ static int env_step_impl(PfbHandle h, float* actions, const float* noise, bool r
   const int builders = spares ? (h->sm_count < tiles ? h->sm_count : tiles) : 0;
   const int grid = tiles + 2 * builders;
   const bool prof = h->prof_ev && h->prof_n < h->prof_cap;
-  const size_t dyn_smem = (size_t)h->step_dyn_smem;
   if (prof) CUDA_OK(cudaEventRecord(h->prof_ev[2 * h->prof_n], s));
 #define STEP_ARGS h->qx, h->hover, h->rng, h->buf.state, qx_rows(h), actions, noise, h->buf.obs, h->buf.reward, h->buf.term, h->buf.trunc,    \
                   h->buf.info, h->buf.start_pos, h->buf.start_orn, cnt_cur, list_cur, cnt_next, cnt_b0, list_b0, cnt_b1, list_b1, elist_b0,   \
@@ -1285,7 +1237,7 @@ int pfb_env_step(PfbHandle h, const float* actions, const float* noise, void* st
   REQUIRE_BOUND(h);
   if (require_env(h)) return -1;
   if (actions && ((uintptr_t)actions & 15)) return fail("pfb_env_step: actions must be 16-byte aligned");
-  return env_step_impl(h, actions ? const_cast<float*>(actions) : h->buf.setpoint, noise, false, (cudaStream_t)stream);
+  return env_step_impl(h, actions ? const_cast<float*>(actions) : h->buf.setpoint, noise, false, 0, (cudaStream_t)stream);
 }
 
 // QuadX-Hover with autoreset: n_steps >= kFusedMinSteps run as fused launches of up to kRolloutMaxSteps env steps (k_hover_rollout)
@@ -1335,10 +1287,9 @@ static int hover_rollout_fused(PfbHandle h, int n_steps, cudaStream_t s) {
 int pfb_env_rollout(PfbHandle h, int n_steps, void* stream) {
   REQUIRE_BOUND(h);
   if (require_env(h)) return -1;
-  static const int fused_min = getenv("PFB_FUSED_MIN") ? atoi(getenv("PFB_FUSED_MIN")) : kFusedMinSteps;  // tests / experiments
-  if (n_steps >= fused_min && hover_fused_ok(h)) return hover_rollout_fused(h, n_steps, (cudaStream_t)stream);
+  if (n_steps >= kFusedMinSteps && hover_fused_ok(h)) return hover_rollout_fused(h, n_steps, (cudaStream_t)stream);
   for (int k = 0; k < n_steps; ++k)
-    if (env_step_impl(h, h->buf.setpoint, nullptr, true, (cudaStream_t)stream)) return -1;
+    if (env_step_impl(h, h->buf.setpoint, nullptr, true, 0, (cudaStream_t)stream)) return -1;
   return 0;
 }
 
@@ -1349,7 +1300,7 @@ int pfb_env_step_host(PfbHandle h, const float* host_actions, float* host_obs, f
   cudaStream_t s = (cudaStream_t)stream;
   const int O = pfb_obs_dim(h);
   CUDA_OK(cudaMemcpyAsync(h->buf.setpoint, host_actions, (size_t)h->n * pfb_setpoint_dim(h) * sizeof(float), cudaMemcpyHostToDevice, s));
-  if (env_step_impl(h, h->buf.setpoint, nullptr, false, s)) return -1;
+  if (env_step_impl(h, h->buf.setpoint, nullptr, false, 0, s)) return -1;
   // obs | reward | term | trunc laid out back to back on both sides (what the Python mirror allocates): one copy, one
   // PCIe transaction stream instead of four latency-bound ones
   const size_t ob = (size_t)h->n * O * sizeof(float), rb = (size_t)h->n * sizeof(float), fb = (size_t)h->n;
@@ -1371,6 +1322,10 @@ int pfb_env_step_host(PfbHandle h, const float* host_actions, float* host_obs, f
 // Zero-copy variant of pfb_env_step_host: the step kernel reads the actions from, and writes obs / reward / term / trunc
 // straight into, PINNED (device-mapped) host memory.  The PCIe transfers then overlap the launch tile by tile instead of
 // bracketing it as two copies; no staging through the bound device buffers.
+// The PCIe link is the bottleneck by 10x; with every CTA resident in one wave the bus idles while all warps compute and then
+// takes the whole output at once.  Requesting dynamic shared memory the kernel never touches caps the CTAs resident per SM, so
+// the step runs as several waves and the output of a wave crosses the bus while the next one computes.
+constexpr size_t kMappedDynSmem = 12 * 1024;
 int pfb_env_step_mapped(PfbHandle h, const float* host_actions, float* host_obs, float* host_reward, uint8_t* host_term,
                         uint8_t* host_trunc, void* stream) {
   REQUIRE_BOUND(h);
@@ -1386,9 +1341,7 @@ int pfb_env_step_mapped(PfbHandle h, const float* host_actions, float* host_obs,
   if (((uintptr_t)da & 15) || ((uintptr_t)dob & 15)) return fail("pfb_env_step_mapped: actions and obs must be 16-byte aligned");
   const PfbBuffers saved = h->buf;
   h->buf.obs = (float*)dob; h->buf.reward = (float*)dr; h->buf.term = (uint8_t*)dte; h->buf.trunc = (uint8_t*)dtr;
-  h->step_dyn_smem = h->mapped_dyn_smem;
-  const int rc = env_step_impl(h, (float*)da, nullptr, false, (cudaStream_t)stream);
-  h->step_dyn_smem = 0;
+  const int rc = env_step_impl(h, (float*)da, nullptr, false, kMappedDynSmem, (cudaStream_t)stream);
   h->buf = saved;
   return rc;
 }

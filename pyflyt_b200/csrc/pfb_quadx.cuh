@@ -66,7 +66,6 @@ struct HoverParams {
   int flight_mode;
   float dome2;  // flight_dome_size squared (inf stays inf)
   int ma;       // 1: MAQuadXHover per-agent epilogue (pz_envs/quadx_envs/ma_quadx_hover_env.py)
-  int stagger_ns, stagger_mod;  // experiment (PFB_HOVER_STAGGER=ns,mod): tile t starts (t % mod) * ns late, see DESIGN.md 9
 };
 
 // QuadX-Waypoints constants (gym_envs/quadx_envs/quadx_waypoints_env.py:38-52, utils/waypoint_handler.py)
