@@ -51,6 +51,9 @@ extern "C" {
 #define PFB_MAX_MOTORS 4
 #define PFB_MAX_SURFACES 5
 #define PFB_MAX_SHAPES 16
+/* Distinct vehicle tables one QuadX handle can fly at once (pfb_set_models).  The K tables travel as ONE kernel argument of
+ * K x 640 bytes (fp32 tables), so the cap keeps that argument at 10 KB, well inside the 32 KB kernel-argument limit.      */
+#define PFB_MAX_QUADX_MODELS 16
 
 #define PFB_SHAPE_BOX 0
 #define PFB_SHAPE_CYLINDER 1
@@ -252,6 +255,14 @@ int pfb_reseed(PfbHandle h, uint64_t seed, void* stream);
 /* Global index of this handle's env 0 (rank * n_envs when the batch is sharded over GPUs): keeps
  * the Philox streams, and therefore every trajectory, independent of the number of ranks.          */
 int pfb_set_env_offset(PfbHandle h, uint64_t first_global_env);
+
+/* Several vehicle models in one QuadX handle (Aviary(drone_options=[...]) with one dict per drone, aviary.py:75,196-199):
+ * installs k QuadX tables and env i flies models[index_host[i]] (host array of n_envs entries, each < k).  Every table must
+ * be QuadX with the same physics_hz and control_hz (one substep ratio per handle), 1 <= k <= PFB_MAX_QUADX_MODELS.  k = 1
+ * makes the handle uniform again (the same kernels as a handle created with that table).  An analytic wind set with
+ * pfb_set_wind reaches every table, before or after this call.  Not for MAQuadXHover handles.  A set-up call like
+ * pfb_create: it synchronises the device, and it invalidates the spare post-reset states; follow it with pfb_env_reset.   */
+int pfb_set_models(PfbHandle h, const PfbModel* models, int k, const uint8_t* index_host);
 
 /* Aviary.register_wind_field_function for an analytic field (NULL or kind PFB_WIND_NONE: still air).  Takes effect from the
  * next call on; every vehicle kind.                                                                                  */

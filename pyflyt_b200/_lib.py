@@ -75,6 +75,7 @@ def lib() -> C.CDLL:
     L.pfb_set_noise_dump.argtypes = [vp, vp]
     L.pfb_reseed.argtypes = [vp, u64, vp]
     L.pfb_set_wind.argtypes = [vp, vp]
+    L.pfb_set_models.argtypes = [vp, vp, i32, vp]
     L.pfb_bind.argtypes = [vp, vp]
     L.pfb_reset.argtypes = [vp, vp, vp]
     L.pfb_set_mode.argtypes = [vp, i32, vp]
@@ -108,7 +109,7 @@ def check(rc: int) -> None:
 
 EXPORTS = [
     "pfb_last_error", "pfb_abi_version", "pfb_sizeof_model", "pfb_sizeof_env_config", "pfb_sizeof_buffers",
-    "pfb_model_from_files", "pfb_create", "pfb_destroy", "pfb_set_env_offset", "pfb_state_rows", "pfb_state_layout", "pfb_state_floats", "pfb_set_noise_dump", "pfb_reseed", "pfb_set_wind", "pfb_sizeof_wind",
+    "pfb_model_from_files", "pfb_create", "pfb_destroy", "pfb_set_env_offset", "pfb_state_rows", "pfb_state_layout", "pfb_state_floats", "pfb_set_noise_dump", "pfb_reseed", "pfb_set_wind", "pfb_sizeof_wind", "pfb_set_models",
     "pfb_istate_rows", "pfb_setpoint_dim",
     "pfb_obs_dim", "pfb_aux_dim", "pfb_bind", "pfb_reset", "pfb_set_mode", "pfb_aviary_step", "pfb_observe_state",
     "pfb_set_base_velocity",

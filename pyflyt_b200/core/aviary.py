@@ -8,6 +8,11 @@ Mirrors the surface of the reference's ``Aviary`` that its environments use
 difference in meaning: drone ``i`` lives in its OWN world (the reference puts them in one Bullet world),
 so ``contact_array[i]`` is "drone i touched the floor during the last step".
 
+``drone_options`` may be a sequence with one dict per drone, as in the reference (aviary.py:75): a QuadX batch then flies up
+to ``MAX_QUADX_MODELS`` different vehicle tables (``models``), drone ``i`` the table ``model_index[i]``.  All of them must run
+at the same ``control_hz``.  Drones ``32 k .. 32 k + 31`` share one warp: a batch runs fastest when each such tile flies one
+model (DESIGN.md §4a).
+
 All state is held in caller-visible ``torch`` tensors; the CUDA library (libpyflyt_b200.so) only sees
 raw device pointers.  There is no CPU path.
 """
@@ -21,7 +26,7 @@ import numpy as np
 import torch
 
 from .. import _lib
-from ..models import PfbEnvConfig, build_model
+from ..models import ModelSetError, PfbEnvConfig, PfbModel, build_model, build_model_set
 
 
 class AviaryInitException(Exception):
@@ -45,7 +50,7 @@ class BatchedAviary:
         start_pos,
         start_orn,
         drone_type: str = "quadx",
-        drone_options: dict[str, Any] | None = None,
+        drone_options: dict[str, Any] | Sequence[dict[str, Any]] | None = None,
         physics_hz: int = 240,
         seed: None | int = None,
         device: str | torch.device = "cuda:0",
@@ -65,16 +70,29 @@ class BatchedAviary:
             drone_type = drone_type[0]
         if drone_type not in ("quadx", "fixedwing", "rocket"):
             raise AviaryInitException(f"Can't find `drone_type` {drone_type} amongst known types ['quadx', 'fixedwing', 'rocket'].")
+        # one options dict per drone (aviary.py:75, 196-199): the distinct vehicle tables + the model index of every drone
+        models, index = None, None
+        if drone_options is not None and not isinstance(drone_options, dict):
+            try:
+                models, index = build_model_set(drone_type, drone_options, physics_hz, int(start_pos.shape[0]))
+            except ModelSetError as e:
+                raise AviaryInitException(str(e)) from None
         if not torch.cuda.is_available():
             raise _lib.PfbError("pyflyt_b200 needs a CUDA device (H100, sm_90a); there is no CPU fallback.")
-        opts = dict(drone_options or {})
-        control_hz = int(opts.pop("control_hz", 120))
         self.device = torch.device(device)
         self.num_drones = int(start_pos.shape[0])
         self.drone_type = drone_type
         self.physics_hz = int(physics_hz)
         self.physics_period = 1.0 / physics_hz
-        self.model = build_model(drone_type, opts.pop("drone_model", None), opts.pop("model_dir", None), physics_hz, control_hz, **opts)
+        if models is None:
+            opts = dict(drone_options or {})
+            control_hz = int(opts.pop("control_hz", 120))
+            self.model = build_model(drone_type, opts.pop("drone_model", None), opts.pop("model_dir", None), physics_hz, control_hz, **opts)
+            self.models = [self.model]
+        else:
+            control_hz = int(models[0].control_hz)
+            self.model = models[0]
+            self.models = models
         self.env_config = env_config
         self.updates_per_step = int(physics_hz / control_hz)  # aviary.py:288-289 (single control rate)
         self.step_period = 1.0 / control_hz
@@ -86,6 +104,11 @@ class BatchedAviary:
         _lib.check(L.pfb_create(C.byref(self.model), C.byref(env_config) if env_config is not None else None, self.num_drones, dev_index, self.seed, C.byref(self._h)))
         _lib.check(L.pfb_set_env_offset(self._h, int(env_offset)))
         n, dev = self.num_drones, self.device
+        if len(self.models) > 1:  # drone i flies self.models[model_index[i]]; one table keeps the handle as pfb_create made it
+            tables = (PfbModel * len(models))(*models)
+            idx = np.ascontiguousarray(index, dtype=np.uint8)
+            _lib.check(L.pfb_set_models(self._h, tables, len(models), idx.ctypes.data_as(C.c_void_p)))
+        self.model_index = torch.as_tensor(np.zeros(n, dtype=np.uint8) if index is None else index, dtype=torch.uint8, device=dev)
         f32 = dict(dtype=torch.float32, device=dev)
         self.obs_dim = L.pfb_obs_dim(self._h)
         self.setpoint_dim = L.pfb_setpoint_dim(self._h)

@@ -5,6 +5,7 @@
 #include <cuda_runtime.h>
 
 #include <cstdint>
+#include <type_traits>
 
 #include "../../include/pyflyt_b200.h"
 #include "pfb_fixedwing.cuh"
@@ -26,6 +27,26 @@ struct RngParams {
   uint32_t env_offset_lo; // global id of local env 0 (multi-GPU sharding keeps streams rank-independent)
   uint32_t env_offset_hi;
 };
+
+// ---- mixed-model QuadX handles (pfb_set_models) ------------------------------------------------------------------------
+// The kernels that integrate a QuadX drone take their coefficient table as a template type PS, passed BY VALUE as the
+// __grid_constant__ kernel parameter:
+//   PS = QuadXParams    one table for every env (the only form before mixed models; the K = 1 kernels)
+//   PS = QuadXModelSet  up to PFB_MAX_QUADX_MODELS tables + the per-env model index; env i binds m[index[i]].  The tables
+//                       stay in the parameter constant bank: a lane's table is read with a register-indexed constant load
+// qx_model(ps, i) is env i's table; qx_model0(ps) is table 0, used for the fields that are equal in every table of a set
+// (ratio, dt, noise_loc, wind: pfb_set_models checks physics_hz / control_hz and the kind) so that they stay warp-uniform.
+constexpr int kMaxQuadXModels = PFB_MAX_QUADX_MODELS;
+struct QuadXModelSet {
+  pfb::QuadXParams m[kMaxQuadXModels];
+  const uint8_t* index;  // device [whole tiles * 32]: model of env i (the tile padding reads model 0)
+};
+__device__ __forceinline__ const pfb::QuadXParams& qx_model(const pfb::QuadXParams& p, int64_t) { return p; }
+__device__ __forceinline__ const pfb::QuadXParams& qx_model(const QuadXModelSet& s, int64_t i) { return s.m[s.index[i]]; }
+__device__ __forceinline__ const pfb::QuadXParams& qx_model0(const pfb::QuadXParams& p) { return p; }
+__device__ __forceinline__ const pfb::QuadXParams& qx_model0(const QuadXModelSet& s) { return s.m[0]; }
+template <class PS>
+constexpr bool kUniform = std::is_same<PS, pfb::QuadXParams>::value;
 
 struct PfbContext {
   PfbModel model;
@@ -67,7 +88,24 @@ struct PfbContext {
   cudaEvent_t* prof_ev;   // [2 * prof_cap]
   int prof_cap;
   int prof_n;
+  size_t spare_bytes;     // size of d_spare
+  // mixed-model QuadX handle (pfb_set_models with k > 1): the tables and d_model_index; nullptr = every env flies `qx`
+  QuadXModelSet* qxset;
+  uint8_t* d_model_index;
 };
+
+// Runs BODY with PS = the coefficient-table type of the QuadX kernels and `ps` = the value to pass: the handle's table, or its
+// model set on a mixed-model handle
+#define QX_PARAMS_SWITCH(h, BODY)                                                   \
+  if ((h)->qxset) {                                                                 \
+    using PS = QuadXModelSet;                                                       \
+    const PS& ps = *(h)->qxset;                                                     \
+    BODY;                                                                           \
+  } else {                                                                          \
+    using PS = pfb::QuadXParams;                                                    \
+    const PS& ps = (h)->qx;                                                         \
+    BODY;                                                                           \
+  }
 
 // One warp per CTA: a CTA retires as soon as its own warp is done, so the SM back-fills sooner and the single wave has a
 // shorter tail.  448 threads per SM resident (<= 146 regs/thread) for the generic kernels.  The warp-tiled QuadX-Hover

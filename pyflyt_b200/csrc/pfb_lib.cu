@@ -90,19 +90,20 @@ __global__ void __launch_bounds__(kBlock) k_quadx_set_mode(float* __restrict__ s
 }
 
 // n_steps x Aviary.step() (aviary.py:480-531)
-template <int MODE, bool INJECT, bool TILED>
+template <int MODE, bool INJECT, bool TILED, class PS>
 __global__ void __launch_bounds__(kBlock, kMinBlocks)
-    k_quadx_aviary_step(const __grid_constant__ QuadXParams p, const __grid_constant__ RngParams rng,
+    k_quadx_aviary_step(const __grid_constant__ PS ps, const __grid_constant__ RngParams rng,
                         float* __restrict__ st, int32_t* __restrict__ ist, int rows, const float* __restrict__ setpoint,
                         const float* __restrict__ noise, int n_steps, uint32_t seq, int64_t N) {
   int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= N) return;
+  const QuadXParams& p = qx_model(ps, i);
   QuadXRegs s;
   int step_count;
   qx_load_any<MODE, TILED>(st, ist, rows, N, i, s, step_count);
   float4 sp = __ldg(reinterpret_cast<const float4*>(setpoint) + i);
   s.sp[0] = sp.x; s.sp[1] = sp.y; s.sp[2] = sp.z; s.sp[3] = sp.w;
-  auto nz = make_noise<INJECT>(noise, N, i, rng, seq, TAG_AVIARY, p.noise_loc, p.ratio);
+  auto nz = make_noise<INJECT>(noise, N, i, rng, seq, TAG_AVIARY, qx_model0(ps).noise_loc, qx_model0(ps).ratio);
   for (int k = 0; k < n_steps; ++k) quadx_aviary_step<MODE>(p, s, nz);
   qx_store_any<MODE, TILED>(st, ist, rows, N, i, s, step_count);
 }
@@ -228,7 +229,8 @@ __device__ __forceinline__ void hover_warmup_inline(const QuadXParams& p, QuadXR
 }
 // Out-of-line form for the COLD fallback inside the step role (a spare that cannot be used): everything by value, so the
 // caller's register-resident state never has its address taken.  Slow (the coefficient table is read from the stack copy),
-// and rare.
+// and rare.  A uniform-table kernel must name its __grid_constant__ parameter itself in the call (kUniform below): a copy
+// made through a reference to it makes nvcc stage the whole parameter in local memory first, a second 640-byte stack copy.
 template <int MODE>
 __device__ __noinline__ QuadXRegs hover_warmup_cold(const QuadXParams p, QuadXRegs s, int to, const RngParams rng, int64_t N, int64_t i,
                                                     uint32_t seq) {
@@ -246,9 +248,10 @@ __device__ __forceinline__ QuadXRegs hover_fresh(float px, float py, float pz, f
 
 // Builder CTAs of the step launch (the first 2 * builders CTAs of the grid): the first `builders` of them (phase 0) start the next
 // spare of the envs that are being reset by this launch (done list of the previous launch), the others (phase 1) finish the
-// spares started by the previous launch.  ONE copy of the warm-up loop serves both phases.
-template <int MODE>
-__device__ __forceinline__ void hover_build(const QuadXParams& p, const HoverParams& h, const RngParams& rng, int b, int builders,
+// spares started by the previous launch.  ONE copy of the warm-up loop serves both phases.  Each spare is integrated with the
+// table of the env it belongs to.
+template <int MODE, class PS>
+__device__ __forceinline__ void hover_build(const PS& ps, const HoverParams& h, const RngParams& rng, int b, int builders,
                                             const int32_t* __restrict__ b0_count, const int32_t* __restrict__ b0_list,
                                             const int32_t* __restrict__ b1_count, const int32_t* __restrict__ b1_list,
                                             uint32_t* __restrict__ b0_elist, const uint32_t* __restrict__ b1_elist,
@@ -285,7 +288,7 @@ __device__ __forceinline__ void hover_build(const QuadXParams& p, const HoverPar
       const F4 sp = ld_f4(rec + SP_SETPOINT);
       s.sp[0] = sp.x; s.sp[1] = sp.y; s.sp[2] = sp.z; s.sp[3] = sp.w;
     }
-    hover_warmup_inline<MODE, false>(p, s, phase ? split : 0, phase ? h.warmup_steps : split, rng, nullptr, N, i, e);
+    hover_warmup_inline<MODE, false>(qx_model(ps, i), s, phase ? split : 0, phase ? h.warmup_steps : split, rng, nullptr, N, i, e);
     quadx_store_tile<7, 4>(rec, s, 0);
     if (phase == 0) {
       st_f4(rec + SP_POSE, px, py, pz, ox);
@@ -310,9 +313,9 @@ __device__ __forceinline__ void hover_build(const QuadXParams& p, const HoverPar
 //   RANDACT   actions are drawn on device, uniform in the env's action box (quadx_base_env.py:79-102)
 //   AUTORESET gymnasium NEXT_STEP autoreset: an env that finished on the previous call is reset on this one (its action
 //             is ignored; obs = first observation of the new episode, reward 0, flags cleared)
-template <int MODE, bool INJECT, bool RANDACT, bool AUTORESET, bool MA>
+template <int MODE, bool INJECT, bool RANDACT, bool AUTORESET, bool MA, class PS>
 __global__ void __launch_bounds__(kBlock, kHoverBlocks)
-    k_hover_step(const __grid_constant__ QuadXParams p, const __grid_constant__ HoverParams h,
+    k_hover_step(const __grid_constant__ PS ps, const __grid_constant__ HoverParams h,
                  const __grid_constant__ RngParams rng, float* __restrict__ st, int rows, float* __restrict__ actions,
                  const float* __restrict__ noise, float* __restrict__ obs, float* __restrict__ reward, uint8_t* __restrict__ term,
                  uint8_t* __restrict__ trunc, uint8_t* __restrict__ info, const float* __restrict__ start_pos,
@@ -325,7 +328,7 @@ __global__ void __launch_bounds__(kBlock, kHoverBlocks)
   // dispatched at t = 0, not behind the ~2000 step CTAs
   const int n_build = AUTORESET ? 2 * builders : 0;
   if (AUTORESET && (int)blockIdx.x < n_build) {  // builder CTA (CTA-uniform role)
-    hover_build<MODE>(p, h, rng, (int)blockIdx.x, builders, b0_count, b0_list, b1_count, b1_list, b0_elist, b1_elist, start_pos, start_orn, spare,
+    hover_build<MODE>(ps, h, rng, (int)blockIdx.x, builders, b0_count, b0_list, b1_count, b1_list, b0_elist, b1_elist, start_pos, start_orn, spare,
                       episode, N);
     return;
   }
@@ -336,6 +339,7 @@ __global__ void __launch_bounds__(kBlock, kHoverBlocks)
   const int64_t tile_first = (int64_t)tile * kBlock;
   const int64_t i = tile_first + lane;
   const bool active = i < N;
+  const QuadXParams& p = qx_model(ps, i);  // the model index is padded to whole tiles: every lane may read it
   if (AUTORESET && tile == 0 && lane == 0) *next_count = 0;  // arm the counter the NEXT launch appends to
   float* rec = st + qx_tile_base(i, rows);  // the state tensor is padded to whole tiles: every lane may load
 
@@ -351,7 +355,7 @@ __global__ void __launch_bounds__(kBlock, kHoverBlocks)
   __syncwarp();
   float act[4] = {0.f, 0.f, 0.f, 0.f};
   float past[4] = {0.f, 0.f, 0.f, 0.f};
-  auto nz = make_noise<INJECT>(noise, N, active ? i : 0, rng, step_seq, TAG_ENV_STEP, p.noise_loc, p.ratio);
+  auto nz = make_noise<INJECT>(noise, N, active ? i : 0, rng, step_seq, TAG_ENV_STEP, qx_model0(ps).noise_loc, qx_model0(ps).ratio);
   nz.prefetch4();
   if (!INJECT && noise_dump && active) nz.set_dump(noise_dump + i, N);
   if (RANDACT) {
@@ -454,7 +458,8 @@ __global__ void __launch_bounds__(kBlock, kHoverBlocks)
         }
       }
       if (!hit) {
-        s = hover_warmup_cold<MODE>(p, hover_fresh<MODE>(px, py, pz, ox, oy, oz), h.warmup_steps, rng, N, i, nseq);
+        if constexpr (kUniform<PS>) s = hover_warmup_cold<MODE>(ps, hover_fresh<MODE>(px, py, pz, ox, oy, oz), h.warmup_steps, rng, N, i, nseq);
+        else s = hover_warmup_cold<MODE>(p, hover_fresh<MODE>(px, py, pz, ox, oy, oz), h.warmup_steps, rng, N, i, nseq);
         quadx_requantize(s);  // an inline warm-up must leave exactly what a copied spare holds
       }
 #pragma unroll
@@ -536,13 +541,14 @@ __device__ __forceinline__ void hover_build_full(const QuadXParams& p, const Hov
 }
 // before the first fused launch (or after single-step launches): every env gets the spares episode[i] + 1 .. + kRolloutAhead - 1
 // it does not have yet (episode[i] itself is valid by the step pipeline's invariant)
-template <int MODE>
+template <int MODE, class PS>
 __global__ void __launch_bounds__(kBlock, kHoverBlocks)
-    k_hover_spare_ahead(const __grid_constant__ QuadXParams p, const __grid_constant__ HoverParams h, const __grid_constant__ RngParams rng,
+    k_hover_spare_ahead(const __grid_constant__ PS ps, const __grid_constant__ HoverParams h, const __grid_constant__ RngParams rng,
                         const float* __restrict__ start_pos, const float* __restrict__ start_orn, float* __restrict__ spare,
                         const uint32_t* __restrict__ episode, int64_t N) {
   const int64_t i = (int64_t)blockIdx.x * kBlock + threadIdx.x;
   if (i >= N) return;
+  const QuadXParams& p = qx_model(ps, i);
   const uint32_t e0 = episode[i];
 #pragma unroll 1
   for (int a = 1; a < kRolloutAhead; ++a) {
@@ -555,33 +561,33 @@ __global__ void __launch_bounds__(kBlock, kHoverBlocks)
   }
 }
 // behind a fused launch: the spares it consumed, listed as (env, episode to build)
-template <int MODE>
+template <int MODE, class PS>
 __global__ void __launch_bounds__(kBlock, kHoverBlocks)
-    k_hover_spare_topup(const __grid_constant__ QuadXParams p, const __grid_constant__ HoverParams h, const __grid_constant__ RngParams rng,
+    k_hover_spare_topup(const __grid_constant__ PS ps, const __grid_constant__ HoverParams h, const __grid_constant__ RngParams rng,
                         const float* __restrict__ start_pos, const float* __restrict__ start_orn, float* __restrict__ spare,
                         const int32_t* __restrict__ count, const int2* __restrict__ list, int64_t N) {
   const int n = *count;
   for (int t = (int)(blockIdx.x * kBlock + threadIdx.x); t < n; t += (int)(gridDim.x * kBlock)) {
     const int2 en = list[t];
-    hover_build_full<MODE>(p, h, rng, start_pos, start_orn, spare, N, (int64_t)en.x, (uint32_t)en.y);
+    hover_build_full<MODE>(qx_model(ps, (int64_t)en.x), h, rng, start_pos, start_orn, spare, N, (int64_t)en.x, (uint32_t)en.y);
   }
 }
 // switching from single-step launches to the fused rollout: the spares whose first half was integrated by the last step launch
 // are finished here (phase 1 of hover_build on the list the next step launch would have used), so that episode[] is current
-template <int MODE>
+template <int MODE, class PS>
 __global__ void __launch_bounds__(kBlock, kHoverBlocks)
-    k_hover_drain(const __grid_constant__ QuadXParams p, const __grid_constant__ HoverParams h, const __grid_constant__ RngParams rng,
+    k_hover_drain(const __grid_constant__ PS ps, const __grid_constant__ HoverParams h, const __grid_constant__ RngParams rng,
                   const int32_t* __restrict__ b1_count, const int32_t* __restrict__ b1_list, const uint32_t* __restrict__ b1_elist,
                   const float* __restrict__ start_pos, const float* __restrict__ start_orn, float* __restrict__ spare, uint32_t* __restrict__ episode,
                   int builders, int64_t N) {
-  hover_build<MODE>(p, h, rng, (int)blockIdx.x + builders, builders, b1_count, b1_list, b1_count, b1_list, nullptr, b1_elist, start_pos, start_orn, spare,
+  hover_build<MODE>(ps, h, rng, (int)blockIdx.x + builders, builders, b1_count, b1_list, b1_count, b1_list, nullptr, b1_elist, start_pos, start_orn, spare,
                     episode, N);
 }
 
 // 14 CTAs per SM: the 2048 tiles of a 65 536-env launch (no builder CTAs here) are still one wave, with 144 registers instead of 128
-template <int MODE>
+template <int MODE, class PS>
 __global__ void __launch_bounds__(kBlock, 14)
-    k_hover_rollout(const __grid_constant__ QuadXParams p, const __grid_constant__ HoverParams h, const __grid_constant__ RngParams rng,
+    k_hover_rollout(const __grid_constant__ PS ps, const __grid_constant__ HoverParams h, const __grid_constant__ RngParams rng,
                     float* __restrict__ st, int rows, float* __restrict__ actions, float* __restrict__ obs, float* __restrict__ reward,
                     uint8_t* __restrict__ term, uint8_t* __restrict__ trunc, uint8_t* __restrict__ info, const float* __restrict__ start_pos,
                     const float* __restrict__ start_orn, const float* __restrict__ spare, uint32_t* __restrict__ episode,
@@ -597,6 +603,7 @@ __global__ void __launch_bounds__(kBlock, 14)
   const int64_t tile_first = (int64_t)tile * kBlock;
   const int64_t i = tile_first + lane;
   const bool active = i < N;
+  const QuadXParams& p = qx_model(ps, i);  // the model index is padded to whole tiles: every lane may read it
   float* rec = st + qx_tile_base(i, rows);
   if (lane == 0) {
     mbar_init(&mbar, 1);
@@ -624,7 +631,7 @@ __global__ void __launch_bounds__(kBlock, 14)
   for (int t = 0; t < T; ++t) {
     const uint32_t step_seq = step_seq0 + (uint32_t)t;
     // ---- the step's draws: motor noise and the action, same counters as a single-step launch
-    auto nz = make_noise<false>(nullptr, N, active ? i : 0, rng, step_seq, TAG_ENV_STEP, p.noise_loc, p.ratio);
+    auto nz = make_noise<false>(nullptr, N, active ? i : 0, rng, step_seq, TAG_ENV_STEP, qx_model0(ps).noise_loc, qx_model0(ps).ratio);
     nz.prefetch4();
     float act[4];
     {
@@ -688,7 +695,8 @@ __global__ void __launch_bounds__(kBlock, 14)
           s.pwm[0] = pw.x; s.pwm[1] = pw.y; s.pwm[2] = pw.z; s.pwm[3] = pw.w;
           s.flags = bits_from_f(m1.w);
         } else {
-          s = hover_warmup_cold<MODE>(p, hover_fresh<MODE>(sx, sy, sz, ox, oy, oz), h.warmup_steps, rng, N, i, e_local);
+          if constexpr (kUniform<PS>) s = hover_warmup_cold<MODE>(ps, hover_fresh<MODE>(sx, sy, sz, ox, oy, oz), h.warmup_steps, rng, N, i, e_local);
+          else s = hover_warmup_cold<MODE>(p, hover_fresh<MODE>(sx, sy, sz, ox, oy, oz), h.warmup_steps, rng, N, i, e_local);
           quadx_requantize(s);
         }
 #pragma unroll
@@ -740,13 +748,14 @@ __global__ void __launch_bounds__(kBlock, 14)
 }
 
 // After a user reset of every env: each env gets a complete fresh spare (dense warps, all envs).
-template <int MODE>
+template <int MODE, class PS>
 __global__ void __launch_bounds__(kBlock, kHoverBlocks)
-    k_hover_spare_build(const __grid_constant__ QuadXParams p, const __grid_constant__ HoverParams h, const __grid_constant__ RngParams rng,
+    k_hover_spare_build(const __grid_constant__ PS ps, const __grid_constant__ HoverParams h, const __grid_constant__ RngParams rng,
                         const float* __restrict__ start_pos, const float* __restrict__ start_orn, float* __restrict__ spare,
                         uint32_t* __restrict__ episode, int64_t N) {
   const int64_t i = (int64_t)blockIdx.x * kBlock + threadIdx.x;
   if (i >= N) return;
+  const QuadXParams& p = qx_model(ps, i);
   const uint32_t e = episode[i] + 1u;
   float* rec = spare + ((int64_t)(e & kSpareMask) * N + i) * SP_ROWS;
   const float px = start_pos[3 * i + 0], py = start_pos[3 * i + 1], pz = start_pos[3 * i + 2];
@@ -761,9 +770,9 @@ __global__ void __launch_bounds__(kBlock, kHoverBlocks)
 }
 
 // env.reset() for all / masked envs
-template <int MODE, bool INJECT>
+template <int MODE, bool INJECT, class PS>
 __global__ void __launch_bounds__(kBlock)
-    k_hover_reset(const __grid_constant__ QuadXParams p, const __grid_constant__ HoverParams h,
+    k_hover_reset(const __grid_constant__ PS ps, const __grid_constant__ HoverParams h,
                   const __grid_constant__ RngParams rng, float* __restrict__ st, int rows,
                   const float* __restrict__ start_pos, const float* __restrict__ start_orn,
                   const uint8_t* __restrict__ mask, const float* __restrict__ noise, float* __restrict__ obs,
@@ -771,6 +780,7 @@ __global__ void __launch_bounds__(kBlock)
   const int64_t i = (int64_t)blockIdx.x * kBlock + threadIdx.x;
   if (i >= N) return;
   if (mask && !mask[i]) return;
+  const QuadXParams& p = qx_model(ps, i);
   const int O = (h.angle_representation == 0 ? 20 : 21) + (h.ma ? 3 : 0);
   float row[kObsMax];
   QuadXRegs s = hover_fresh<MODE>(start_pos[3 * i + 0], start_pos[3 * i + 1], start_pos[3 * i + 2], start_orn[3 * i + 0], start_orn[3 * i + 1],
@@ -937,8 +947,9 @@ int pfb_create(const PfbModel* model, const PfbEnvConfig* env, int64_t n_envs, i
     const bool hover = env->env_kind == PFB_ENV_QUADX_HOVER;
     const size_t rec = env->env_kind == PFB_ENV_QUADX_WAYPOINTS ? (size_t)qwp_spare_rows()
                        : (env->env_kind == PFB_ENV_DOGFIGHT ? (size_t)df_spare_rows() : (size_t)SP_ROWS * (hover ? kSpareBufs : 1));
-    CUDA_OK(cudaMalloc(&c->d_spare, rec * (size_t)n_envs * sizeof(float)));
-    CUDA_OK(cudaMemset(c->d_spare, 0, rec * (size_t)n_envs * sizeof(float)));
+    c->spare_bytes = rec * (size_t)n_envs * sizeof(float);
+    CUDA_OK(cudaMalloc(&c->d_spare, c->spare_bytes));
+    CUDA_OK(cudaMemset(c->d_spare, 0, c->spare_bytes));
     if (hover) {
       CUDA_OK(cudaMalloc(&c->d_consumed, (size_t)(kRolloutMaxSteps / 2 + 1) * (size_t)n_envs * sizeof(int2)));  // (env, episode) per reset of a fused launch
       CUDA_OK(cudaMalloc(&c->d_elist, 4 * (size_t)n_envs * sizeof(uint32_t)));
@@ -974,6 +985,8 @@ int pfb_destroy(PfbHandle h) {
   }
   cudaFree(h->d_counters);
   cudaFree(h->d_done_list);
+  if (h->d_model_index) cudaFree(h->d_model_index);
+  delete h->qxset;
   if (h->prof_ev) {
     for (int i = 0; i < 2 * h->prof_cap; ++i) cudaEventDestroy(h->prof_ev[i]);
     delete[] h->prof_ev;
@@ -1057,14 +1070,14 @@ int pfb_aviary_step(PfbHandle h, int n_steps, const float* noise, void* stream) 
   if (is_rk(h)) return rk_aviary_step(h, n_steps, noise, s);
   const int mode = h->mode;
   const uint32_t seq = (uint32_t)h->aviary_seq++;
-#define AV_ARGS h->qx, h->rng, h->buf.state, h->buf.istate, qx_rows(h), h->buf.setpoint, noise, n_steps, seq, h->n
+#define AV_ARGS ps, h->rng, h->buf.state, h->buf.istate, qx_rows(h), h->buf.setpoint, noise, n_steps, seq, h->n
   const int g = grid_for(h->n);
   if (is_tiled(h)) {
-    if (noise) { PFB_MODE_SWITCH(mode, (k_quadx_aviary_step<MODE, true, true><<<g, kBlock, 0, s>>>(AV_ARGS))); }
-    else { PFB_MODE_SWITCH(mode, (k_quadx_aviary_step<MODE, false, true><<<g, kBlock, 0, s>>>(AV_ARGS))); }
+    if (noise) { QX_PARAMS_SWITCH(h, PFB_MODE_SWITCH(mode, (k_quadx_aviary_step<MODE, true, true, PS><<<g, kBlock, 0, s>>>(AV_ARGS)))); }
+    else { QX_PARAMS_SWITCH(h, PFB_MODE_SWITCH(mode, (k_quadx_aviary_step<MODE, false, true, PS><<<g, kBlock, 0, s>>>(AV_ARGS)))); }
   } else {
-    if (noise) { PFB_MODE_SWITCH(mode, (k_quadx_aviary_step<MODE, true, false><<<g, kBlock, 0, s>>>(AV_ARGS))); }
-    else { PFB_MODE_SWITCH(mode, (k_quadx_aviary_step<MODE, false, false><<<g, kBlock, 0, s>>>(AV_ARGS))); }
+    if (noise) { QX_PARAMS_SWITCH(h, PFB_MODE_SWITCH(mode, (k_quadx_aviary_step<MODE, true, false, PS><<<g, kBlock, 0, s>>>(AV_ARGS)))); }
+    else { QX_PARAMS_SWITCH(h, PFB_MODE_SWITCH(mode, (k_quadx_aviary_step<MODE, false, false, PS><<<g, kBlock, 0, s>>>(AV_ARGS)))); }
   }
 #undef AV_ARGS
   LAUNCH_CHECK(h);
@@ -1107,15 +1120,15 @@ int pfb_env_reset(PfbHandle h, const uint8_t* mask, const float* noise, void* st
   // resets draw from their own Philox stream; the high bit keeps them apart from in-step autoresets
   const uint32_t seq = 0x80000000u | (uint32_t)h->reset_seq++;
   if (h->d_spare && !mask) CUDA_OK(cudaMemsetAsync(h->d_counters, 0, 4 * sizeof(int32_t), s));  // a full reset empties the rebuild queues
-#define HR_ARGS h->qx, h->hover, h->rng, h->buf.state, qx_rows(h), h->buf.start_pos, h->buf.start_orn, mask, noise, h->buf.obs, seq, h->n
-  if (noise) { PFB_MODE_SWITCH(mode, (k_hover_reset<MODE, true><<<grid_for(h->n), kBlock, 0, s>>>(HR_ARGS))); }
-  else { PFB_MODE_SWITCH(mode, (k_hover_reset<MODE, false><<<grid_for(h->n), kBlock, 0, s>>>(HR_ARGS))); }
+#define HR_ARGS ps, h->hover, h->rng, h->buf.state, qx_rows(h), h->buf.start_pos, h->buf.start_orn, mask, noise, h->buf.obs, seq, h->n
+  if (noise) { QX_PARAMS_SWITCH(h, PFB_MODE_SWITCH(mode, (k_hover_reset<MODE, true, PS><<<grid_for(h->n), kBlock, 0, s>>>(HR_ARGS)))); }
+  else { QX_PARAMS_SWITCH(h, PFB_MODE_SWITCH(mode, (k_hover_reset<MODE, false, PS><<<grid_for(h->n), kBlock, 0, s>>>(HR_ARGS)))); }
 #undef HR_ARGS
   LAUNCH_CHECK(h);
   if (h->d_spare && !mask) {  // every env gets a fresh spare.  A masked reset keeps the spares: they are keyed by (env, episode
                               // number) and stay valid; a masked env simply is not `done` on the next step
-    PFB_MODE_SWITCH(mode, (k_hover_spare_build<MODE><<<grid_for(h->n), kBlock, 0, s>>>(h->qx, h->hover, h->rng, h->buf.start_pos, h->buf.start_orn,
-                                                                                      h->d_spare, h->d_episode, h->n)));
+    QX_PARAMS_SWITCH(h, PFB_MODE_SWITCH(mode, (k_hover_spare_build<MODE, PS><<<grid_for(h->n), kBlock, 0, s>>>(ps, h->hover, h->rng, h->buf.start_pos,
+                                                                                                              h->buf.start_orn, h->d_spare, h->d_episode, h->n))));
     LAUNCH_CHECK(h);
   }
   h->mode = mode;
@@ -1151,27 +1164,28 @@ static int env_step_impl(PfbHandle h, float* actions, const float* noise, bool r
   const int grid = tiles + 2 * builders;
   const bool prof = h->prof_ev && h->prof_n < h->prof_cap;
   if (prof) CUDA_OK(cudaEventRecord(h->prof_ev[2 * h->prof_n], s));
-#define STEP_ARGS h->qx, h->hover, h->rng, h->buf.state, qx_rows(h), actions, noise, h->buf.obs, h->buf.reward, h->buf.term, h->buf.trunc,    \
+#define STEP_ARGS ps, h->hover, h->rng, h->buf.state, qx_rows(h), actions, noise, h->buf.obs, h->buf.reward, h->buf.term, h->buf.trunc,       \
                   h->buf.info, h->buf.start_pos, h->buf.start_orn, cnt_cur, list_cur, cnt_next, cnt_b0, list_b0, cnt_b1, list_b1, elist_b0,   \
                   elist_b1, h->d_spare, h->d_episode, spare_copy, builders, h->noise_dump, seq, h->n
   if (autoreset) {
     if (noise) return fail("injected noise (parity mode) is only supported with autoreset = 0");
     if (randact) {
-      PFB_MODE_SWITCH(mode, (k_hover_step<MODE, false, true, true, false><<<grid, kBlock, dyn_smem, s>>>(STEP_ARGS)));
+      QX_PARAMS_SWITCH(h, PFB_MODE_SWITCH(mode, (k_hover_step<MODE, false, true, true, false, PS><<<grid, kBlock, dyn_smem, s>>>(STEP_ARGS))));
     } else {
-      PFB_MODE_SWITCH(mode, (k_hover_step<MODE, false, false, true, false><<<grid, kBlock, dyn_smem, s>>>(STEP_ARGS)));
+      QX_PARAMS_SWITCH(h, PFB_MODE_SWITCH(mode, (k_hover_step<MODE, false, false, true, false, PS><<<grid, kBlock, dyn_smem, s>>>(STEP_ARGS))));
     }
-  } else if (h->hover.ma) {
+  } else if (h->hover.ma) {  // one vehicle table (pfb_set_models refuses MAQuadXHover handles)
     if (randact) return fail("MAQuadXHover has no on-device action generator");
-    if (noise) { PFB_MODE_SWITCH(mode, (k_hover_step<MODE, true, false, false, true><<<grid, kBlock, dyn_smem, s>>>(STEP_ARGS))); }
-    else { PFB_MODE_SWITCH(mode, (k_hover_step<MODE, false, false, false, true><<<grid, kBlock, dyn_smem, s>>>(STEP_ARGS))); }
+    const QuadXParams& ps = h->qx;
+    if (noise) { PFB_MODE_SWITCH(mode, (k_hover_step<MODE, true, false, false, true, QuadXParams><<<grid, kBlock, dyn_smem, s>>>(STEP_ARGS))); }
+    else { PFB_MODE_SWITCH(mode, (k_hover_step<MODE, false, false, false, true, QuadXParams><<<grid, kBlock, dyn_smem, s>>>(STEP_ARGS))); }
   } else {
     if (noise) {
-      PFB_MODE_SWITCH(mode, (k_hover_step<MODE, true, false, false, false><<<grid, kBlock, dyn_smem, s>>>(STEP_ARGS)));
+      QX_PARAMS_SWITCH(h, PFB_MODE_SWITCH(mode, (k_hover_step<MODE, true, false, false, false, PS><<<grid, kBlock, dyn_smem, s>>>(STEP_ARGS))));
     } else if (randact) {
-      PFB_MODE_SWITCH(mode, (k_hover_step<MODE, false, true, false, false><<<grid, kBlock, dyn_smem, s>>>(STEP_ARGS)));
+      QX_PARAMS_SWITCH(h, PFB_MODE_SWITCH(mode, (k_hover_step<MODE, false, true, false, false, PS><<<grid, kBlock, dyn_smem, s>>>(STEP_ARGS))));
     } else {
-      PFB_MODE_SWITCH(mode, (k_hover_step<MODE, false, false, false, false><<<grid, kBlock, dyn_smem, s>>>(STEP_ARGS)));
+      QX_PARAMS_SWITCH(h, PFB_MODE_SWITCH(mode, (k_hover_step<MODE, false, false, false, false, PS><<<grid, kBlock, dyn_smem, s>>>(STEP_ARGS))));
     }
   }
 #undef STEP_ARGS
@@ -1206,8 +1220,69 @@ int pfb_set_wind(PfbHandle h, const PfbWind* wind) {
     }
   }
   h->qx.wind = w;
+  if (h->qxset)
+    for (int j = 0; j < kMaxQuadXModels; ++j) h->qxset->m[j].wind = w;
   h->fw.wind = w;
   h->rk.wind = w;
+  return 0;
+}
+
+int pfb_set_models(PfbHandle h, const PfbModel* models, int k, const uint8_t* index_host) {
+  if (!h || !models || !index_host) return fail("pfb_set_models: null argument");
+  if (h->model.kind != PFB_KIND_QUADX) return fail("pfb_set_models: only QuadX handles fly several vehicle models");
+  if (is_ma(h)) return fail("pfb_set_models: MAQuadXHover handles fly one vehicle model");
+  if (k < 1 || k > PFB_MAX_QUADX_MODELS) return fail("pfb_set_models: k = %d, must be in 1..%d", k, PFB_MAX_QUADX_MODELS);
+  QuadXParams tables[PFB_MAX_QUADX_MODELS];
+  for (int j = 0; j < k; ++j) {
+    const PfbModel& m = models[j];
+    if (m.abi_version != PFB_ABI_VERSION) return fail("pfb_set_models: model %d has ABI %d != library ABI %d", j, m.abi_version, PFB_ABI_VERSION);
+    if (m.kind != PFB_KIND_QUADX) return fail("pfb_set_models: model %d is not a QuadX (kind %d)", j, m.kind);
+    // every kernel runs ONE substep ratio and one dt per handle
+    if (m.physics_hz != models[0].physics_hz || m.control_hz != models[0].control_hz)
+      return fail("pfb_set_models: model %d runs at physics_hz %g / control_hz %g, model 0 at %g / %g: every model of a handle needs the same rates", j,
+                  m.physics_hz, m.control_hz, models[0].physics_hz, models[0].control_hz);
+    memset(&tables[j], 0, sizeof(QuadXParams));
+    if (build_quadx_params(m, tables[j]) != 0) return -1;
+    if (tables[j].ratio != tables[0].ratio || tables[j].dt != tables[0].dt || tables[j].ctrl_dt != tables[0].ctrl_dt ||
+        tables[j].noise_loc != tables[0].noise_loc)
+      return fail("pfb_set_models: model %d has a different substep ratio, dt or motor count than model 0", j);
+  }
+  for (int64_t i = 0; i < h->n; ++i)
+    if (index_host[i] >= k) return fail("pfb_set_models: index[%lld] = %d, must be < k = %d", (long long)i, (int)index_host[i], k);
+  CUDA_OK(cudaSetDevice(h->device));
+  // The spare post-reset states were integrated with the previous tables: nothing may still be building them, and every record
+  // is marked invalid (a reset then integrates its warm-up inline until pfb_env_reset rebuilds them).  QuadX-Hover's builder
+  // queues are emptied as a full reset does; QuadX-Waypoints keeps its done list, which its tail CTAs reset the envs from.
+  if (h->side) CUDA_OK(cudaStreamSynchronize(h->side));
+  CUDA_OK(cudaDeviceSynchronize());
+  if (h->d_spare) CUDA_OK(cudaMemset(h->d_spare, 0, h->spare_bytes));
+  if (h->d_episode) CUDA_OK(cudaMemset(h->d_counters, 0, 4 * sizeof(int32_t)));
+  h->fused_ready = 0;
+  const WindParams wind = h->qx.wind;
+  h->model = models[0];
+  h->qx = tables[0];
+  h->qx.wind = wind;
+  if (k == 1) {  // uniform again: the handle runs the single-table kernels
+    if (h->d_model_index) CUDA_OK(cudaFree(h->d_model_index));
+    h->d_model_index = nullptr;
+    delete h->qxset;
+    h->qxset = nullptr;
+    return 0;
+  }
+  if (!h->qxset) {
+    h->qxset = new (std::nothrow) QuadXModelSet();
+    if (!h->qxset) return fail("out of host memory");
+  }
+  memset(h->qxset, 0, sizeof(QuadXModelSet));
+  for (int j = 0; j < k; ++j) {
+    h->qxset->m[j] = tables[j];
+    h->qxset->m[j].wind = wind;
+  }
+  const size_t padded = (size_t)grid_for(h->n) * kBlock;  // whole tiles: the tile kernels read the index of every lane
+  if (!h->d_model_index) CUDA_OK(cudaMalloc(&h->d_model_index, padded));
+  CUDA_OK(cudaMemset(h->d_model_index, 0, padded));
+  CUDA_OK(cudaMemcpy(h->d_model_index, index_host, (size_t)h->n, cudaMemcpyHostToDevice));
+  h->qxset->index = h->d_model_index;
   return 0;
 }
 
@@ -1254,13 +1329,14 @@ static int hover_rollout_fused(PfbHandle h, int n_steps, cudaStream_t s) {
     const uint64_t k = h->step_seq;
     const int builders = h->sm_count < tiles ? h->sm_count : tiles;
     if (k >= 2) {
-      PFB_MODE_SWITCH(mode, (k_hover_drain<MODE><<<builders, kBlock, 0, s>>>(h->qx, h->hover, h->rng, h->d_counters + ((k + 2) % 4),
-                                                                            h->d_done_list + ((k + 2) % 4) * h->n, h->d_elist + ((k + 2) % 4) * h->n,
-                                                                            h->buf.start_pos, h->buf.start_orn, h->d_spare, h->d_episode, builders, h->n)));
+      QX_PARAMS_SWITCH(h, PFB_MODE_SWITCH(mode, (k_hover_drain<MODE, PS><<<builders, kBlock, 0, s>>>(
+                                                     ps, h->hover, h->rng, h->d_counters + ((k + 2) % 4), h->d_done_list + ((k + 2) % 4) * h->n,
+                                                     h->d_elist + ((k + 2) % 4) * h->n, h->buf.start_pos, h->buf.start_orn, h->d_spare, h->d_episode,
+                                                     builders, h->n))));
       LAUNCH_CHECK(h);
     }
-    PFB_MODE_SWITCH(mode, (k_hover_spare_ahead<MODE><<<tiles, kBlock, 0, s>>>(h->qx, h->hover, h->rng, h->buf.start_pos, h->buf.start_orn, h->d_spare,
-                                                                              h->d_episode, h->n)));
+    QX_PARAMS_SWITCH(h, PFB_MODE_SWITCH(mode, (k_hover_spare_ahead<MODE, PS><<<tiles, kBlock, 0, s>>>(ps, h->hover, h->rng, h->buf.start_pos, h->buf.start_orn,
+                                                                                                      h->d_spare, h->d_episode, h->n))));
     LAUNCH_CHECK(h);
     h->fused_ready = 1;
   }
@@ -1270,13 +1346,14 @@ static int hover_rollout_fused(PfbHandle h, int n_steps, cudaStream_t s) {
     const int T = n_steps < kRolloutMaxSteps ? n_steps : kRolloutMaxSteps;
     const uint64_t k0 = h->step_seq, k_last = k0 + (uint64_t)T - 1;
     CUDA_OK(cudaMemsetAsync(h->d_counters, 0, 8 * sizeof(int32_t), s));  // [0..3] step pipeline lists, [5] spares consumed by this launch
-    PFB_MODE_SWITCH(mode, (k_hover_rollout<MODE><<<tiles, kBlock, 0, s>>>(
-                              h->qx, h->hover, h->rng, h->buf.state, qx_rows(h), h->buf.setpoint, h->buf.obs, h->buf.reward, h->buf.term, h->buf.trunc,
-                              h->buf.info, h->buf.start_pos, h->buf.start_orn, h->d_spare, h->d_episode, h->d_counters + 5, h->d_consumed,
-                              h->d_counters + (k_last % 4), h->d_done_list + (k_last % 4) * h->n, (uint32_t)k0, T, h->n)));
+    QX_PARAMS_SWITCH(h, PFB_MODE_SWITCH(mode, (k_hover_rollout<MODE, PS><<<tiles, kBlock, 0, s>>>(
+                                                   ps, h->hover, h->rng, h->buf.state, qx_rows(h), h->buf.setpoint, h->buf.obs, h->buf.reward, h->buf.term,
+                                                   h->buf.trunc, h->buf.info, h->buf.start_pos, h->buf.start_orn, h->d_spare, h->d_episode, h->d_counters + 5,
+                                                   h->d_consumed, h->d_counters + (k_last % 4), h->d_done_list + (k_last % 4) * h->n, (uint32_t)k0, T, h->n))));
     LAUNCH_CHECK(h);
-    PFB_MODE_SWITCH(mode, (k_hover_spare_topup<MODE><<<topup_grid, kBlock, 0, s>>>(h->qx, h->hover, h->rng, h->buf.start_pos, h->buf.start_orn, h->d_spare,
-                                                                                   h->d_counters + 5, h->d_consumed, h->n)));
+    QX_PARAMS_SWITCH(h, PFB_MODE_SWITCH(mode, (k_hover_spare_topup<MODE, PS><<<topup_grid, kBlock, 0, s>>>(ps, h->hover, h->rng, h->buf.start_pos,
+                                                                                                           h->buf.start_orn, h->d_spare, h->d_counters + 5,
+                                                                                                           h->d_consumed, h->n))));
     LAUNCH_CHECK(h);
     h->step_seq += (uint64_t)T;
     n_steps -= T;

@@ -163,9 +163,9 @@ enum { QSP_POSE = QW_ROWS, QSP_VALID = QW_ROWS + 6, QSP_FLAGS = QW_ROWS + 7, QSP
 static_assert(QW_ROWS + 9 <= QSP_ROWS, "spare record too small");
 int qwp_spare_rows() { return QSP_ROWS; }
 
-template <int MODE, bool INJECT, bool RANDACT, bool AUTORESET>
+template <int MODE, bool INJECT, bool RANDACT, bool AUTORESET, class PS>
 __global__ void __launch_bounds__(kBlock, kMinBlocks)
-    k_qxwp_step(const __grid_constant__ QuadXParams p, const __grid_constant__ HoverParams h, const __grid_constant__ QxWaypointParams w,
+    k_qxwp_step(const __grid_constant__ PS ps, const __grid_constant__ HoverParams h, const __grid_constant__ QxWaypointParams w,
                 const __grid_constant__ RngParams rng, float* __restrict__ st, int32_t* __restrict__ ist, float* __restrict__ actions,
                 const float* __restrict__ noise, float* __restrict__ obs, float* __restrict__ reward, uint8_t* __restrict__ term,
                 uint8_t* __restrict__ trunc, uint8_t* __restrict__ info, const float* __restrict__ start_pos,
@@ -193,6 +193,7 @@ __global__ void __launch_bounds__(kBlock, kMinBlocks)
 #pragma unroll 1
   for (; t < t_end; t += t_stride) {
     const int64_t i = tail ? (prev_list ? (int64_t)prev_list[t] : (int64_t)t) : block_first + threadIdx.x;
+    const QuadXParams& p = qx_model(ps, i);
     QuadXRegs s;
     QwState wp;
     float act[4] = {0.f, 0.f, 0.f, 0.f};
@@ -274,7 +275,7 @@ __global__ void __launch_bounds__(kBlock, kMinBlocks)
       wp.yaw_err = st[(int64_t)QW_YAWERR * N + i];
       if (wp.first < w.num_targets) qw_load_target0(tb, ts, wp);
       rew = -0.1f;
-      auto nz = make_noise<INJECT>(noise, N, i, rng, step_seq, TAG_ENV_STEP, p.noise_loc, p.ratio);
+      auto nz = make_noise<INJECT>(noise, N, i, rng, step_seq, TAG_ENV_STEP, qx_model0(ps).noise_loc, qx_model0(ps).ratio);
 #pragma unroll 1
       for (int k = 0; k < w.env_step_ratio; ++k) {
         if (s.flags & (FLAG_TERM | FLAG_TRUNC)) break;
@@ -332,9 +333,9 @@ __global__ void __launch_bounds__(kBlock, kMinBlocks)
   }
 }
 
-template <int MODE, bool INJECT>
+template <int MODE, bool INJECT, class PS>
 __global__ void __launch_bounds__(kBlock)
-    k_qxwp_reset(const __grid_constant__ QuadXParams p, const __grid_constant__ HoverParams h, const __grid_constant__ QxWaypointParams w,
+    k_qxwp_reset(const __grid_constant__ PS ps, const __grid_constant__ HoverParams h, const __grid_constant__ QxWaypointParams w,
                  const __grid_constant__ RngParams rng, float* __restrict__ st, int32_t* __restrict__ ist,
                  const float* __restrict__ start_pos, const float* __restrict__ start_orn, const float* __restrict__ reset_targets,
                  const uint8_t* __restrict__ mask, const float* __restrict__ noise, float* __restrict__ obs, uint32_t seq, int64_t N) {
@@ -342,6 +343,7 @@ __global__ void __launch_bounds__(kBlock)
   const int64_t i = (int64_t)blockIdx.x * kBlock + threadIdx.x;
   if (i >= N) return;
   if (mask && !mask[i]) return;
+  const QuadXParams& p = qx_model(ps, i);
   const int O = (h.angle_representation == 0 ? 20 : 21) + (w.use_yaw_targets ? 4 : 3) * w.num_targets;
   QuadXRegs s;
   QwState wp;
@@ -386,17 +388,17 @@ int qwp_env_reset(PfbContext* h, const uint8_t* mask, const float* noise, cudaSt
     if (!mask) CUDA_OK(cudaMemsetAsync(h->d_counters, 0, 4 * sizeof(int32_t), s));  // a full reset empties the autoreset queues
     else if (pfb_drop_masked_done(h, mask, s)) return -1;  // a masked one takes its envs out of the pending done list
   }
-#define QR_ARGS h->qx, h->hover, h->qwp, h->rng, h->buf.state, h->buf.istate, h->buf.start_pos, h->buf.start_orn, h->buf.reset_targets, mask, noise, \
+#define QR_ARGS ps, h->hover, h->qwp, h->rng, h->buf.state, h->buf.istate, h->buf.start_pos, h->buf.start_orn, h->buf.reset_targets, mask, noise, \
                 h->buf.obs, seq, h->n
-  if (noise) { QW_MODE_SWITCH(mode, (k_qxwp_reset<MODE, true><<<g, kBlock, 0, s>>>(QR_ARGS))); }
-  else { QW_MODE_SWITCH(mode, (k_qxwp_reset<MODE, false><<<g, kBlock, 0, s>>>(QR_ARGS))); }
+  if (noise) { QX_PARAMS_SWITCH(h, QW_MODE_SWITCH(mode, (k_qxwp_reset<MODE, true, PS><<<g, kBlock, 0, s>>>(QR_ARGS)))); }
+  else { QX_PARAMS_SWITCH(h, QW_MODE_SWITCH(mode, (k_qxwp_reset<MODE, false, PS><<<g, kBlock, 0, s>>>(QR_ARGS)))); }
 #undef QR_ARGS
   LAUNCH_CHECK(h);
   if (spare) {  // every env gets a fresh spare: the step kernel in build mode over all envs, same stream
-    QW_MODE_SWITCH(mode, (k_qxwp_step<MODE, false, false, true><<<g, kBlock, 0, s>>>(
-                             h->qx, h->hover, h->qwp, h->rng, h->buf.state, h->buf.istate, h->buf.setpoint, nullptr, h->buf.obs, h->buf.reward,
-                             h->buf.term, h->buf.trunc, h->buf.info, h->buf.start_pos, h->buf.start_orn, nullptr, nullptr, nullptr, nullptr,
-                             nullptr, spare, 0, 1, g, 0u, h->n)));
+    QX_PARAMS_SWITCH(h, QW_MODE_SWITCH(mode, (k_qxwp_step<MODE, false, false, true, PS><<<g, kBlock, 0, s>>>(
+                                                  ps, h->hover, h->qwp, h->rng, h->buf.state, h->buf.istate, h->buf.setpoint, nullptr, h->buf.obs,
+                                                  h->buf.reward, h->buf.term, h->buf.trunc, h->buf.info, h->buf.start_pos, h->buf.start_orn, nullptr,
+                                                  nullptr, nullptr, nullptr, nullptr, spare, 0, 1, g, 0u, h->n))));
     LAUNCH_CHECK(h);
   }
   h->mode = mode;
@@ -410,17 +412,17 @@ int qwp_env_step(PfbContext* h, float* actions, const float* noise, bool randact
   const int spare_copy = (spare && !h->env.inline_reset) ? 1 : 0;
   SPARE_BEFORE_STEP(h, s);
   if (pl.prof) CUDA_OK(cudaEventRecord(h->prof_ev[2 * h->prof_n], s));
-#define QS_ARGS h->qx, h->hover, h->qwp, h->rng, h->buf.state, h->buf.istate, actions, noise, h->buf.obs, h->buf.reward, h->buf.term,     \
+#define QS_ARGS ps, h->hover, h->qwp, h->rng, h->buf.state, h->buf.istate, actions, noise, h->buf.obs, h->buf.reward, h->buf.term,     \
                 h->buf.trunc, h->buf.info, h->buf.start_pos, h->buf.start_orn, pl.cnt_prev, pl.list_prev, pl.cnt_cur, pl.list_cur, \
                 pl.cnt_next, spare, spare_copy, 0, pl.tail, pl.seq, h->n
   if (h->env.autoreset) {
     if (noise) return fail("injected noise (parity mode) is only supported with autoreset = 0");
-    if (randact) { QW_MODE_SWITCH(mode, (k_qxwp_step<MODE, false, true, true><<<pl.grid, kBlock, 0, s>>>(QS_ARGS))); }
-    else { QW_MODE_SWITCH(mode, (k_qxwp_step<MODE, false, false, true><<<pl.grid, kBlock, 0, s>>>(QS_ARGS))); }
+    if (randact) { QX_PARAMS_SWITCH(h, QW_MODE_SWITCH(mode, (k_qxwp_step<MODE, false, true, true, PS><<<pl.grid, kBlock, 0, s>>>(QS_ARGS)))); }
+    else { QX_PARAMS_SWITCH(h, QW_MODE_SWITCH(mode, (k_qxwp_step<MODE, false, false, true, PS><<<pl.grid, kBlock, 0, s>>>(QS_ARGS)))); }
   } else {
-    if (noise) { QW_MODE_SWITCH(mode, (k_qxwp_step<MODE, true, false, false><<<pl.grid, kBlock, 0, s>>>(QS_ARGS))); }
-    else if (randact) { QW_MODE_SWITCH(mode, (k_qxwp_step<MODE, false, true, false><<<pl.grid, kBlock, 0, s>>>(QS_ARGS))); }
-    else { QW_MODE_SWITCH(mode, (k_qxwp_step<MODE, false, false, false><<<pl.grid, kBlock, 0, s>>>(QS_ARGS))); }
+    if (noise) { QX_PARAMS_SWITCH(h, QW_MODE_SWITCH(mode, (k_qxwp_step<MODE, true, false, false, PS><<<pl.grid, kBlock, 0, s>>>(QS_ARGS)))); }
+    else if (randact) { QX_PARAMS_SWITCH(h, QW_MODE_SWITCH(mode, (k_qxwp_step<MODE, false, true, false, PS><<<pl.grid, kBlock, 0, s>>>(QS_ARGS)))); }
+    else { QX_PARAMS_SWITCH(h, QW_MODE_SWITCH(mode, (k_qxwp_step<MODE, false, false, false, PS><<<pl.grid, kBlock, 0, s>>>(QS_ARGS)))); }
   }
 #undef QS_ARGS
   LAUNCH_CHECK(h);
@@ -430,10 +432,10 @@ int qwp_env_step(PfbContext* h, float* actions, const float* noise, bool randact
   }
   if (spare) {  // rebuild the spares this launch consumed, on the side stream, while the next launches run
     SPARE_REBUILD_BEGIN(h, s);
-    QW_MODE_SWITCH(mode, (k_qxwp_step<MODE, false, false, true><<<h->sm_count, kBlock, 0, h->side>>>(
-                             h->qx, h->hover, h->qwp, h->rng, h->buf.state, h->buf.istate, actions, nullptr, h->buf.obs, h->buf.reward, h->buf.term,
-                             h->buf.trunc, h->buf.info, h->buf.start_pos, h->buf.start_orn, pl.cnt_prev, pl.list_prev, pl.cnt_cur, pl.list_cur,
-                             pl.cnt_next, spare, 0, 1, h->sm_count, pl.seq, h->n)));
+    QX_PARAMS_SWITCH(h, QW_MODE_SWITCH(mode, (k_qxwp_step<MODE, false, false, true, PS><<<h->sm_count, kBlock, 0, h->side>>>(
+                                                  ps, h->hover, h->qwp, h->rng, h->buf.state, h->buf.istate, actions, nullptr, h->buf.obs, h->buf.reward,
+                                                  h->buf.term, h->buf.trunc, h->buf.info, h->buf.start_pos, h->buf.start_orn, pl.cnt_prev, pl.list_prev,
+                                                  pl.cnt_cur, pl.list_cur, pl.cnt_next, spare, 0, 1, h->sm_count, pl.seq, h->n))));
     LAUNCH_CHECK(h);
     SPARE_REBUILD_DONE(h);
   }

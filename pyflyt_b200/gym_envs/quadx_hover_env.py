@@ -7,13 +7,15 @@ substeps, 3 control ticks), reward accumulation, termination / truncation and th
 computed in registers.  Constructor arguments, observation layout, action box, reward and termination
 rules are the reference's; tensors replace numpy arrays and every output has a leading env axis.
 
+``drone_options`` may be a sequence of ``num_envs`` dicts: env ``i`` then flies its own vehicle model (``BatchedAviary``).
+
 ``QuadXHoverEnv`` is the single-env, numpy-in/numpy-out adaptor with the reference's exact
 ``reset``/``step`` signature (what ``gymnasium.make("PyFlyt/QuadX-Hover-v4")`` returns).
 """
 
 from __future__ import annotations
 
-from typing import Any, Literal
+from typing import Any, Literal, Sequence
 
 import numpy as np
 import torch
@@ -38,7 +40,7 @@ class QuadXHoverVecEnv:
         render_mode: None | str = None,
         start_pos: np.ndarray | None = None,
         start_orn: np.ndarray | None = None,
-        drone_options: dict[str, Any] | None = None,
+        drone_options: dict[str, Any] | Sequence[dict[str, Any]] | None = None,
         autoreset: bool = True,
         seed: int | None = None,
         device: str | torch.device = "cuda:0",

@@ -13,7 +13,7 @@ count.
 
 from __future__ import annotations
 
-from typing import Literal
+from typing import Literal, Sequence
 
 import numpy as np
 import torch
@@ -40,7 +40,7 @@ class QuadXWaypointsVecEnv:
         angle_representation: Literal["euler", "quaternion"] = "quaternion",
         agent_hz: int = 30,
         render_mode: None | str = None,
-        drone_options: dict | None = None,
+        drone_options: dict | Sequence[dict] | None = None,  # a sequence: one vehicle model per env (BatchedAviary)
         autoreset: bool = True,
         seed: int | None = None,
         device: str | torch.device = "cuda:0",

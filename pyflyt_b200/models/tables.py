@@ -354,6 +354,69 @@ def build_model(
     return m
 
 
+MAX_QUADX_MODELS = 16  # PFB_MAX_QUADX_MODELS (include/pyflyt_b200.h)
+
+
+class ModelSetError(ValueError):
+    """A ``drone_options`` sequence the batched stepper cannot fly in one handle (``BatchedAviary`` raises it as
+    ``AviaryInitException``)."""
+
+
+def _options_key(opts: dict) -> str:
+    return repr(sorted((str(k), repr(v)) for k, v in opts.items()))
+
+
+def build_model_set(kind: str, drone_options, physics_hz: int, n: int) -> tuple[list[PfbModel], np.ndarray]:
+    """Per-drone vehicle tables for ``n`` drones of one ``kind``.
+
+    ``drone_options`` is what the reference's ``Aviary`` takes (aviary.py:75, 196-199): ``None`` or one dict for every drone,
+    or a sequence of ``n`` dicts (or ``None``), one per drone.  Returns ``(tables, index)``: the distinct tables and a uint8
+    array ``[n]``, drone ``i`` flies ``tables[index[i]]``.  Two drones share a table when their built tables are byte-equal,
+    so a sequence that names the same vehicle in two ways still builds one table.
+
+    Raises ``ModelSetError`` for a sequence of the wrong length (the reference's message), for entries with different
+    ``control_hz`` (each handle runs one substep ratio), for more than ``MAX_QUADX_MODELS`` distinct QuadX tables and for more
+    than one distinct fixed-wing or rocket table."""
+    if drone_options is None or isinstance(drone_options, dict):
+        entries = [dict(drone_options or {})]
+        index = np.zeros(n, dtype=np.int64)
+    else:
+        seq = list(drone_options)
+        if len(seq) != n:  # aviary.py:150-153
+            raise ModelSetError(
+                f"If multiple `drone_options` ({len(seq)}) are used, must have same number of `drone_options` as number of drones ({n})."
+            )
+        keys: dict[str, int] = {}
+        entries, index = [], np.zeros(n, dtype=np.int64)
+        for i, d in enumerate(seq):
+            d = dict(d or {})
+            key = _options_key(d)
+            if key not in keys:
+                keys[key] = len(entries)
+                entries.append(d)
+            index[i] = keys[key]
+    rates = sorted({int(e.get("control_hz", 120)) for e in entries})
+    if len(rates) > 1:
+        raise ModelSetError(f"every drone of a batch needs the same control_hz (one substep ratio per batch); got {rates}.")
+    tables: list[PfbModel] = []
+    by_bytes: dict[bytes, int] = {}
+    remap = np.zeros(len(entries), dtype=np.int64)
+    for j, e in enumerate(entries):
+        opts = dict(e)
+        control_hz = int(opts.pop("control_hz", 120))
+        m = build_model(kind, opts.pop("drone_model", None), opts.pop("model_dir", None), physics_hz, control_hz, **opts)
+        b = C.string_at(C.addressof(m), C.sizeof(m))
+        if b not in by_bytes:
+            by_bytes[b] = len(tables)
+            tables.append(m)
+        remap[j] = by_bytes[b]
+    if kind != "quadx" and len(tables) > 1:
+        raise ModelSetError(f"a {kind} batch flies one vehicle model; the drone_options build {len(tables)} different ones.")
+    if len(tables) > MAX_QUADX_MODELS:
+        raise ModelSetError(f"a batch flies at most {MAX_QUADX_MODELS} different vehicle models; the drone_options build {len(tables)}.")
+    return tables, remap[index].astype(np.uint8)
+
+
 def model_from_files(kind: str, urdf_path: str, yaml_path: str, physics_hz: int = 240, control_hz: int = 120, **options) -> PfbModel:
     """The same table built INSIDE the C-ABI (``pfb_model_from_files``, pyflyt_b200/csrc/pfb_model_files.cu) from a
     ``<model>.urdf`` + ``<model>.yaml`` pair in the reference's layout (base_drone.py:104-110): what a non-Python caller uses.

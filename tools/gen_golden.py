@@ -75,6 +75,70 @@ def fly_quadx(name, mode, drone_model, start_pos, start_orn, setpoint_schedule, 
     print(name, "final pos", states[-1][3], "draws", len(rng.normal_log))
 
 
+def fly_quadx_mixed(name, mode, drone_options, start_pos, start_orn, setpoint_schedule, n_steps, seed):
+    """Aviary-level flight of several QuadX drones with ONE options dict per drone in one reference Aviary (aviary.py:75,
+    196-199).  ``model_dir`` entries are given relative to tests/golden and resolved here; the fixture stores them relative.
+    setpoint_schedule: {step_index: [n, 4]} applied before the step.  The noise log holds the draws in the reference's order:
+    per physics step, one per drone in drone order."""
+    n = len(drone_options)
+    resolved = [dict(d, model_dir=os.path.join(OUT, d["model_dir"])) if "model_dir" in d else dict(d) for d in drone_options]
+    rng = ril.ScriptedNoise(seed)
+    env = Aviary(
+        start_pos=np.array(start_pos, dtype=np.float64),
+        start_orn=np.array(start_orn, dtype=np.float64),
+        drone_type="quadx",
+        drone_options=resolved,
+        np_random=rng,
+    )
+    env.set_mode(mode)
+    sp_after_mode = np.array([d.setpoint for d in env.drones], dtype=np.float64)
+    states, auxs, contacts, sps = [], [], [], []
+    for i in range(n_steps):
+        if i in setpoint_schedule:
+            env.set_all_setpoints(np.array(setpoint_schedule[i], dtype=np.float64))
+        sps.append(np.array([d.setpoint for d in env.drones], dtype=np.float64))
+        env.step()
+        states.append(np.array([d.state for d in env.drones]))
+        auxs.append(np.array([d.aux_state for d in env.drones]))
+        contacts.append(np.array([bool(env.contact_array[env.planeId, d.Id]) for d in env.drones]))
+    np.savez_compressed(
+        os.path.join(OUT, f"{name}.npz"),
+        kind="quadx_mixed_aviary",
+        mode=mode,
+        n_drones=n,
+        drone_options=json.dumps(drone_options),
+        start_pos=np.array(start_pos, dtype=np.float64),
+        start_orn=np.array(start_orn, dtype=np.float64),
+        setpoint_after_set_mode=sp_after_mode,
+        setpoints=np.array(sps),
+        noise=np.array(rng.normal_log),
+        state=np.array(states),
+        aux=np.array(auxs),
+        contact=np.array(contacts),
+    )
+    print(name, "final z", np.array(states[-1])[:, 3, 2], "draws", len(rng.normal_log), "contacts", int(np.sum(contacts)))
+
+
+def mixed_model_fixtures():
+    """Six drones alternating cf2x / primitive_drone, one of the primitive_drone slots flying primitive_tuned (a copy whose
+    YAML changes thrust_coef, drag_coef_xyz and an ang_vel gain) loaded through model_dir: three distinct tables.
+    No drone touches the floor: QuadX.update_physics drops the rotational drag when getContactPoints() of the WHOLE world is
+    non-empty (quadx.py:508-510), so in one reference Aviary a drone's floor contact changes every other drone's flight,
+    while the batched stepper gives each drone its own world."""
+    opts = [dict(drone_model="cf2x"), dict(drone_model="primitive_drone"), dict(drone_model="cf2x"),
+            dict(drone_model="primitive_tuned", model_dir="vehicles"), dict(drone_model="cf2x"), dict(drone_model="primitive_drone")]
+    n = len(opts)
+    pos = [[10.0 * k, 0.0, 60.0 + 0.5 * k] for k in range(n)]
+    orn = [[0.05 * k, -0.04 * k, 0.3 * k] for k in range(n)]
+    r = np.random.default_rng(91)
+    sched0 = {k: np.concatenate([r.uniform(-0.4, 0.4, (n, 3)), r.uniform(0.2, 0.6, (n, 1))], axis=1) for k in range(0, 300, 60)}
+    fly_quadx_mixed("mixed_models_quadx_mode0", 0, opts, pos, orn, sched0, 300, seed=92)
+    pos7 = [[10.0 * k, 0.0, 2.0 + 0.5 * k] for k in range(n)]
+    sched7 = {k: np.concatenate([r.uniform(-1.0, 1.0, (n, 2)) + np.array(pos7)[:, :2], r.uniform(-0.8, 0.8, (n, 1)), r.uniform(1.0, 4.0, (n, 1))], axis=1)
+              for k in range(0, 300, 100)}
+    fly_quadx_mixed("mixed_models_quadx_mode7", 7, opts, pos7, orn, sched7, 300, seed=93)
+
+
 def wind_fields(wind):
     """npz entries describing an AnalyticWind (absent = still air)"""
     if wind is None:
@@ -696,3 +760,5 @@ if __name__ == "__main__":
         wind_fixtures()
     if which in ("all", "touchdown"):
         touchdown_fixtures()
+    if which in ("all", "mixed"):
+        mixed_model_fixtures()
