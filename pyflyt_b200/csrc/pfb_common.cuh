@@ -204,6 +204,9 @@ PFB_HD float u32_to_unit_open(uint32_t u) {
   return ((float)(u >> 8) + 1.0f) * (1.0f / 16777216.0f);
 }
 
+// stream tags of the Philox counters (top byte of the last counter word)
+enum { TAG_AVIARY = 0, TAG_ENV_STEP = 1, TAG_RESET = 2, TAG_ACTION = 3 };
+
 // two standard normals from two uniforms (Box–Muller); noise only, so fast intrinsics are fine
 PFB_HD void box_muller(uint32_t a, uint32_t b, float& n0, float& n1) {
   float u1 = u32_to_unit_open(a);

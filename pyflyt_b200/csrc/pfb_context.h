@@ -158,29 +158,96 @@ static inline StepPlan plan_step(PfbContext* h) {
   return p;
 }
 
-// ---- reset pipeline plumbing shared by the env kinds that keep spare post-reset states (DESIGN.md §4) ----------------
-// before step k: the rebuild of the spares consumed by step k - 2 must be complete (an env cannot finish again sooner)
-#define SPARE_BEFORE_STEP(h, s)                                                                          \
-  do {                                                                                                   \
-    if ((h)->d_spare && (h)->env.autoreset && (h)->step_seq >= 2)                                        \
-      CUDA_OK(cudaStreamWaitEvent((s), (h)->ev_spare[((h)->step_seq - 2) % 4], 0));                      \
-  } while (0)
-// after step k was launched on `s`: order the side stream behind it; the caller then launches the build-mode kernel on
-// (h)->side and calls SPARE_REBUILD_DONE
-#define SPARE_REBUILD_BEGIN(h, s)                              \
-  do {                                                         \
-    CUDA_OK(cudaEventRecord((h)->ev_step, (s)));               \
-    CUDA_OK(cudaStreamWaitEvent((h)->side, (h)->ev_step, 0));  \
-  } while (0)
-#define SPARE_REBUILD_DONE(h) CUDA_OK(cudaEventRecord((h)->ev_spare[(h)->step_seq % 4], (h)->side))
-// before a user reset rewrites the spares: the last rebuild must have finished
-#define SPARE_BEFORE_RESET(h, s)                                                                         \
-  do {                                                                                                   \
-    if ((h)->d_spare && (h)->step_seq > 0) CUDA_OK(cudaStreamWaitEvent((s), (h)->ev_spare[((h)->step_seq - 1) % 4], 0)); \
-  } while (0)
-
 // pfb_lib.cu: a masked user reset on an autoreset handle removes the masked envs / arenas from the pending done list
 int pfb_drop_masked_done(PfbContext* h, const uint8_t* mask, cudaStream_t s);
+
+// Runs BODY with `constexpr int MODE` = the QuadX flight mode `mode`
+#define PFB_MODE_SWITCH(mode, BODY)                         \
+  switch (mode) {                                           \
+    case -1: { constexpr int MODE = -1; BODY; } break;      \
+    case 0: { constexpr int MODE = 0; BODY; } break;        \
+    case 1: { constexpr int MODE = 1; BODY; } break;        \
+    case 2: { constexpr int MODE = 2; BODY; } break;        \
+    case 3: { constexpr int MODE = 3; BODY; } break;        \
+    case 4: { constexpr int MODE = 4; BODY; } break;        \
+    case 5: { constexpr int MODE = 5; BODY; } break;        \
+    case 6: { constexpr int MODE = 6; BODY; } break;        \
+    case 7: { constexpr int MODE = 7; BODY; } break;        \
+    default: return fail("`mode` must be between -1 and 7, got %d", mode); \
+  }
+
+// ---- host side of the tail-CTA env kinds (pfb_tail_step.cuh): QuadX-Waypoints, Fixedwing-Waypoints, Rocket-Landing, Dogfight ----
+// Each kind passes one generic lambda `launch(StepVariant<INJECT, RANDACT, AUTORESET>{}, const TailLaunch&)` that launches its step
+// kernel and returns 0 or the result of fail(); it serves the step, the side-stream spare rebuild and the build after a reset.
+template <bool INJECT, bool RANDACT, bool AUTORESET>
+struct StepVariant {
+  static constexpr bool inject = INJECT, randact = RANDACT, autoreset = AUTORESET;
+};
+struct TailLaunch {
+  int grid, tail_blocks;
+  float* spare;
+  int spare_copy, build;
+  const int32_t *prev_count, *prev_list;
+  int32_t *cur_count, *cur_list, *next_count;
+  uint32_t seq;
+  cudaStream_t stream;
+};
+
+template <class Launch>
+int tail_env_step(PfbContext* h, const float* noise, bool randact, cudaStream_t s, Launch&& launch) {
+  const StepPlan pl = plan_step(h);
+  float* spare = h->env.autoreset ? h->d_spare : nullptr;
+  // the rebuild of the spares consumed by step k - 2 must be complete before step k (an env cannot finish again sooner)
+  if (spare && h->step_seq >= 2) CUDA_OK(cudaStreamWaitEvent(s, h->ev_spare[(h->step_seq - 2) % 4], 0));
+  if (pl.prof) CUDA_OK(cudaEventRecord(h->prof_ev[2 * h->prof_n], s));
+  const TailLaunch L = {pl.grid, pl.tail, spare, (spare && !h->env.inline_reset) ? 1 : 0, 0,
+                        pl.cnt_prev, pl.list_prev, pl.cnt_cur, pl.list_cur, pl.cnt_next, pl.seq, s};
+  int rc;
+  if (h->env.autoreset) {
+    if (noise) return fail("injected noise (parity mode) is only supported with autoreset = 0");
+    rc = randact ? launch(StepVariant<false, true, true>{}, L) : launch(StepVariant<false, false, true>{}, L);
+  } else {
+    rc = noise ? launch(StepVariant<true, false, false>{}, L)
+               : (randact ? launch(StepVariant<false, true, false>{}, L) : launch(StepVariant<false, false, false>{}, L));
+  }
+  if (rc) return rc;
+  LAUNCH_CHECK(h);
+  if (pl.prof) {
+    CUDA_OK(cudaEventRecord(h->prof_ev[2 * h->prof_n + 1], s));
+    h->prof_n += 1;
+  }
+  if (spare) {  // rebuild the spares this launch consumed, on the side stream (ordered behind it), while the next launches run
+    CUDA_OK(cudaEventRecord(h->ev_step, s));
+    CUDA_OK(cudaStreamWaitEvent(h->side, h->ev_step, 0));
+    const TailLaunch B = {h->sm_count, h->sm_count, spare, 0, 1, pl.cnt_prev, pl.list_prev, pl.cnt_cur, pl.list_cur, pl.cnt_next, pl.seq, h->side};
+    if (launch(StepVariant<false, false, true>{}, B)) return -1;
+    LAUNCH_CHECK(h);
+    CUDA_OK(cudaEventRecord(h->ev_spare[h->step_seq % 4], h->side));
+  }
+  h->step_seq += 1;
+  return 0;
+}
+
+// `reset(grid)` launches the kind's reset kernel over every env and returns 0 or the result of fail()
+template <class Reset, class Launch>
+int tail_env_reset(PfbContext* h, const uint8_t* mask, cudaStream_t s, Reset&& reset, Launch&& launch) {
+  const int g = grid_for(h->n);
+  float* spare = h->env.autoreset ? h->d_spare : nullptr;
+  if (spare) {
+    // the spares are rewritten below: the last rebuild must have finished
+    if (h->step_seq > 0) CUDA_OK(cudaStreamWaitEvent(s, h->ev_spare[(h->step_seq - 1) % 4], 0));
+    if (!mask) CUDA_OK(cudaMemsetAsync(h->d_counters, 0, 4 * sizeof(int32_t), s));  // a full reset empties the autoreset queues
+    else if (pfb_drop_masked_done(h, mask, s)) return -1;  // a masked one takes its envs out of the pending done list
+  }
+  if (reset(g)) return -1;
+  LAUNCH_CHECK(h);
+  if (spare) {  // every env gets a fresh spare: the step kernel in build mode over all envs, same stream
+    const TailLaunch B = {g, g, spare, 0, 1, nullptr, nullptr, nullptr, nullptr, nullptr, 0u, s};
+    if (launch(StepVariant<false, false, true>{}, B)) return -1;
+    LAUNCH_CHECK(h);
+  }
+  return 0;
+}
 
 // fixedwing translation unit (pfb_fixedwing.cu)
 int fw_build_params(const PfbModel& m, const PfbEnvConfig* env, pfb::FixedwingParams& p, pfb::WaypointParams& w);
@@ -193,6 +260,7 @@ int fw_aviary_step(PfbContext* h, int n_steps, const float* noise, cudaStream_t 
 int fw_observe(PfbContext* h, cudaStream_t s);
 int fw_env_reset(PfbContext* h, const uint8_t* mask, const float* noise, cudaStream_t s);
 int fw_env_step(PfbContext* h, float* actions, const float* noise, bool randact, cudaStream_t s);
+int fw_spare_rows();
 
 // rocket translation unit (pfb_rocket.cu)
 int rk_build_params(const PfbModel& m, const PfbEnvConfig* env, pfb::RocketParams& p, pfb::LandingParams& l);
@@ -206,6 +274,7 @@ int rk_aviary_step(PfbContext* h, int n_steps, const float* noise, cudaStream_t 
 int rk_observe(PfbContext* h, cudaStream_t s);
 int rk_env_reset(PfbContext* h, const uint8_t* mask, const float* noise, cudaStream_t s);
 int rk_env_step(PfbContext* h, float* actions, const float* noise, bool randact, cudaStream_t s);
+int rk_spare_rows();
 
 // dogfight translation unit (pfb_dogfight.cu): fixedwing vehicles, arenas of 2*team_size adjacent envs
 int df_build_params(const PfbEnvConfig* env, pfb::DogfightParams& d);

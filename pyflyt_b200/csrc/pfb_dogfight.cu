@@ -12,6 +12,7 @@
 
 #include "pfb_context.h"
 #include "pfb_noise.cuh"
+#include "pfb_tail_step.cuh"
 
 using namespace pfb;
 
@@ -290,29 +291,19 @@ __global__ void __launch_bounds__(kBlock, kAeroBlocks)
   __shared__ float smem[kBlock * kDfObsStride];
   __shared__ uint8_t row_skip[kBlock];
   constexpr int O = 23 + 14 * (A - 1);
-  const bool tail = AUTORESET && (int)blockIdx.x < tail_blocks;
-  const int64_t block_first = tail ? 0 : (int64_t)((int)blockIdx.x - (AUTORESET ? tail_blocks : 0)) * kBlock;
+  // work items are whole arenas: a regular lane owns one agent; tail lanes stride over the done-arena list
+  const TailPlan pl = tail_plan<AUTORESET, A>(tail_blocks, build, prev_count, prev_list, next_count, N);
+  const bool tail = pl.tail;
+  const int64_t block_first = pl.block_first;
   const int li = threadIdx.x % A;                 // agent index inside its arena
   const int base = (threadIdx.x & 31) - li;       // lane of the arena's agent 0
-  // work items are whole arenas: a regular lane owns one agent; tail lanes stride over the done-arena list
-  int t, t_end, t_stride;
-  if (tail) {
-    if (blockIdx.x == 0 && threadIdx.x == 0 && !build) *next_count = 0;
-    t = (blockIdx.x * kBlock + threadIdx.x) / A;
-    t_end = prev_list ? *prev_count : (int)(N / A);  // build mode after a user reset: every arena
-    t_stride = tail_blocks * kBlock / A;
-  } else {
-    t = 0;
-    t_end = (block_first + threadIdx.x < N) ? 1 : 0;  // N is a multiple of A: an arena is never cut
-    t_stride = 1;
-  }
   bool skip = true;
   float* row = smem + threadIdx.x * kDfObsStride;
 #pragma unroll 1
-  for (;; t += t_stride) {
+  for (int t = pl.t0;; t += pl.stride) {
     // whole arenas enter or leave together (t is arena-uniform), so every shuffle below names exactly the
     // lanes that are present
-    const bool go = t < t_end;
+    const bool go = t < pl.t_end;
     unsigned lanes = __ballot_sync(0xffffffffu, go);
     if (lanes == 0u) break;
     if (!go) continue;
@@ -377,10 +368,7 @@ __global__ void __launch_bounds__(kBlock, kAeroBlocks)
       if (AUTORESET && arena_done) continue;
       float act[4];
       if (RANDACT) {
-        uint64_t g = ((uint64_t)rng.env_offset_hi << 32 | rng.env_offset_lo) + (uint64_t)i;
-        U4 r = philox4x32_10(U4{(uint32_t)g, (uint32_t)(g >> 32), step_seq, (uint32_t)TAG_ACTION << 24}, rng.k0, rng.k1);
-        act[0] = 2.0f * u32_to_unit_open(r.x) - 1.0f; act[1] = 2.0f * u32_to_unit_open(r.y) - 1.0f;
-        act[2] = 2.0f * u32_to_unit_open(r.z) - 1.0f; act[3] = 2.0f * u32_to_unit_open(r.w) - 1.0f;
+        fixedwing_random_action(rng, i, step_seq, act);
         reinterpret_cast<float4*>(actions)[i] = make_float4(act[0], act[1], act[2], act[3]);
       } else {
         float4 a4 = __ldg(reinterpret_cast<const float4*>(actions) + i);
@@ -416,40 +404,18 @@ __global__ void __launch_bounds__(kBlock, kAeroBlocks)
     if (info)
       info[i] = (uint8_t)(((flags & FLAG_OOB) ? 1 : 0) | ((flags & FLAG_COLLISION) ? 2 : 0) | ((flags & FLAG_DF_DEAD) ? 4 : 0) | ((flags & FLAG_DF_WIN) ? 8 : 0));
     if (tail) {
-      float* dst = obs + i * O;
-      for (int k = 0; k < O; ++k) dst[k] = row[k];
+      obs_write_row(obs, i, O, row);
     } else {
       skip = false;
       if (AUTORESET) {  // queue arenas whose agents have ALL left self.agents (the arena's first lane speaks for it)
         const unsigned arena_mask = ((1u << A) - 1u) << base;
         const unsigned done_lanes = __ballot_sync(lanes, (flags & FLAG_AGENT_DONE) != 0);
-        const bool leader_done = (li == 0) && ((done_lanes & arena_mask) == arena_mask);
-        unsigned m = __ballot_sync(lanes, leader_done);
-        if (leader_done) {
-          int lane = threadIdx.x & 31;
-          int leader = __ffs(m) - 1;
-          int b0 = 0;
-          if (lane == leader) b0 = atomicAdd(cur_count, __popc(m));
-          b0 = __shfl_sync(m, b0, leader);
-          cur_list[b0 + __popc(m & ((1u << lane) - 1u))] = (int32_t)i;
-        }
+        done_list_append(lanes, (li == 0) && ((done_lanes & arena_mask) == arena_mask), i, cur_count, cur_list);
       }
     }
   }
   if (tail) return;
-  row_skip[threadIdx.x] = skip ? 1 : 0;
-  __syncthreads();
-  int64_t rows = N - block_first;
-  if (rows > kBlock) rows = kBlock;
-  const int total = (int)rows * O;
-  float* dst = obs + block_first * O;
-  const int dr = kBlock / O, dc = kBlock - dr * O;
-  int r = threadIdx.x / O, c = threadIdx.x - r * O;
-  for (int j = threadIdx.x; j < total; j += kBlock) {
-    if (!row_skip[r]) dst[j] = smem[r * kDfObsStride + c];
-    r += dr; c += dc;
-    if (c >= O) { c -= O; ++r; }
-  }
+  obs_write_block<kDfObsStride>(obs, smem, row_skip, skip, block_first, O, N);
 }
 
 template <int A, bool INJECT>
@@ -482,77 +448,39 @@ __global__ void __launch_bounds__(kBlock)
 // ---------------------------------------------------------------------------------------------------
 // launchers
 // ---------------------------------------------------------------------------------------------------
+// one launch of k_df_step (arenas of A = 2 * team_size) for tail_env_step / tail_env_reset
+static auto df_launcher(PfbContext* h, float* actions, const float* noise) {
+  return [=](auto v, const TailLaunch& L) -> int {
+    using V = decltype(v);
+    auto k = h->df.team_size == 1 ? k_df_step<2, V::inject, V::randact, V::autoreset> : k_df_step<4, V::inject, V::randact, V::autoreset>;
+    k<<<L.grid, kBlock, 0, L.stream>>>(h->fw, h->df, h->rng, h->buf.state, h->buf.istate, actions, noise, h->buf.obs, h->buf.reward, h->buf.term,
+                                       h->buf.trunc, h->buf.info, h->buf.start_pos, h->buf.start_orn, L.prev_count, L.prev_list, L.cur_count,
+                                       L.cur_list, L.next_count, L.spare, L.spare_copy, L.build, L.tail_blocks, L.seq, h->n);
+    return 0;
+  };
+}
+
 int df_env_reset(PfbContext* h, const uint8_t* mask, const float* noise, cudaStream_t s) {
   const uint32_t seq = 0x80000000u | (uint32_t)h->reset_seq++;
-  const int g = grid_for(h->n);
   const int A = 2 * h->df.team_size;
   if (h->n % A) return fail("the number of envs (%lld) must be a multiple of the arena size %d", (long long)h->n, A);
   const int rnd = h->env.randomize_drop;  // reused as "draw the spawn on device" for the dogfight
-  float* spare = h->env.autoreset ? h->d_spare : nullptr;
-  if (spare) {
-    SPARE_BEFORE_RESET(h, s);
-    if (!mask) CUDA_OK(cudaMemsetAsync(h->d_counters, 0, 4 * sizeof(int32_t), s));  // a full reset empties the autoreset queues
-    else if (pfb_drop_masked_done(h, mask, s)) return -1;  // a masked one takes its envs out of the pending done list
-  }
+  auto reset = [&](int g) -> int {
 #define DR_ARGS h->fw, h->df, h->rng, h->buf.state, h->buf.istate, h->buf.start_pos, h->buf.start_orn, mask, noise, h->buf.obs, seq, rnd, h->n
-  if (A == 2) { if (noise) k_df_reset<2, true><<<g, kBlock, 0, s>>>(DR_ARGS); else k_df_reset<2, false><<<g, kBlock, 0, s>>>(DR_ARGS); }
-  else { if (noise) k_df_reset<4, true><<<g, kBlock, 0, s>>>(DR_ARGS); else k_df_reset<4, false><<<g, kBlock, 0, s>>>(DR_ARGS); }
+    if (A == 2) { if (noise) k_df_reset<2, true><<<g, kBlock, 0, s>>>(DR_ARGS); else k_df_reset<2, false><<<g, kBlock, 0, s>>>(DR_ARGS); }
+    else { if (noise) k_df_reset<4, true><<<g, kBlock, 0, s>>>(DR_ARGS); else k_df_reset<4, false><<<g, kBlock, 0, s>>>(DR_ARGS); }
 #undef DR_ARGS
-  LAUNCH_CHECK(h);
-  if (spare) {  // every arena gets fresh spares: the step kernel in build mode over all arenas, same stream
-#define DB_ARGS h->fw, h->df, h->rng, h->buf.state, h->buf.istate, h->buf.setpoint, nullptr, h->buf.obs, h->buf.reward, h->buf.term, h->buf.trunc, \
-                h->buf.info, h->buf.start_pos, h->buf.start_orn, nullptr, nullptr, nullptr, nullptr, nullptr, spare, 0, 1, g, 0u, h->n
-    if (A == 2) k_df_step<2, false, false, true><<<g, kBlock, 0, s>>>(DB_ARGS);
-    else k_df_step<4, false, false, true><<<g, kBlock, 0, s>>>(DB_ARGS);
-#undef DB_ARGS
-    LAUNCH_CHECK(h);
-  }
+    return 0;
+  };
+  if (tail_env_reset(h, mask, s, reset, df_launcher(h, h->buf.setpoint, nullptr))) return -1;
   h->mode = 0;
   return 0;
 }
 
 int df_env_step(PfbContext* h, float* actions, const float* noise, bool randact, cudaStream_t s) {
-  StepPlan pl = plan_step(h);
   const int A = 2 * h->df.team_size;
   if (h->n % A) return fail("the number of envs (%lld) must be a multiple of the arena size %d", (long long)h->n, A);
-  float* spare = h->env.autoreset ? h->d_spare : nullptr;
-  const int spare_copy = (spare && !h->env.inline_reset) ? 1 : 0;
-  SPARE_BEFORE_STEP(h, s);
-  if (pl.prof) CUDA_OK(cudaEventRecord(h->prof_ev[2 * h->prof_n], s));
-#define DF_ARGS h->fw, h->df, h->rng, h->buf.state, h->buf.istate, actions, noise, h->buf.obs, h->buf.reward, h->buf.term, h->buf.trunc, \
-                h->buf.info, h->buf.start_pos, h->buf.start_orn, pl.cnt_prev, pl.list_prev, pl.cnt_cur, pl.list_cur, pl.cnt_next, spare, \
-                spare_copy, 0, pl.tail, pl.seq, h->n
-#define DF_LAUNCH(AA)                                                                                         \
-  if (h->env.autoreset) {                                                                                     \
-    if (noise) return fail("injected noise (parity mode) is only supported with autoreset = 0");              \
-    if (randact) k_df_step<AA, false, true, true><<<pl.grid, kBlock, 0, s>>>(DF_ARGS);                        \
-    else k_df_step<AA, false, false, true><<<pl.grid, kBlock, 0, s>>>(DF_ARGS);                               \
-  } else {                                                                                                    \
-    if (noise) k_df_step<AA, true, false, false><<<pl.grid, kBlock, 0, s>>>(DF_ARGS);                         \
-    else if (randact) k_df_step<AA, false, true, false><<<pl.grid, kBlock, 0, s>>>(DF_ARGS);                  \
-    else k_df_step<AA, false, false, false><<<pl.grid, kBlock, 0, s>>>(DF_ARGS);                              \
-  }
-  if (A == 2) { DF_LAUNCH(2) } else { DF_LAUNCH(4) }
-#undef DF_LAUNCH
-#undef DF_ARGS
-  LAUNCH_CHECK(h);
-  if (pl.prof) {
-    CUDA_OK(cudaEventRecord(h->prof_ev[2 * h->prof_n + 1], s));
-    h->prof_n += 1;
-  }
-  if (spare) {  // rebuild the spares this launch consumed, on the side stream, while the next launches run
-    SPARE_REBUILD_BEGIN(h, s);
-#define DB_ARGS h->fw, h->df, h->rng, h->buf.state, h->buf.istate, actions, nullptr, h->buf.obs, h->buf.reward, h->buf.term, h->buf.trunc, \
-                h->buf.info, h->buf.start_pos, h->buf.start_orn, pl.cnt_prev, pl.list_prev, pl.cnt_cur, pl.list_cur, pl.cnt_next, spare, 0, 1, \
-                h->sm_count, pl.seq, h->n
-    if (A == 2) k_df_step<2, false, false, true><<<h->sm_count, kBlock, 0, h->side>>>(DB_ARGS);
-    else k_df_step<4, false, false, true><<<h->sm_count, kBlock, 0, h->side>>>(DB_ARGS);
-#undef DB_ARGS
-    LAUNCH_CHECK(h);
-    SPARE_REBUILD_DONE(h);
-  }
-  h->step_seq += 1;
-  return 0;
+  return tail_env_step(h, noise, randact, s, df_launcher(h, actions, noise));
 }
 
 // ===================================================================================================

@@ -6,6 +6,7 @@
 
 #include "pfb_context.h"
 #include "pfb_noise.cuh"
+#include "pfb_tail_step.cuh"
 
 using namespace pfb;
 
@@ -203,10 +204,99 @@ __device__ __forceinline__ void wp_reset_env(const FixedwingParams& p, const Way
   (void)wp_update_distance(s, wp);     // end_reset -> compute_state
 }
 
-// ---- spare post-reset states: the QuadX-Hover reset pipeline (pfb_lib.cu, DESIGN.md §4) for this env.  A spare is an
-// env-major record of 64 floats: the FW_* state words INCLUDING the episode's targets and new_distance, then:
-enum { WSP_POSE = FW_ROWS, WSP_VALID = FW_ROWS + 6, WSP_FLAGS = FW_ROWS + 7, WSP_EPISODE = FW_ROWS + 8, WSP_ROWS = 64 };
-static_assert(FW_ROWS + 9 <= WSP_ROWS, "spare record too small");
+// ---- spare post-reset states (pfb_tail_step.cuh): a record holds the FW_* state words INCLUDING the episode's targets and
+// new_distance
+enum { WSP_ROWS = 64 };
+int fw_spare_rows() { return WSP_ROWS; }
+
+// the Fixedwing-Waypoints env for tail_step (pfb_tail_step.cuh)
+template <bool INJECT, bool RANDACT>
+struct WpEnv {
+  const FixedwingParams& p;
+  const WaypointParams& w;
+  const RngParams& rng;
+  using Regs = FixedwingRegs;
+  using Item = WpState;
+  static constexpr int kStateRows = FW_ROWS, kSpareRows = WSP_ROWS, kActions = 4, kObsStride = kWpObsStride;
+  __device__ __forceinline__ int obs_dim() const { return (w.angle_representation == 0 ? 22 : 23) + 3 * w.num_targets; }
+  __device__ __forceinline__ bool pose_keyed() const { return true; }
+  __device__ __forceinline__ WpState item(int64_t) const {
+    WpState wp;
+    return wp;
+  }
+  // a spare's targets are copied into the state rows: the episode starts at target 0
+  __device__ __forceinline__ void load_spare(const float* __restrict__ rec, float* __restrict__ st, int32_t* __restrict__ ist, int64_t N,
+                                             int64_t i, FixedwingRegs& s, WpState& wp) const {
+    fixedwing_load(rec, ist, N, i, s, 1, 0);
+    float* tb = st + i;
+    for (int k = 0; k < 3 * w.num_targets; ++k) tb[(int64_t)(FW_TARGETS + k) * N] = rec[FW_TARGETS + k];
+    wp.first = 0;
+    wp.reached_now = false;
+    wp.new_dist = rec[FW_DIST];
+  }
+  // the targets go to the spare record being built, or to the state rows
+  __device__ __forceinline__ void reset(const float* pose, uint32_t nseq, float* __restrict__ rec, float* __restrict__ st, int64_t N, int64_t i,
+                                        FixedwingRegs& s, WpState& wp) const {
+    wp_reset_env<false>(p, w, rng, pose, nullptr, nullptr, nseq, N, i, rec ? rec : st + i, rec ? 1 : N, s, wp);
+  }
+  __device__ __forceinline__ void store_spare(float* __restrict__ rec, int32_t* __restrict__ ist, int64_t N, int64_t i, const FixedwingRegs& s,
+                                              const WpState& wp) const {
+    fixedwing_store(rec, ist, N, i, s, false, 1, 0);
+    rec[FW_DIST] = wp.new_dist;
+  }
+  __device__ __forceinline__ void load(const float* __restrict__ st, const int32_t* __restrict__ ist, int64_t N, int64_t i, FixedwingRegs& s) const {
+    fixedwing_load(st, ist, N, i, s);
+  }
+  __device__ __forceinline__ void action(float* __restrict__ actions, int64_t i, uint32_t step_seq, float* act) const {
+    if (RANDACT) {
+      fixedwing_random_action(rng, i, step_seq, act);
+      reinterpret_cast<float4*>(actions)[i] = make_float4(act[0], act[1], act[2], act[3]);
+    } else {
+      float4 a4 = __ldg(reinterpret_cast<const float4*>(actions) + i);
+      act[0] = a4.x; act[1] = a4.y; act[2] = a4.z; act[3] = a4.w;
+    }
+  }
+  __device__ __forceinline__ void step(const float* __restrict__ st, const int32_t* __restrict__ ist, const float* __restrict__ noise, int64_t N,
+                                       int64_t i, uint32_t step_seq, const float* act, FixedwingRegs& s, WpState& wp, int& step_count,
+                                       float& rew) const {
+    // fixedwing_base_env.py:257-261: the throttle channel is remapped from [-1, 1] to [0, 1]
+    s.sp[0] = act[0]; s.sp[1] = act[1]; s.sp[2] = act[2]; s.sp[3] = act[3] * 0.5f + 0.5f;
+    step_count = ist[(int64_t)FI_STEP * N + i];
+    wp.first = ist[(int64_t)FI_NTARGETS * N + i];
+    wp.reached_now = false;
+    wp.new_dist = st[(int64_t)FW_DIST * N + i];
+    wp_load_target0(st + i, N, wp);
+    rew = -0.1f;
+    auto nz = make_noise<INJECT>(noise, N, i, rng, step_seq, TAG_ENV_STEP, p.noise_loc, p.ratio);
+    const bool full = fixedwing_full_model(p);
+#pragma unroll 1
+    for (int k = 0; k < w.env_step_ratio; ++k) {
+      if (s.flags & (FLAG_TERM | FLAG_TRUNC)) break;
+      if (full) fixedwing_aviary_step<0, true>(p, s, nz);
+      else fixedwing_aviary_step<0>(p, s, nz);
+      float old = wp_update_distance(s, wp);
+      wp_term_trunc_reward(w, s, wp, old, step_count, rew, st + i, N);
+    }
+    step_count += 1;
+  }
+  // the reference builds the observation in compute_state, BEFORE compute_term_trunc_reward advances the
+  // target list: a target reached on the last Aviary step is still the head of the reported list
+  __device__ __forceinline__ void observe(const float* __restrict__ st, int64_t N, int64_t i, const float* act, const FixedwingRegs& s,
+                                          const WpState& wp, float* row) const {
+    wp_observation(w, s, act, wp.first - (wp.reached_now ? 1 : 0), st + i, N, row);
+  }
+  __device__ __forceinline__ void store(float* __restrict__ st, int32_t* __restrict__ ist, int64_t N, int64_t i, const FixedwingRegs& s,
+                                        const WpState& wp, int step_count) const {
+    fixedwing_store(st, ist, N, i, s);
+    st[(int64_t)FW_DIST * N + i] = wp.new_dist;
+    ist[(int64_t)FI_STEP * N + i] = step_count;
+    ist[(int64_t)FI_NTARGETS * N + i] = wp.first;
+  }
+  __device__ __forceinline__ uint8_t info(const FixedwingRegs& s, const WpState& wp) const {
+    return (uint8_t)(((s.flags & FLAG_OOB) ? 1 : 0) | ((s.flags & FLAG_COLLISION) ? 2 : 0) | ((s.flags & FLAG_ENV_COMPLETE) ? 4 : 0) |
+                     (wp.first << 3));
+  }
+};
 
 template <bool INJECT, bool RANDACT, bool AUTORESET>
 __global__ void __launch_bounds__(kBlock, kAeroBlocks)
@@ -218,156 +308,8 @@ __global__ void __launch_bounds__(kBlock, kAeroBlocks)
                 const int32_t* __restrict__ prev_list, int32_t* __restrict__ cur_count, int32_t* __restrict__ cur_list,
                 int32_t* __restrict__ next_count, float* __restrict__ spare, int spare_copy, int build, int tail_blocks,
                 uint32_t step_seq, int64_t N) {
-  __shared__ float smem[kBlock * kWpObsStride];
-  __shared__ uint8_t row_skip[kBlock];
-  const int slot = (int)threadIdx.x;  // env within the CTA
-  const int O = (w.angle_representation == 0 ? 22 : 23) + 3 * w.num_targets;
-  const bool tail = AUTORESET && (int)blockIdx.x < tail_blocks;
-  const int64_t block_first = tail ? 0 : (int64_t)((int)blockIdx.x - (AUTORESET ? tail_blocks : 0)) * kBlock;
-  int t, t_end, t_stride;
-  if (tail) {
-    if (blockIdx.x == 0 && threadIdx.x == 0 && !build) *next_count = 0;
-    t = blockIdx.x * kBlock + slot;
-    t_end = prev_list ? *prev_count : (int)N;  // build mode after a user reset: every env
-    t_stride = tail_blocks * kBlock;
-  } else {
-    t = 0;
-    t_end = (block_first + slot < N) ? 1 : 0;
-    t_stride = 1;
-  }
-  bool skip = true;
-  float* row = smem + slot * kWpObsStride;
-#pragma unroll 1
-  for (; t < t_end; t += t_stride) {
-    const int64_t i = tail ? (prev_list ? (int64_t)prev_list[t] : (int64_t)t) : block_first + slot;
-    FixedwingRegs s;
-    WpState wp;
-    float act[4] = {0.f, 0.f, 0.f, 0.f};
-    int step_count = 0;
-    float rew = 0.0f;
-    float* tb = st + i;  // where this env's targets live (field-major state rows, or the spare record being built)
-    int64_t ts = N;
-    if (tail) {
-      // env.reset(): normally a copy of the env's spare (state, targets, new_distance of the NEXT episode); build mode
-      // computes that spare; without a usable spare the warm-up runs inline with the same episode number
-      float* rec = spare ? spare + i * WSP_ROWS : nullptr;
-      uint32_t nseq = step_seq | 0x40000000u;
-      bool hit = false;
-      float pose[6];
-#pragma unroll
-      for (int k = 0; k < 3; ++k) { pose[k] = start_pos[3 * i + k]; pose[3 + k] = start_orn[3 * i + k]; }
-      if (rec) {
-        nseq = __float_as_uint(rec[WSP_EPISODE]) + (build ? 1u : 0u);
-        hit = !build && spare_copy && rec[WSP_VALID] != 0.0f;
-#pragma unroll
-        for (int k = 0; k < 6; ++k) hit = hit && (rec[WSP_POSE + k] == pose[k]);
-      }
-      if (hit) {
-        fixedwing_load(rec, ist, N, i, s, 1, 0);
-        s.flags = __float_as_uint(rec[WSP_FLAGS]);
-        for (int k = 0; k < 3 * w.num_targets; ++k) tb[(int64_t)(FW_TARGETS + k) * ts] = rec[FW_TARGETS + k];
-        wp.first = 0;
-        wp.reached_now = false;
-        wp.new_dist = rec[FW_DIST];
-      } else {
-        if (build) {
-          rec[WSP_VALID] = 0.0f;  // invalid until the warm-up below is stored
-#pragma unroll
-          for (int k = 0; k < 6; ++k) rec[WSP_POSE + k] = pose[k];
-          tb = rec;
-          ts = 1;
-        }
-        wp_reset_env<false>(p, w, rng, pose, nullptr, nullptr, nseq, N, i, tb, ts, s, wp);
-      }
-      if (build) {
-        fixedwing_store(rec, ist, N, i, s, false, 1, 0);
-        rec[FW_DIST] = wp.new_dist;
-        rec[WSP_FLAGS] = __uint_as_float(s.flags);
-        rec[WSP_EPISODE] = __uint_as_float(nseq);
-        rec[WSP_VALID] = 1.0f;
-        continue;
-      }
-      s.flags |= fresh_tag(step_seq);
-    } else {
-      fixedwing_load(st, ist, N, i, s);
-      if (AUTORESET && (s.flags & (FLAG_TERM | FLAG_TRUNC | fresh_tag(step_seq)))) continue;  // a tail CTA owns this env
-      s.flags &= ~(uint32_t)FLAG_FRESH_ANY;
-      if (RANDACT) {
-        uint64_t g = ((uint64_t)rng.env_offset_hi << 32 | rng.env_offset_lo) + (uint64_t)i;
-        U4 r = philox4x32_10(U4{(uint32_t)g, (uint32_t)(g >> 32), step_seq, (uint32_t)TAG_ACTION << 24}, rng.k0, rng.k1);
-        act[0] = 2.0f * u32_to_unit_open(r.x) - 1.0f; act[1] = 2.0f * u32_to_unit_open(r.y) - 1.0f;
-        act[2] = 2.0f * u32_to_unit_open(r.z) - 1.0f; act[3] = 2.0f * u32_to_unit_open(r.w) - 1.0f;
-        reinterpret_cast<float4*>(actions)[i] = make_float4(act[0], act[1], act[2], act[3]);
-      } else {
-        float4 a4 = __ldg(reinterpret_cast<const float4*>(actions) + i);
-        act[0] = a4.x; act[1] = a4.y; act[2] = a4.z; act[3] = a4.w;
-      }
-      // fixedwing_base_env.py:257-261: the throttle channel is remapped from [-1, 1] to [0, 1]
-      s.sp[0] = act[0]; s.sp[1] = act[1]; s.sp[2] = act[2]; s.sp[3] = act[3] * 0.5f + 0.5f;
-      step_count = ist[(int64_t)FI_STEP * N + i];
-      wp.first = ist[(int64_t)FI_NTARGETS * N + i];
-      wp.reached_now = false;
-      wp.new_dist = st[(int64_t)FW_DIST * N + i];
-      wp_load_target0(tb, ts, wp);
-      rew = -0.1f;
-      auto nz = make_noise<INJECT>(noise, N, i, rng, step_seq, TAG_ENV_STEP, p.noise_loc, p.ratio);
-      const bool full = fixedwing_full_model(p);
-#pragma unroll 1
-      for (int k = 0; k < w.env_step_ratio; ++k) {
-        if (s.flags & (FLAG_TERM | FLAG_TRUNC)) break;
-        if (full) fixedwing_aviary_step<0, true>(p, s, nz);
-        else fixedwing_aviary_step<0>(p, s, nz);
-        float old = wp_update_distance(s, wp);
-        wp_term_trunc_reward(w, s, wp, old, step_count, rew, tb, ts);
-      }
-      step_count += 1;
-    }
-    // the reference builds the observation in compute_state, BEFORE compute_term_trunc_reward advances the
-    // target list: a target reached on the last Aviary step is still the head of the reported list
-    wp_observation(w, s, act, wp.first - (wp.reached_now ? 1 : 0), tb, ts, row);
-    fixedwing_store(st, ist, N, i, s);
-    st[(int64_t)FW_DIST * N + i] = wp.new_dist;
-    ist[(int64_t)FI_STEP * N + i] = step_count;
-    ist[(int64_t)FI_NTARGETS * N + i] = wp.first;
-    reward[i] = rew;
-    term[i] = (s.flags & FLAG_TERM) ? 1 : 0;
-    trunc[i] = (s.flags & FLAG_TRUNC) ? 1 : 0;
-    if (info)
-      info[i] = (uint8_t)(((s.flags & FLAG_OOB) ? 1 : 0) | ((s.flags & FLAG_COLLISION) ? 2 : 0) | ((s.flags & FLAG_ENV_COMPLETE) ? 4 : 0) |
-                          (wp.first << 3));
-    if (tail) {
-      float* dst = obs + i * O;
-      for (int k = 0; k < O; ++k) dst[k] = row[k];
-    } else {
-      skip = false;
-      if (AUTORESET) {
-        bool done = (s.flags & (FLAG_TERM | FLAG_TRUNC)) != 0;
-        unsigned m = __ballot_sync(__activemask(), done);
-        if (done) {
-          int lane = threadIdx.x & 31;
-          int leader = __ffs(m) - 1;
-          int base = 0;
-          if (lane == leader) base = atomicAdd(cur_count, __popc(m));
-          base = __shfl_sync(m, base, leader);
-          cur_list[base + __popc(m & ((1u << lane) - 1u))] = (int32_t)i;
-        }
-      }
-    }
-  }
-  if (tail) return;
-  row_skip[slot] = skip ? 1 : 0;
-  __syncthreads();
-  int64_t rows = N - block_first;
-  if (rows > kBlock) rows = kBlock;
-  const int total = (int)rows * O;
-  float* dst = obs + block_first * O;
-  const int dr = kBlock / O, dc = kBlock - dr * O;
-  int r = threadIdx.x / O, c = threadIdx.x - r * O;
-  for (int j = threadIdx.x; j < total; j += kBlock) {
-    if (!row_skip[r]) dst[j] = smem[r * kWpObsStride + c];
-    r += dr; c += dc;
-    if (c >= O) { c -= O; ++r; }
-  }
+  tail_step<AUTORESET>(WpEnv<INJECT, RANDACT>{p, w, rng}, st, ist, actions, noise, obs, reward, term, trunc, info, start_pos, start_orn,
+                       prev_count, prev_list, cur_count, cur_list, next_count, spare, spare_copy, build, tail_blocks, step_seq, N);
 }
 
 template <bool INJECT>
@@ -438,65 +380,34 @@ int fw_observe(PfbContext* h, cudaStream_t s) {
   return 0;
 }
 
+// one launch of k_fwwp_step for tail_env_step / tail_env_reset
+static auto fwwp_launcher(PfbContext* h, float* actions, const float* noise) {
+  return [=](auto v, const TailLaunch& L) -> int {
+    using V = decltype(v);
+    k_fwwp_step<V::inject, V::randact, V::autoreset><<<L.grid, kBlock, 0, L.stream>>>(
+        h->fw, h->wp, h->rng, h->buf.state, h->buf.istate, actions, noise, h->buf.obs, h->buf.reward, h->buf.term, h->buf.trunc, h->buf.info,
+        h->buf.start_pos, h->buf.start_orn, L.prev_count, L.prev_list, L.cur_count, L.cur_list, L.next_count, L.spare, L.spare_copy, L.build,
+        L.tail_blocks, L.seq, h->n);
+    return 0;
+  };
+}
+
 int fw_env_reset(PfbContext* h, const uint8_t* mask, const float* noise, cudaStream_t s) {
   const uint32_t seq = 0x80000000u | (uint32_t)h->reset_seq++;
-  const int g = grid_for(h->n);
-  float* spare = h->env.autoreset ? h->d_spare : nullptr;
-  if (spare) {
-    SPARE_BEFORE_RESET(h, s);
-    if (!mask) CUDA_OK(cudaMemsetAsync(h->d_counters, 0, 4 * sizeof(int32_t), s));  // a full reset empties the autoreset queues
-    else if (pfb_drop_masked_done(h, mask, s)) return -1;  // a masked one takes its envs out of the pending done list
-  }
-  if (noise)
-    k_fwwp_reset<true><<<g, kBlock, 0, s>>>(h->fw, h->wp, h->rng, h->buf.state, h->buf.istate, h->buf.start_pos, h->buf.start_orn,
-                                            h->buf.reset_targets, mask, noise, h->buf.obs, seq, h->n);
-  else
-    k_fwwp_reset<false><<<g, kBlock, 0, s>>>(h->fw, h->wp, h->rng, h->buf.state, h->buf.istate, h->buf.start_pos, h->buf.start_orn,
-                                             h->buf.reset_targets, mask, nullptr, h->buf.obs, seq, h->n);
-  LAUNCH_CHECK(h);
-  if (spare) {  // every env gets a fresh spare: the step kernel in build mode over all envs, same stream
-    k_fwwp_step<false, false, true><<<g, kBlock, 0, s>>>(h->fw, h->wp, h->rng, h->buf.state, h->buf.istate, h->buf.setpoint, nullptr, h->buf.obs,
-                                                         h->buf.reward, h->buf.term, h->buf.trunc, h->buf.info, h->buf.start_pos, h->buf.start_orn,
-                                                         nullptr, nullptr, nullptr, nullptr, nullptr, spare, 0, 1, g, 0u, h->n);
-    LAUNCH_CHECK(h);
-  }
+  auto reset = [&](int g) -> int {
+    if (noise)
+      k_fwwp_reset<true><<<g, kBlock, 0, s>>>(h->fw, h->wp, h->rng, h->buf.state, h->buf.istate, h->buf.start_pos, h->buf.start_orn,
+                                              h->buf.reset_targets, mask, noise, h->buf.obs, seq, h->n);
+    else
+      k_fwwp_reset<false><<<g, kBlock, 0, s>>>(h->fw, h->wp, h->rng, h->buf.state, h->buf.istate, h->buf.start_pos, h->buf.start_orn,
+                                               h->buf.reset_targets, mask, nullptr, h->buf.obs, seq, h->n);
+    return 0;
+  };
+  if (tail_env_reset(h, mask, s, reset, fwwp_launcher(h, h->buf.setpoint, nullptr))) return -1;
   h->mode = 0;
   return 0;
 }
 
 int fw_env_step(PfbContext* h, float* actions, const float* noise, bool randact, cudaStream_t s) {
-  const StepPlan pl = plan_step(h);
-  float* spare = h->env.autoreset ? h->d_spare : nullptr;
-  const int spare_copy = (spare && !h->env.inline_reset) ? 1 : 0;
-  SPARE_BEFORE_STEP(h, s);
-  if (pl.prof) CUDA_OK(cudaEventRecord(h->prof_ev[2 * h->prof_n], s));
-#define WP_ARGS h->fw, h->wp, h->rng, h->buf.state, h->buf.istate, actions, noise, h->buf.obs, h->buf.reward, h->buf.term, \
-                h->buf.trunc, h->buf.info, h->buf.start_pos, h->buf.start_orn, pl.cnt_prev, pl.list_prev, pl.cnt_cur, pl.list_cur, \
-                pl.cnt_next, spare, spare_copy, 0, pl.tail, pl.seq, h->n
-  if (h->env.autoreset) {
-    if (noise) return fail("injected noise (parity mode) is only supported with autoreset = 0");
-    if (randact) k_fwwp_step<false, true, true><<<pl.grid, kBlock, 0, s>>>(WP_ARGS);
-    else k_fwwp_step<false, false, true><<<pl.grid, kBlock, 0, s>>>(WP_ARGS);
-  } else {
-    if (noise) k_fwwp_step<true, false, false><<<pl.grid, kBlock, 0, s>>>(WP_ARGS);
-    else if (randact) k_fwwp_step<false, true, false><<<pl.grid, kBlock, 0, s>>>(WP_ARGS);
-    else k_fwwp_step<false, false, false><<<pl.grid, kBlock, 0, s>>>(WP_ARGS);
-  }
-#undef WP_ARGS
-  LAUNCH_CHECK(h);
-  if (pl.prof) {
-    CUDA_OK(cudaEventRecord(h->prof_ev[2 * h->prof_n + 1], s));
-    h->prof_n += 1;
-  }
-  if (spare) {  // rebuild the spares this launch consumed, on the side stream, while the next launches run
-    SPARE_REBUILD_BEGIN(h, s);
-    k_fwwp_step<false, false, true><<<h->sm_count, kBlock, 0, h->side>>>(h->fw, h->wp, h->rng, h->buf.state, h->buf.istate, actions, nullptr,
-                                                                         h->buf.obs, h->buf.reward, h->buf.term, h->buf.trunc, h->buf.info,
-                                                                         h->buf.start_pos, h->buf.start_orn, pl.cnt_prev, pl.list_prev, pl.cnt_cur,
-                                                                         pl.list_cur, pl.cnt_next, spare, 0, 1, h->sm_count, pl.seq, h->n);
-    LAUNCH_CHECK(h);
-    SPARE_REBUILD_DONE(h);
-  }
-  h->step_seq += 1;
-  return 0;
+  return tail_env_step(h, noise, randact, s, fwwp_launcher(h, actions, noise));
 }

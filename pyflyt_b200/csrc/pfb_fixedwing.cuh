@@ -444,4 +444,13 @@ PFB_HD void fixedwing_drone_state(const FixedwingRegs& s, float* out12, float* a
   aux6[5] = s.thr;
 }
 
+// env.step() with random actions: uniform in [-1, 1]^4, drawn from env i's TAG_ACTION Philox stream (as quadx_random_action)
+template <class Rng>
+PFB_HD void fixedwing_random_action(const Rng& rng, int64_t i, uint32_t step_seq, float* act) {
+  uint64_t g = ((uint64_t)rng.env_offset_hi << 32 | rng.env_offset_lo) + (uint64_t)i;
+  U4 r = philox4x32_10(U4{(uint32_t)g, (uint32_t)(g >> 32), step_seq, (uint32_t)TAG_ACTION << 24}, rng.k0, rng.k1);
+  act[0] = 2.0f * u32_to_unit_open(r.x) - 1.0f; act[1] = 2.0f * u32_to_unit_open(r.y) - 1.0f;
+  act[2] = 2.0f * u32_to_unit_open(r.z) - 1.0f; act[3] = 2.0f * u32_to_unit_open(r.w) - 1.0f;
+}
+
 }  // namespace pfb

@@ -833,20 +833,6 @@ int pfb_drop_masked_done(PfbContext* h, const uint8_t* mask, cudaStream_t s) {
 // ---------------------------------------------------------------------------------------------------
 // host side
 // ---------------------------------------------------------------------------------------------------
-#define PFB_MODE_SWITCH(mode, BODY)                         \
-  switch (mode) {                                           \
-    case -1: { constexpr int MODE = -1; BODY; } break;      \
-    case 0: { constexpr int MODE = 0; BODY; } break;        \
-    case 1: { constexpr int MODE = 1; BODY; } break;        \
-    case 2: { constexpr int MODE = 2; BODY; } break;        \
-    case 3: { constexpr int MODE = 3; BODY; } break;        \
-    case 4: { constexpr int MODE = 4; BODY; } break;        \
-    case 5: { constexpr int MODE = 5; BODY; } break;        \
-    case 6: { constexpr int MODE = 6; BODY; } break;        \
-    case 7: { constexpr int MODE = 7; BODY; } break;        \
-    default: return fail("`mode` must be between -1 and 7, got %d", mode); \
-  }
-
 extern "C" {
 
 const char* pfb_last_error(void) { return g_err; }
@@ -945,8 +931,11 @@ int pfb_create(const PfbModel* model, const PfbEnvConfig* env, int64_t n_envs, i
     // spare post-reset states: env-major records (QuadX-Hover: two per env, double-buffered by episode parity, rebuilt by
     // builder CTAs inside the step launches; the other env kinds: one per env, rebuilt on a library-owned side stream)
     const bool hover = env->env_kind == PFB_ENV_QUADX_HOVER;
-    const size_t rec = env->env_kind == PFB_ENV_QUADX_WAYPOINTS ? (size_t)qwp_spare_rows()
-                       : (env->env_kind == PFB_ENV_DOGFIGHT ? (size_t)df_spare_rows() : (size_t)SP_ROWS * (hover ? kSpareBufs : 1));
+    size_t rec = (size_t)SP_ROWS * kSpareBufs;  // floats per env
+    if (env->env_kind == PFB_ENV_QUADX_WAYPOINTS) rec = (size_t)qwp_spare_rows();
+    else if (env->env_kind == PFB_ENV_FIXEDWING_WAYPOINTS) rec = (size_t)fw_spare_rows();
+    else if (env->env_kind == PFB_ENV_ROCKET_LANDING) rec = (size_t)rk_spare_rows();
+    else if (env->env_kind == PFB_ENV_DOGFIGHT) rec = (size_t)df_spare_rows();
     c->spare_bytes = rec * (size_t)n_envs * sizeof(float);
     CUDA_OK(cudaMalloc(&c->d_spare, c->spare_bytes));
     CUDA_OK(cudaMemset(c->d_spare, 0, c->spare_bytes));

@@ -33,7 +33,6 @@ struct InjectedNoise {  // parity tests: the CPU-drawn sequence, [substep][N]
 // Aviary steps at once — the env-step kernels call it before they touch the state they loaded, so that the ~400
 // integer instructions of the generator run in the shadow of the state loads instead of inside the physics loop.
 // set_dump(): optional [substep][N] buffer that receives every draw handed out (tests replay them through the oracle).
-enum { TAG_AVIARY = 0, TAG_ENV_STEP = 1, TAG_RESET = 2, TAG_ACTION = 3 };
 struct PhiloxNoise {
   uint32_t k0, k1, env_lo, env_hi, seq, tag;
   uint32_t step, pre;

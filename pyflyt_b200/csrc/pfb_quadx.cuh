@@ -899,4 +899,20 @@ PFB_HD void ma_hover_observation(const HoverParams& h, const QuadXRegs& s, const
   obs[o++] = sx; obs[o++] = sy; obs[o++] = sz;
 }
 
+// env.step() with random actions (quadx_base_env.py:79-102): uniform in the action box of the flight mode, drawn from env i's
+// TAG_ACTION Philox stream.  Rng: the kernels' RngParams (key k0, k1; global id of local env 0 in env_offset_hi:lo)
+template <int MODE, class Rng>
+PFB_HD void quadx_random_action(const Rng& rng, int64_t i, uint32_t step_seq, float* act) {
+  uint64_t g = ((uint64_t)rng.env_offset_hi << 32 | rng.env_offset_lo) + (uint64_t)i;
+  U4 r = philox4x32_10(U4{(uint32_t)g, (uint32_t)(g >> 32), step_seq, (uint32_t)TAG_ACTION << 24}, rng.k0, rng.k1);
+  const float pi = 3.14159265358979323846f;
+  if (MODE == -1) {
+    act[0] = 0.8f * u32_to_unit_open(r.x); act[1] = 0.8f * u32_to_unit_open(r.y);
+    act[2] = 0.8f * u32_to_unit_open(r.z); act[3] = 0.8f * u32_to_unit_open(r.w);
+  } else {
+    act[0] = pi * (2.0f * u32_to_unit_open(r.x) - 1.0f); act[1] = pi * (2.0f * u32_to_unit_open(r.y) - 1.0f);
+    act[2] = pi * (2.0f * u32_to_unit_open(r.z) - 1.0f); act[3] = 0.8f * u32_to_unit_open(r.w);
+  }
+}
+
 }  // namespace pfb

@@ -9,6 +9,7 @@
 // the grid reset the envs that finished on the previous launch (NEXT_STEP autoreset, inline warm-up).
 #include "pfb_noise.cuh"
 #include "pfb_quadx.cuh"
+#include "pfb_tail_step.cuh"
 
 using namespace pfb;
 
@@ -157,11 +158,106 @@ __device__ __forceinline__ void qw_reset_env(const QuadXParams& p, const QxWaypo
   (void)qw_update_distance(w, s, wp);  // end_reset -> compute_state
 }
 
-// ---- spare post-reset states: the QuadX-Hover reset pipeline (pfb_lib.cu, DESIGN.md §4) for this env.  A spare is an
-// env-major record of 128 floats: the QW_* state words INCLUDING the episode's targets, new_distance and yaw error, then:
-enum { QSP_POSE = QW_ROWS, QSP_VALID = QW_ROWS + 6, QSP_FLAGS = QW_ROWS + 7, QSP_EPISODE = QW_ROWS + 8, QSP_ROWS = 128 };
-static_assert(QW_ROWS + 9 <= QSP_ROWS, "spare record too small");
+// ---- spare post-reset states (pfb_tail_step.cuh): a record holds the QW_* state words INCLUDING the episode's targets,
+// new_distance and yaw error
+enum { QSP_ROWS = 128 };
 int qwp_spare_rows() { return QSP_ROWS; }
+
+// the QuadX-Waypoints env for tail_step (pfb_tail_step.cuh)
+template <int MODE, bool INJECT, bool RANDACT, class PS>
+struct QwEnv {
+  const PS& ps;
+  const HoverParams& h;
+  const QxWaypointParams& w;
+  const RngParams& rng;
+  using Regs = QuadXRegs;
+  struct Item {
+    const QuadXParams* p;
+    QwState wp;
+  };
+  static constexpr int kStateRows = QW_ROWS, kSpareRows = QSP_ROWS, kActions = 4, kObsStride = kQwObsStride;
+  __device__ __forceinline__ int obs_dim() const { return (h.angle_representation == 0 ? 20 : 21) + (w.use_yaw_targets ? 4 : 3) * w.num_targets; }
+  __device__ __forceinline__ bool pose_keyed() const { return true; }
+  __device__ __forceinline__ Item item(int64_t i) const {
+    Item x;
+    x.p = &qx_model(ps, i);
+    return x;
+  }
+  // a spare's targets are copied into the state rows: the episode starts at target 0
+  __device__ __forceinline__ void load_spare(const float* __restrict__ rec, float* __restrict__ st, int32_t* __restrict__ ist, int64_t N,
+                                             int64_t i, QuadXRegs& s, Item& x) const {
+    quadx_load<MODE>(rec, ist, N, i, s, 1, 0);
+#pragma unroll
+    for (int k = 0; k < 4; ++k) { s.sp[k] = 0.0f; s.pwm[k] = rec[QX_PWM + k]; }
+    float* tb = st + i;
+    for (int k = 0; k < 4 * w.num_targets; ++k) tb[(int64_t)(QW_TARGETS + k) * N] = rec[QW_TARGETS + k];
+    x.wp.first = 0;
+    x.wp.reached_now = false;
+    x.wp.new_dist = rec[QW_DIST];
+    x.wp.yaw_err = rec[QW_YAWERR];
+  }
+  // the targets go to the spare record being built, or to the state rows
+  __device__ __forceinline__ void reset(const float* pose, uint32_t nseq, float* __restrict__ rec, float* __restrict__ st, int64_t N, int64_t i,
+                                        QuadXRegs& s, Item& x) const {
+    qw_reset_env<MODE, false>(*x.p, w, rng, pose, nullptr, nullptr, nseq, N, i, rec ? rec : st + i, rec ? 1 : N, s, x.wp);
+  }
+  __device__ __forceinline__ void store_spare(float* __restrict__ rec, int32_t* __restrict__ ist, int64_t N, int64_t i, const QuadXRegs& s,
+                                              const Item& x) const {
+    quadx_store<MODE>(rec, ist, N, i, s, false, 1, 0);
+    rec[QW_DIST] = x.wp.new_dist;
+    rec[QW_YAWERR] = x.wp.yaw_err;
+  }
+  __device__ __forceinline__ void load(const float* __restrict__ st, const int32_t* __restrict__ ist, int64_t N, int64_t i, QuadXRegs& s) const {
+    quadx_load<MODE>(st, ist, N, i, s);
+  }
+  __device__ __forceinline__ void action(float* __restrict__ actions, int64_t i, uint32_t step_seq, float* act) const {
+    if (RANDACT) {
+      quadx_random_action<MODE>(rng, i, step_seq, act);
+      reinterpret_cast<float4*>(actions)[i] = make_float4(act[0], act[1], act[2], act[3]);
+    } else {
+      float4 a4 = __ldg(reinterpret_cast<const float4*>(actions) + i);
+      act[0] = a4.x; act[1] = a4.y; act[2] = a4.z; act[3] = a4.w;
+    }
+  }
+  __device__ __forceinline__ void step(const float* __restrict__ st, const int32_t* __restrict__ ist, const float* __restrict__ noise, int64_t N,
+                                       int64_t i, uint32_t step_seq, const float* act, QuadXRegs& s, Item& x, int& step_count, float& rew) const {
+#pragma unroll
+    for (int k = 0; k < 4; ++k) s.sp[k] = act[k];
+    step_count = ist[(int64_t)QI_STEP * N + i];
+    x.wp.first = ist[(int64_t)QWI_NTARGETS * N + i];
+    x.wp.reached_now = false;
+    x.wp.new_dist = st[(int64_t)QW_DIST * N + i];
+    x.wp.yaw_err = st[(int64_t)QW_YAWERR * N + i];
+    if (x.wp.first < w.num_targets) qw_load_target0(st + i, N, x.wp);
+    rew = -0.1f;
+    auto nz = make_noise<INJECT>(noise, N, i, rng, step_seq, TAG_ENV_STEP, qx_model0(ps).noise_loc, qx_model0(ps).ratio);
+#pragma unroll 1
+    for (int k = 0; k < w.env_step_ratio; ++k) {
+      if (s.flags & (FLAG_TERM | FLAG_TRUNC)) break;
+      quadx_aviary_step<MODE>(*x.p, s, nz);
+      float old = qw_update_distance(w, s, x.wp);
+      qw_term_trunc_reward(w, s, x.wp, old, step_count, rew, st + i, N);
+    }
+    step_count += 1;
+  }
+  // the reference builds the observation in compute_state, BEFORE compute_term_trunc_reward advances the target list
+  __device__ __forceinline__ void observe(const float* __restrict__ st, int64_t N, int64_t i, const float* act, const QuadXRegs& s, const Item& x,
+                                          float* row) const {
+    qw_observation(h, w, s, act, x.wp.first - (x.wp.reached_now ? 1 : 0), st + i, N, row);
+  }
+  __device__ __forceinline__ void store(float* __restrict__ st, int32_t* __restrict__ ist, int64_t N, int64_t i, const QuadXRegs& s, const Item& x,
+                                        int step_count) const {
+    quadx_store<MODE>(st, ist, N, i, s);
+    st[(int64_t)QW_DIST * N + i] = x.wp.new_dist;
+    st[(int64_t)QW_YAWERR * N + i] = x.wp.yaw_err;
+    ist[(int64_t)QI_STEP * N + i] = step_count;
+    ist[(int64_t)QWI_NTARGETS * N + i] = x.wp.first;
+  }
+  __device__ __forceinline__ uint8_t info(const QuadXRegs& s, const Item& x) const {
+    return (uint8_t)(((s.flags & FLAG_OOB) ? 1 : 0) | ((s.flags & FLAG_COLLISION) ? 2 : 0) | ((s.flags & FLAG_QW_COMPLETE) ? 4 : 0) |
+                     (x.wp.first << 3));
+  }
+};
 
 template <int MODE, bool INJECT, bool RANDACT, bool AUTORESET, class PS>
 __global__ void __launch_bounds__(kBlock, kMinBlocks)
@@ -172,165 +268,8 @@ __global__ void __launch_bounds__(kBlock, kMinBlocks)
                 const float* __restrict__ start_orn, const int32_t* __restrict__ prev_count, const int32_t* __restrict__ prev_list,
                 int32_t* __restrict__ cur_count, int32_t* __restrict__ cur_list, int32_t* __restrict__ next_count,
                 float* __restrict__ spare, int spare_copy, int build, int tail_blocks, uint32_t step_seq, int64_t N) {
-  __shared__ float smem[kBlock * kQwObsStride];
-  __shared__ uint8_t row_skip[kBlock];
-  const int O = (h.angle_representation == 0 ? 20 : 21) + (w.use_yaw_targets ? 4 : 3) * w.num_targets;
-  const bool tail = AUTORESET && (int)blockIdx.x < tail_blocks;
-  const int64_t block_first = tail ? 0 : (int64_t)((int)blockIdx.x - (AUTORESET ? tail_blocks : 0)) * kBlock;
-  int t, t_end, t_stride;
-  if (tail) {
-    if (blockIdx.x == 0 && threadIdx.x == 0 && !build) *next_count = 0;
-    t = blockIdx.x * kBlock + threadIdx.x;
-    t_end = prev_list ? *prev_count : (int)N;  // build mode after a user reset: every env
-    t_stride = tail_blocks * kBlock;
-  } else {
-    t = 0;
-    t_end = (block_first + threadIdx.x < N) ? 1 : 0;
-    t_stride = 1;
-  }
-  bool skip = true;
-  float* row = smem + threadIdx.x * kQwObsStride;
-#pragma unroll 1
-  for (; t < t_end; t += t_stride) {
-    const int64_t i = tail ? (prev_list ? (int64_t)prev_list[t] : (int64_t)t) : block_first + threadIdx.x;
-    const QuadXParams& p = qx_model(ps, i);
-    QuadXRegs s;
-    QwState wp;
-    float act[4] = {0.f, 0.f, 0.f, 0.f};
-    int step_count = 0;
-    float rew = 0.0f;
-    float* tb = st + i;  // where this env's targets live (field-major state rows, or the spare record being built)
-    int64_t ts = N;
-    if (tail) {
-      // env.reset(): normally a copy of the env's spare (state, targets, distances of the NEXT episode); build mode
-      // computes that spare; without a usable spare the warm-up runs inline with the same episode number
-      float* rec = spare ? spare + i * QSP_ROWS : nullptr;
-      uint32_t nseq = step_seq | 0x40000000u;
-      bool hit = false;
-      float pose[6];
-#pragma unroll
-      for (int k = 0; k < 3; ++k) { pose[k] = start_pos[3 * i + k]; pose[3 + k] = start_orn[3 * i + k]; }
-      if (rec) {
-        nseq = __float_as_uint(rec[QSP_EPISODE]) + (build ? 1u : 0u);
-        hit = !build && spare_copy && rec[QSP_VALID] != 0.0f;
-#pragma unroll
-        for (int k = 0; k < 6; ++k) hit = hit && (rec[QSP_POSE + k] == pose[k]);
-      }
-      if (hit) {
-        quadx_load<MODE>(rec, ist, N, i, s, 1, 0);
-        s.flags = __float_as_uint(rec[QSP_FLAGS]);
-#pragma unroll
-        for (int k = 0; k < 4; ++k) { s.sp[k] = 0.0f; s.pwm[k] = rec[QX_PWM + k]; }
-        for (int k = 0; k < 4 * w.num_targets; ++k) tb[(int64_t)(QW_TARGETS + k) * ts] = rec[QW_TARGETS + k];
-        wp.first = 0;
-        wp.reached_now = false;
-        wp.new_dist = rec[QW_DIST];
-        wp.yaw_err = rec[QW_YAWERR];
-      } else {
-        if (build) {
-          rec[QSP_VALID] = 0.0f;  // invalid until the warm-up below is stored
-#pragma unroll
-          for (int k = 0; k < 6; ++k) rec[QSP_POSE + k] = pose[k];
-          tb = rec;
-          ts = 1;
-        }
-        qw_reset_env<MODE, false>(p, w, rng, pose, nullptr, nullptr, nseq, N, i, tb, ts, s, wp);
-      }
-      if (build) {
-        quadx_store<MODE>(rec, ist, N, i, s, false, 1, 0);
-        rec[QW_DIST] = wp.new_dist;
-        rec[QW_YAWERR] = wp.yaw_err;
-        rec[QSP_FLAGS] = __uint_as_float(s.flags);
-        rec[QSP_EPISODE] = __uint_as_float(nseq);
-        rec[QSP_VALID] = 1.0f;
-        continue;
-      }
-      s.flags |= fresh_tag(step_seq);
-    } else {
-      quadx_load<MODE>(st, ist, N, i, s);
-      if (AUTORESET && (s.flags & (FLAG_TERM | FLAG_TRUNC | fresh_tag(step_seq)))) continue;  // a tail CTA owns this env
-      s.flags &= ~(uint32_t)FLAG_FRESH_ANY;
-      if (RANDACT) {  // uniform in the action box (quadx_base_env.py:79-102)
-        uint64_t g = ((uint64_t)rng.env_offset_hi << 32 | rng.env_offset_lo) + (uint64_t)i;
-        U4 r = philox4x32_10(U4{(uint32_t)g, (uint32_t)(g >> 32), step_seq, (uint32_t)TAG_ACTION << 24}, rng.k0, rng.k1);
-        const float pi = 3.14159265358979323846f;
-        if (MODE == -1) {
-          act[0] = 0.8f * u32_to_unit_open(r.x); act[1] = 0.8f * u32_to_unit_open(r.y);
-          act[2] = 0.8f * u32_to_unit_open(r.z); act[3] = 0.8f * u32_to_unit_open(r.w);
-        } else {
-          act[0] = pi * (2.0f * u32_to_unit_open(r.x) - 1.0f); act[1] = pi * (2.0f * u32_to_unit_open(r.y) - 1.0f);
-          act[2] = pi * (2.0f * u32_to_unit_open(r.z) - 1.0f); act[3] = 0.8f * u32_to_unit_open(r.w);
-        }
-        reinterpret_cast<float4*>(actions)[i] = make_float4(act[0], act[1], act[2], act[3]);
-      } else {
-        float4 a4 = __ldg(reinterpret_cast<const float4*>(actions) + i);
-        act[0] = a4.x; act[1] = a4.y; act[2] = a4.z; act[3] = a4.w;
-      }
-#pragma unroll
-      for (int k = 0; k < 4; ++k) s.sp[k] = act[k];
-      step_count = ist[(int64_t)QI_STEP * N + i];
-      wp.first = ist[(int64_t)QWI_NTARGETS * N + i];
-      wp.reached_now = false;
-      wp.new_dist = st[(int64_t)QW_DIST * N + i];
-      wp.yaw_err = st[(int64_t)QW_YAWERR * N + i];
-      if (wp.first < w.num_targets) qw_load_target0(tb, ts, wp);
-      rew = -0.1f;
-      auto nz = make_noise<INJECT>(noise, N, i, rng, step_seq, TAG_ENV_STEP, qx_model0(ps).noise_loc, qx_model0(ps).ratio);
-#pragma unroll 1
-      for (int k = 0; k < w.env_step_ratio; ++k) {
-        if (s.flags & (FLAG_TERM | FLAG_TRUNC)) break;
-        quadx_aviary_step<MODE>(p, s, nz);
-        float old = qw_update_distance(w, s, wp);
-        qw_term_trunc_reward(w, s, wp, old, step_count, rew, tb, ts);
-      }
-      step_count += 1;
-    }
-    // the reference builds the observation in compute_state, BEFORE compute_term_trunc_reward advances the target list
-    qw_observation(h, w, s, act, wp.first - (wp.reached_now ? 1 : 0), tb, ts, row);
-    quadx_store<MODE>(st, ist, N, i, s);
-    st[(int64_t)QW_DIST * N + i] = wp.new_dist;
-    st[(int64_t)QW_YAWERR * N + i] = wp.yaw_err;
-    ist[(int64_t)QI_STEP * N + i] = step_count;
-    ist[(int64_t)QWI_NTARGETS * N + i] = wp.first;
-    reward[i] = rew;
-    term[i] = (s.flags & FLAG_TERM) ? 1 : 0;
-    trunc[i] = (s.flags & FLAG_TRUNC) ? 1 : 0;
-    if (info)
-      info[i] = (uint8_t)(((s.flags & FLAG_OOB) ? 1 : 0) | ((s.flags & FLAG_COLLISION) ? 2 : 0) | ((s.flags & FLAG_QW_COMPLETE) ? 4 : 0) |
-                          (wp.first << 3));
-    if (tail) {
-      float* dst = obs + i * O;
-      for (int k = 0; k < O; ++k) dst[k] = row[k];
-    } else {
-      skip = false;
-      if (AUTORESET) {
-        bool done = (s.flags & (FLAG_TERM | FLAG_TRUNC)) != 0;
-        unsigned m = __ballot_sync(__activemask(), done);
-        if (done) {
-          int lane = threadIdx.x & 31;
-          int leader = __ffs(m) - 1;
-          int base = 0;
-          if (lane == leader) base = atomicAdd(cur_count, __popc(m));
-          base = __shfl_sync(m, base, leader);
-          cur_list[base + __popc(m & ((1u << lane) - 1u))] = (int32_t)i;
-        }
-      }
-    }
-  }
-  if (tail) return;
-  row_skip[threadIdx.x] = skip ? 1 : 0;
-  __syncthreads();
-  int64_t rows = N - block_first;
-  if (rows > kBlock) rows = kBlock;
-  const int total = (int)rows * O;
-  float* dst = obs + block_first * O;
-  const int dr = kBlock / O, dc = kBlock - dr * O;
-  int r = threadIdx.x / O, c = threadIdx.x - r * O;
-  for (int j = threadIdx.x; j < total; j += kBlock) {
-    if (!row_skip[r]) dst[j] = smem[r * kQwObsStride + c];
-    r += dr; c += dc;
-    if (c >= O) { c -= O; ++r; }
-  }
+  tail_step<AUTORESET>(QwEnv<MODE, INJECT, RANDACT, PS>{ps, h, w, rng}, st, ist, actions, noise, obs, reward, term, trunc, info, start_pos,
+                       start_orn, prev_count, prev_list, cur_count, cur_list, next_count, spare, spare_copy, build, tail_blocks, step_seq, N);
 }
 
 template <int MODE, bool INJECT, class PS>
@@ -364,81 +303,35 @@ __global__ void __launch_bounds__(kBlock)
 // ---------------------------------------------------------------------------------------------------
 // launchers
 // ---------------------------------------------------------------------------------------------------
-#define QW_MODE_SWITCH(mode, BODY)                          \
-  switch (mode) {                                           \
-    case -1: { constexpr int MODE = -1; BODY; } break;      \
-    case 0: { constexpr int MODE = 0; BODY; } break;        \
-    case 1: { constexpr int MODE = 1; BODY; } break;        \
-    case 2: { constexpr int MODE = 2; BODY; } break;        \
-    case 3: { constexpr int MODE = 3; BODY; } break;        \
-    case 4: { constexpr int MODE = 4; BODY; } break;        \
-    case 5: { constexpr int MODE = 5; BODY; } break;        \
-    case 6: { constexpr int MODE = 6; BODY; } break;        \
-    case 7: { constexpr int MODE = 7; BODY; } break;        \
-    default: return fail("`mode` must be between -1 and 7, got %d", mode); \
-  }
+// one launch of k_qxwp_step for tail_env_step / tail_env_reset
+static auto qwp_launcher(PfbContext* h, float* actions, const float* noise) {
+  return [=](auto v, const TailLaunch& L) -> int {
+    using V = decltype(v);
+    const int mode = h->hover.flight_mode;
+    QX_PARAMS_SWITCH(h, PFB_MODE_SWITCH(mode, (k_qxwp_step<MODE, V::inject, V::randact, V::autoreset, PS><<<L.grid, kBlock, 0, L.stream>>>(
+                                                   ps, h->hover, h->qwp, h->rng, h->buf.state, h->buf.istate, actions, noise, h->buf.obs, h->buf.reward,
+                                                   h->buf.term, h->buf.trunc, h->buf.info, h->buf.start_pos, h->buf.start_orn, L.prev_count, L.prev_list,
+                                                   L.cur_count, L.cur_list, L.next_count, L.spare, L.spare_copy, L.build, L.tail_blocks, L.seq, h->n))));
+    return 0;
+  };
+}
 
 int qwp_env_reset(PfbContext* h, const uint8_t* mask, const float* noise, cudaStream_t s) {
   const uint32_t seq = 0x80000000u | (uint32_t)h->reset_seq++;
   const int mode = h->hover.flight_mode;
-  const int g = grid_for(h->n);
-  float* spare = h->env.autoreset ? h->d_spare : nullptr;
-  if (spare) {
-    SPARE_BEFORE_RESET(h, s);
-    if (!mask) CUDA_OK(cudaMemsetAsync(h->d_counters, 0, 4 * sizeof(int32_t), s));  // a full reset empties the autoreset queues
-    else if (pfb_drop_masked_done(h, mask, s)) return -1;  // a masked one takes its envs out of the pending done list
-  }
+  auto reset = [&](int g) -> int {
 #define QR_ARGS ps, h->hover, h->qwp, h->rng, h->buf.state, h->buf.istate, h->buf.start_pos, h->buf.start_orn, h->buf.reset_targets, mask, noise, \
                 h->buf.obs, seq, h->n
-  if (noise) { QX_PARAMS_SWITCH(h, QW_MODE_SWITCH(mode, (k_qxwp_reset<MODE, true, PS><<<g, kBlock, 0, s>>>(QR_ARGS)))); }
-  else { QX_PARAMS_SWITCH(h, QW_MODE_SWITCH(mode, (k_qxwp_reset<MODE, false, PS><<<g, kBlock, 0, s>>>(QR_ARGS)))); }
+    if (noise) { QX_PARAMS_SWITCH(h, PFB_MODE_SWITCH(mode, (k_qxwp_reset<MODE, true, PS><<<g, kBlock, 0, s>>>(QR_ARGS)))); }
+    else { QX_PARAMS_SWITCH(h, PFB_MODE_SWITCH(mode, (k_qxwp_reset<MODE, false, PS><<<g, kBlock, 0, s>>>(QR_ARGS)))); }
 #undef QR_ARGS
-  LAUNCH_CHECK(h);
-  if (spare) {  // every env gets a fresh spare: the step kernel in build mode over all envs, same stream
-    QX_PARAMS_SWITCH(h, QW_MODE_SWITCH(mode, (k_qxwp_step<MODE, false, false, true, PS><<<g, kBlock, 0, s>>>(
-                                                  ps, h->hover, h->qwp, h->rng, h->buf.state, h->buf.istate, h->buf.setpoint, nullptr, h->buf.obs,
-                                                  h->buf.reward, h->buf.term, h->buf.trunc, h->buf.info, h->buf.start_pos, h->buf.start_orn, nullptr,
-                                                  nullptr, nullptr, nullptr, nullptr, spare, 0, 1, g, 0u, h->n))));
-    LAUNCH_CHECK(h);
-  }
+    return 0;
+  };
+  if (tail_env_reset(h, mask, s, reset, qwp_launcher(h, h->buf.setpoint, nullptr))) return -1;
   h->mode = mode;
   return 0;
 }
 
 int qwp_env_step(PfbContext* h, float* actions, const float* noise, bool randact, cudaStream_t s) {
-  StepPlan pl = plan_step(h);
-  const int mode = h->hover.flight_mode;
-  float* spare = h->env.autoreset ? h->d_spare : nullptr;
-  const int spare_copy = (spare && !h->env.inline_reset) ? 1 : 0;
-  SPARE_BEFORE_STEP(h, s);
-  if (pl.prof) CUDA_OK(cudaEventRecord(h->prof_ev[2 * h->prof_n], s));
-#define QS_ARGS ps, h->hover, h->qwp, h->rng, h->buf.state, h->buf.istate, actions, noise, h->buf.obs, h->buf.reward, h->buf.term,     \
-                h->buf.trunc, h->buf.info, h->buf.start_pos, h->buf.start_orn, pl.cnt_prev, pl.list_prev, pl.cnt_cur, pl.list_cur, \
-                pl.cnt_next, spare, spare_copy, 0, pl.tail, pl.seq, h->n
-  if (h->env.autoreset) {
-    if (noise) return fail("injected noise (parity mode) is only supported with autoreset = 0");
-    if (randact) { QX_PARAMS_SWITCH(h, QW_MODE_SWITCH(mode, (k_qxwp_step<MODE, false, true, true, PS><<<pl.grid, kBlock, 0, s>>>(QS_ARGS)))); }
-    else { QX_PARAMS_SWITCH(h, QW_MODE_SWITCH(mode, (k_qxwp_step<MODE, false, false, true, PS><<<pl.grid, kBlock, 0, s>>>(QS_ARGS)))); }
-  } else {
-    if (noise) { QX_PARAMS_SWITCH(h, QW_MODE_SWITCH(mode, (k_qxwp_step<MODE, true, false, false, PS><<<pl.grid, kBlock, 0, s>>>(QS_ARGS)))); }
-    else if (randact) { QX_PARAMS_SWITCH(h, QW_MODE_SWITCH(mode, (k_qxwp_step<MODE, false, true, false, PS><<<pl.grid, kBlock, 0, s>>>(QS_ARGS)))); }
-    else { QX_PARAMS_SWITCH(h, QW_MODE_SWITCH(mode, (k_qxwp_step<MODE, false, false, false, PS><<<pl.grid, kBlock, 0, s>>>(QS_ARGS)))); }
-  }
-#undef QS_ARGS
-  LAUNCH_CHECK(h);
-  if (pl.prof) {
-    CUDA_OK(cudaEventRecord(h->prof_ev[2 * h->prof_n + 1], s));
-    h->prof_n += 1;
-  }
-  if (spare) {  // rebuild the spares this launch consumed, on the side stream, while the next launches run
-    SPARE_REBUILD_BEGIN(h, s);
-    QX_PARAMS_SWITCH(h, QW_MODE_SWITCH(mode, (k_qxwp_step<MODE, false, false, true, PS><<<h->sm_count, kBlock, 0, h->side>>>(
-                                                  ps, h->hover, h->qwp, h->rng, h->buf.state, h->buf.istate, actions, nullptr, h->buf.obs, h->buf.reward,
-                                                  h->buf.term, h->buf.trunc, h->buf.info, h->buf.start_pos, h->buf.start_orn, pl.cnt_prev, pl.list_prev,
-                                                  pl.cnt_cur, pl.list_cur, pl.cnt_next, spare, 0, 1, h->sm_count, pl.seq, h->n))));
-    LAUNCH_CHECK(h);
-    SPARE_REBUILD_DONE(h);
-  }
-  h->step_seq += 1;
-  return 0;
+  return tail_env_step(h, noise, randact, s, qwp_launcher(h, actions, noise));
 }

@@ -5,6 +5,7 @@
 #include "pfb_context.h"
 #include "pfb_noise.cuh"
 #include "pfb_rocket_host.h"
+#include "pfb_tail_step.cuh"
 
 using namespace pfb;
 
@@ -196,10 +197,89 @@ static __device__ __noinline__ RocketRegs landing_reset_env_shared(const RocketP
 // whole register file instead of spilling (contact response + wind + variable-mass composite: ~170 live registers)
 constexpr int kLandBlocks = 8;
 
-// ---- spare post-reset states: the QuadX-Hover reset pipeline (pfb_lib.cu, DESIGN.md §4) for this env.  A spare is an
-// env-major record of 64 floats: the RK_* state words, then:
-enum { LSP_POSE = RK_ROWS, LSP_VALID = RK_ROWS + 6, LSP_FLAGS = RK_ROWS + 7, LSP_EPISODE = RK_ROWS + 8, LSP_ROWS = 64 };
-static_assert(RK_ROWS + 9 <= LSP_ROWS, "spare record too small");
+// ---- spare post-reset states (pfb_tail_step.cuh): a record holds the RK_* state words
+enum { LSP_ROWS = 64 };
+int rk_spare_rows() { return LSP_ROWS; }
+
+// the Rocket-Landing env for tail_step (pfb_tail_step.cuh)
+template <bool INJECT, bool RANDACT>
+struct LandEnv {
+  const RocketParams& p;
+  const LandingParams& l;
+  const RngParams& rng;
+  using Regs = RocketRegs;
+  struct Item {
+    bool pad_obs;  // landing_pad_contact as the observation reports it
+  };
+  static constexpr int kStateRows = RK_ROWS, kSpareRows = LSP_ROWS, kActions = 7, kObsStride = kLandObsStride;
+  __device__ __forceinline__ int obs_dim() const { return (l.angle_representation == 0 ? 12 : 13) + 17; }
+  __device__ __forceinline__ bool pose_keyed() const { return !l.randomize_drop; }  // a randomised drop does not read the start pose
+  __device__ __forceinline__ Item item(int64_t) const { return Item{false}; }
+  __device__ __forceinline__ void load_spare(const float* __restrict__ rec, float* __restrict__, int32_t* __restrict__ ist, int64_t N, int64_t i,
+                                             RocketRegs& s, Item&) const {
+    rocket_load(rec, ist, N, i, s, 1, 0);
+  }
+  // the episode number also keys a randomised drop
+  __device__ __forceinline__ void reset(const float* pose, uint32_t nseq, float* __restrict__, float* __restrict__, int64_t N, int64_t i,
+                                        RocketRegs& s, Item&) const {
+    s = landing_reset_env_shared(&p, &l, &rng, pose[0], pose[1], pose[2], pose[3], pose[4], pose[5], nseq, l.randomize_drop, N, i);
+  }
+  __device__ __forceinline__ void store_spare(float* __restrict__ rec, int32_t* __restrict__ ist, int64_t N, int64_t i, const RocketRegs& s,
+                                              const Item&) const {
+    rocket_store(rec, ist, N, i, s, false, 1, 0);
+  }
+  __device__ __forceinline__ void load(const float* __restrict__ st, const int32_t* __restrict__ ist, int64_t N, int64_t i, RocketRegs& s) const {
+    rocket_load(st, ist, N, i, s);
+  }
+  __device__ __forceinline__ void action(float* __restrict__ actions, int64_t i, uint32_t step_seq, float* act) const {
+    if (RANDACT) {  // rocket_base_env.py:82-107: [-1,1]^3, ignition {0..1}, throttle [0,1], gimbal [-1,1]^2
+      uint64_t g = ((uint64_t)rng.env_offset_hi << 32 | rng.env_offset_lo) + (uint64_t)i;
+      U4 a = philox4x32_10(U4{(uint32_t)g, (uint32_t)(g >> 32), step_seq, (uint32_t)TAG_ACTION << 24}, rng.k0, rng.k1);
+      U4 b = philox4x32_10(U4{(uint32_t)g, (uint32_t)(g >> 32), step_seq, ((uint32_t)TAG_ACTION << 24) | 1u}, rng.k0, rng.k1);
+      act[0] = 2.0f * u32_to_unit_open(a.x) - 1.0f; act[1] = 2.0f * u32_to_unit_open(a.y) - 1.0f; act[2] = 2.0f * u32_to_unit_open(a.z) - 1.0f;
+      act[3] = u32_to_unit_open(a.w); act[4] = u32_to_unit_open(b.x);
+      act[5] = 2.0f * u32_to_unit_open(b.y) - 1.0f; act[6] = 2.0f * u32_to_unit_open(b.z) - 1.0f;
+      for (int k = 0; k < 7; ++k) actions[7 * i + k] = act[k];
+    } else {
+#pragma unroll
+      for (int k = 0; k < 7; ++k) act[k] = __ldg(actions + 7 * i + k);
+    }
+  }
+  __device__ __forceinline__ void step(const float* __restrict__, const int32_t* __restrict__ ist, const float* __restrict__ noise, int64_t N,
+                                       int64_t i, uint32_t step_seq, const float* act, RocketRegs& s, Item& x, int& step_count, float& rew) const {
+#pragma unroll
+    for (int k = 0; k < 7; ++k) s.sp[k] = act[k];
+    step_count = ist[(int64_t)RI_STEP * N + i];
+    auto nz = make_noise<INJECT>(noise, N, i, rng, step_seq, TAG_ENV_STEP, p.noise_loc, p.ratio);
+    LandingPrev prev, cur;
+    landing_snapshot(s, cur);  // the values of the last compute_state are the state we just loaded
+    x.pad_obs = (s.flags & FLAG_PAD_OBS) != 0;
+#pragma unroll 1
+    for (int k = 0; k < l.env_step_ratio; ++k) {
+      if (s.flags & (FLAG_TERM | FLAG_TRUNC)) break;
+      rocket_aviary_step(p, s, nz, true);
+      prev = cur;
+      landing_snapshot(s, cur);
+      // compute_state runs BEFORE compute_term_trunc_reward: the observation carries landing_pad_contact
+      // as it stood after the previous Aviary step
+      x.pad_obs = (s.flags & FLAG_PAD_OBS) != 0;
+      landing_term_trunc_reward(l, s, prev, cur, step_count, rew);
+    }
+    step_count += 1;
+  }
+  __device__ __forceinline__ void observe(const float* __restrict__, int64_t, int64_t, const float* act, const RocketRegs& s, const Item& x,
+                                          float* row) const {
+    landing_observation(l, s, act, x.pad_obs, row);
+  }
+  __device__ __forceinline__ void store(float* __restrict__ st, int32_t* __restrict__ ist, int64_t N, int64_t i, const RocketRegs& s, const Item&,
+                                        int step_count) const {
+    rocket_store(st, ist, N, i, s);
+    ist[(int64_t)RI_STEP * N + i] = step_count;
+  }
+  __device__ __forceinline__ uint8_t info(const RocketRegs& s, const Item&) const {
+    return (uint8_t)(((s.flags & FLAG_OOB) ? 1 : 0) | ((s.flags & FLAG_COLLISION) ? 2 : 0) | ((s.flags & FLAG_ENV_COMPLETE) ? 4 : 0));
+  }
+};
 
 template <bool INJECT, bool RANDACT, bool AUTORESET>
 __global__ void __launch_bounds__(kBlock, kLandBlocks)
@@ -210,144 +290,8 @@ __global__ void __launch_bounds__(kBlock, kLandBlocks)
                 const int32_t* __restrict__ prev_count, const int32_t* __restrict__ prev_list, int32_t* __restrict__ cur_count,
                 int32_t* __restrict__ cur_list, int32_t* __restrict__ next_count, float* __restrict__ spare, int spare_copy, int build,
                 int tail_blocks, uint32_t step_seq, int64_t N) {
-  __shared__ float smem[kBlock * kLandObsStride];
-  __shared__ uint8_t row_skip[kBlock];
-  const int O = (l.angle_representation == 0 ? 12 : 13) + 17;
-  const bool tail = AUTORESET && (int)blockIdx.x < tail_blocks;
-  const int64_t block_first = tail ? 0 : (int64_t)((int)blockIdx.x - (AUTORESET ? tail_blocks : 0)) * kBlock;
-  int t, t_end, t_stride;
-  if (tail) {
-    if (blockIdx.x == 0 && threadIdx.x == 0 && !build) *next_count = 0;
-    t = blockIdx.x * kBlock + threadIdx.x;
-    t_end = prev_list ? *prev_count : (int)N;  // build mode after a user reset: every env
-    t_stride = tail_blocks * kBlock;
-  } else {
-    t = 0;
-    t_end = (block_first + threadIdx.x < N) ? 1 : 0;
-    t_stride = 1;
-  }
-  bool skip = true;
-  float* row = smem + threadIdx.x * kLandObsStride;
-#pragma unroll 1
-  for (; t < t_end; t += t_stride) {
-    const int64_t i = tail ? (prev_list ? (int64_t)prev_list[t] : (int64_t)t) : block_first + threadIdx.x;
-    RocketRegs s;
-    float act[7] = {0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f};
-    int step_count = 0;
-    float rew = 0.0f;
-    bool pad_obs = false;
-    if (tail) {
-      // env.reset(): normally a copy of the env's spare; build mode computes that spare; without a usable spare the
-      // warm-up runs inline with the same episode number (which also keys a randomised drop)
-      float* rec = spare ? spare + i * LSP_ROWS : nullptr;
-      uint32_t nseq = step_seq | 0x40000000u;
-      bool hit = false;
-      float pose[6];
-#pragma unroll
-      for (int k = 0; k < 3; ++k) { pose[k] = start_pos[3 * i + k]; pose[3 + k] = start_orn[3 * i + k]; }
-      if (rec) {
-        nseq = __float_as_uint(rec[LSP_EPISODE]) + (build ? 1u : 0u);
-        hit = !build && spare_copy && rec[LSP_VALID] != 0.0f;
-        if (!l.randomize_drop) {  // a randomised drop does not read the start pose
-#pragma unroll
-          for (int k = 0; k < 6; ++k) hit = hit && (rec[LSP_POSE + k] == pose[k]);
-        }
-      }
-      if (hit) {
-        rocket_load(rec, ist, N, i, s, 1, 0);
-        s.flags = __float_as_uint(rec[LSP_FLAGS]);
-      } else {
-        if (build) {
-          rec[LSP_VALID] = 0.0f;  // invalid until the warm-up below is stored
-#pragma unroll
-          for (int k = 0; k < 6; ++k) rec[LSP_POSE + k] = pose[k];
-        }
-        s = landing_reset_env_shared(&p, &l, &rng, pose[0], pose[1], pose[2], pose[3], pose[4], pose[5], nseq, l.randomize_drop, N, i);
-      }
-      if (build) {
-        rocket_store(rec, ist, N, i, s, false, 1, 0);
-        rec[LSP_FLAGS] = __uint_as_float(s.flags);
-        rec[LSP_EPISODE] = __uint_as_float(nseq);
-        rec[LSP_VALID] = 1.0f;
-        continue;
-      }
-      s.flags |= fresh_tag(step_seq);
-    } else {
-      rocket_load(st, ist, N, i, s);
-      if (AUTORESET && (s.flags & (FLAG_TERM | FLAG_TRUNC | fresh_tag(step_seq)))) continue;  // a tail CTA owns this env
-      s.flags &= ~(uint32_t)FLAG_FRESH_ANY;
-      if (RANDACT) {  // rocket_base_env.py:82-107: [-1,1]^3, ignition {0..1}, throttle [0,1], gimbal [-1,1]^2
-        uint64_t g = ((uint64_t)rng.env_offset_hi << 32 | rng.env_offset_lo) + (uint64_t)i;
-        U4 a = philox4x32_10(U4{(uint32_t)g, (uint32_t)(g >> 32), step_seq, (uint32_t)TAG_ACTION << 24}, rng.k0, rng.k1);
-        U4 b = philox4x32_10(U4{(uint32_t)g, (uint32_t)(g >> 32), step_seq, ((uint32_t)TAG_ACTION << 24) | 1u}, rng.k0, rng.k1);
-        act[0] = 2.0f * u32_to_unit_open(a.x) - 1.0f; act[1] = 2.0f * u32_to_unit_open(a.y) - 1.0f; act[2] = 2.0f * u32_to_unit_open(a.z) - 1.0f;
-        act[3] = u32_to_unit_open(a.w); act[4] = u32_to_unit_open(b.x);
-        act[5] = 2.0f * u32_to_unit_open(b.y) - 1.0f; act[6] = 2.0f * u32_to_unit_open(b.z) - 1.0f;
-        for (int k = 0; k < 7; ++k) actions[7 * i + k] = act[k];
-      } else {
-#pragma unroll
-        for (int k = 0; k < 7; ++k) act[k] = __ldg(actions + 7 * i + k);
-      }
-#pragma unroll
-      for (int k = 0; k < 7; ++k) s.sp[k] = act[k];
-      step_count = ist[(int64_t)RI_STEP * N + i];
-      auto nz = make_noise<INJECT>(noise, N, i, rng, step_seq, TAG_ENV_STEP, p.noise_loc, p.ratio);
-      LandingPrev prev, cur;
-      landing_snapshot(s, cur);  // the values of the last compute_state are the state we just loaded
-      pad_obs = (s.flags & FLAG_PAD_OBS) != 0;
-#pragma unroll 1
-      for (int k = 0; k < l.env_step_ratio; ++k) {
-        if (s.flags & (FLAG_TERM | FLAG_TRUNC)) break;
-        rocket_aviary_step(p, s, nz, true);
-        prev = cur;
-        landing_snapshot(s, cur);
-        // compute_state runs BEFORE compute_term_trunc_reward: the observation carries landing_pad_contact
-        // as it stood after the previous Aviary step
-        pad_obs = (s.flags & FLAG_PAD_OBS) != 0;
-        landing_term_trunc_reward(l, s, prev, cur, step_count, rew);
-      }
-      step_count += 1;
-    }
-    landing_observation(l, s, act, pad_obs, row);
-    rocket_store(st, ist, N, i, s);
-    ist[(int64_t)RI_STEP * N + i] = step_count;
-    reward[i] = rew;
-    term[i] = (s.flags & FLAG_TERM) ? 1 : 0;
-    trunc[i] = (s.flags & FLAG_TRUNC) ? 1 : 0;
-    if (info) info[i] = (uint8_t)(((s.flags & FLAG_OOB) ? 1 : 0) | ((s.flags & FLAG_COLLISION) ? 2 : 0) | ((s.flags & FLAG_ENV_COMPLETE) ? 4 : 0));
-    if (tail) {
-      float* dst = obs + i * O;
-      for (int k = 0; k < O; ++k) dst[k] = row[k];
-    } else {
-      skip = false;
-      if (AUTORESET) {
-        bool done = (s.flags & (FLAG_TERM | FLAG_TRUNC)) != 0;
-        unsigned m = __ballot_sync(__activemask(), done);
-        if (done) {
-          int lane = threadIdx.x & 31;
-          int leader = __ffs(m) - 1;
-          int base = 0;
-          if (lane == leader) base = atomicAdd(cur_count, __popc(m));
-          base = __shfl_sync(m, base, leader);
-          cur_list[base + __popc(m & ((1u << lane) - 1u))] = (int32_t)i;
-        }
-      }
-    }
-  }
-  if (tail) return;
-  row_skip[threadIdx.x] = skip ? 1 : 0;
-  __syncthreads();
-  int64_t rows = N - block_first;
-  if (rows > kBlock) rows = kBlock;
-  const int total = (int)rows * O;
-  float* dst = obs + block_first * O;
-  const int dr = kBlock / O, dc = kBlock - dr * O;
-  int r = threadIdx.x / O, c = threadIdx.x - r * O;
-  for (int j = threadIdx.x; j < total; j += kBlock) {
-    if (!row_skip[r]) dst[j] = smem[r * kLandObsStride + c];
-    r += dr; c += dc;
-    if (c >= O) { c -= O; ++r; }
-  }
+  tail_step<AUTORESET>(LandEnv<INJECT, RANDACT>{p, l, rng}, st, ist, actions, noise, obs, reward, term, trunc, info, start_pos, start_orn,
+                       prev_count, prev_list, cur_count, cur_list, next_count, spare, spare_copy, build, tail_blocks, step_seq, N);
 }
 
 template <bool INJECT>
@@ -412,67 +356,36 @@ int rk_observe(PfbContext* h, cudaStream_t s) {
   return 0;
 }
 
+// one launch of k_land_step for tail_env_step / tail_env_reset
+static auto land_launcher(PfbContext* h, float* actions, const float* noise) {
+  return [=](auto v, const TailLaunch& L) -> int {
+    using V = decltype(v);
+    k_land_step<V::inject, V::randact, V::autoreset><<<L.grid, kBlock, 0, L.stream>>>(
+        h->rk, h->land, h->rng, h->buf.state, h->buf.istate, actions, noise, h->buf.obs, h->buf.reward, h->buf.term, h->buf.trunc, h->buf.info,
+        h->buf.start_pos, h->buf.start_orn, L.prev_count, L.prev_list, L.cur_count, L.cur_list, L.next_count, L.spare, L.spare_copy, L.build,
+        L.tail_blocks, L.seq, h->n);
+    return 0;
+  };
+}
+
 int rk_env_reset(PfbContext* h, const uint8_t* mask, const float* noise, cudaStream_t s) {
   const uint32_t seq = 0x80000000u | (uint32_t)h->reset_seq++;
-  const int g = grid_for(h->n);
   // an explicit env.reset() honours the bound start_pos / start_orn unless randomize_drop is configured
   const int randomize = h->land.randomize_drop;
-  float* spare = h->env.autoreset ? h->d_spare : nullptr;
-  if (spare) {
-    SPARE_BEFORE_RESET(h, s);
-    if (!mask) CUDA_OK(cudaMemsetAsync(h->d_counters, 0, 4 * sizeof(int32_t), s));  // a full reset empties the autoreset queues
-    else if (pfb_drop_masked_done(h, mask, s)) return -1;  // a masked one takes its envs out of the pending done list
-  }
-  if (noise)
-    k_land_reset<true><<<g, kBlock, 0, s>>>(h->rk, h->land, h->rng, h->buf.state, h->buf.istate, h->buf.start_pos, h->buf.start_orn, mask, noise,
-                                            h->buf.obs, seq, randomize, h->n);
-  else
-    k_land_reset<false><<<g, kBlock, 0, s>>>(h->rk, h->land, h->rng, h->buf.state, h->buf.istate, h->buf.start_pos, h->buf.start_orn, mask,
-                                             nullptr, h->buf.obs, seq, randomize, h->n);
-  LAUNCH_CHECK(h);
-  if (spare) {  // every env gets a fresh spare: the step kernel in build mode over all envs, same stream
-    k_land_step<false, false, true><<<g, kBlock, 0, s>>>(h->rk, h->land, h->rng, h->buf.state, h->buf.istate, h->buf.setpoint, nullptr, h->buf.obs,
-                                                         h->buf.reward, h->buf.term, h->buf.trunc, h->buf.info, h->buf.start_pos, h->buf.start_orn,
-                                                         nullptr, nullptr, nullptr, nullptr, nullptr, spare, 0, 1, g, 0u, h->n);
-    LAUNCH_CHECK(h);
-  }
+  auto reset = [&](int g) -> int {
+    if (noise)
+      k_land_reset<true><<<g, kBlock, 0, s>>>(h->rk, h->land, h->rng, h->buf.state, h->buf.istate, h->buf.start_pos, h->buf.start_orn, mask, noise,
+                                              h->buf.obs, seq, randomize, h->n);
+    else
+      k_land_reset<false><<<g, kBlock, 0, s>>>(h->rk, h->land, h->rng, h->buf.state, h->buf.istate, h->buf.start_pos, h->buf.start_orn, mask,
+                                               nullptr, h->buf.obs, seq, randomize, h->n);
+    return 0;
+  };
+  if (tail_env_reset(h, mask, s, reset, land_launcher(h, h->buf.setpoint, nullptr))) return -1;
   h->mode = 0;
   return 0;
 }
 
 int rk_env_step(PfbContext* h, float* actions, const float* noise, bool randact, cudaStream_t s) {
-  StepPlan pl = plan_step(h);
-  float* spare = h->env.autoreset ? h->d_spare : nullptr;
-  const int spare_copy = (spare && !h->env.inline_reset) ? 1 : 0;
-  SPARE_BEFORE_STEP(h, s);
-  if (pl.prof) CUDA_OK(cudaEventRecord(h->prof_ev[2 * h->prof_n], s));
-#define LD_ARGS h->rk, h->land, h->rng, h->buf.state, h->buf.istate, actions, noise, h->buf.obs, h->buf.reward, h->buf.term, h->buf.trunc, \
-                h->buf.info, h->buf.start_pos, h->buf.start_orn, pl.cnt_prev, pl.list_prev, pl.cnt_cur, pl.list_cur, pl.cnt_next, spare, \
-                spare_copy, 0, pl.tail, pl.seq, h->n
-  if (h->env.autoreset) {
-    if (noise) return fail("injected noise (parity mode) is only supported with autoreset = 0");
-    if (randact) k_land_step<false, true, true><<<pl.grid, kBlock, 0, s>>>(LD_ARGS);
-    else k_land_step<false, false, true><<<pl.grid, kBlock, 0, s>>>(LD_ARGS);
-  } else {
-    if (noise) k_land_step<true, false, false><<<pl.grid, kBlock, 0, s>>>(LD_ARGS);
-    else if (randact) k_land_step<false, true, false><<<pl.grid, kBlock, 0, s>>>(LD_ARGS);
-    else k_land_step<false, false, false><<<pl.grid, kBlock, 0, s>>>(LD_ARGS);
-  }
-#undef LD_ARGS
-  LAUNCH_CHECK(h);
-  if (pl.prof) {
-    CUDA_OK(cudaEventRecord(h->prof_ev[2 * h->prof_n + 1], s));
-    h->prof_n += 1;
-  }
-  if (spare) {  // rebuild the spares this launch consumed, on the side stream, while the next launches run
-    SPARE_REBUILD_BEGIN(h, s);
-    k_land_step<false, false, true><<<h->sm_count, kBlock, 0, h->side>>>(h->rk, h->land, h->rng, h->buf.state, h->buf.istate, actions, nullptr, h->buf.obs,
-                                                                         h->buf.reward, h->buf.term, h->buf.trunc, h->buf.info, h->buf.start_pos,
-                                                                         h->buf.start_orn, pl.cnt_prev, pl.list_prev, pl.cnt_cur, pl.list_cur, pl.cnt_next,
-                                                                         spare, 0, 1, h->sm_count, pl.seq, h->n);
-    LAUNCH_CHECK(h);
-    SPARE_REBUILD_DONE(h);
-  }
-  h->step_seq += 1;
-  return 0;
+  return tail_env_step(h, noise, randact, s, land_launcher(h, actions, noise));
 }
