@@ -293,6 +293,13 @@ int pfb_reset(PfbHandle h, const uint8_t* mask, void* stream);
 /* Aviary.set_mode (aviary.py:440-458, quadx.py:233-373): same mode for every env; resets the PIDs
  * and presets the bound setpoint buffer rows exactly like the reference.                             */
 int pfb_set_mode(PfbHandle h, int mode, void* stream);
+/* Aviary.set_mode(list) (aviary.py:440-458): env i gets QuadX/Fixedwing.set_mode(modes[i]), with the setpoint preset and
+ * PID reset of its new mode; modes is a host array of n_envs entries.  Aviary handles only (created without an env
+ * epilogue).  Ranges: QuadX -1..7, fixed-wing -1..0, rocket 0.  All entries equal: exactly pfb_set_mode(h, modes[0]).
+ * Otherwise the following pfb_aviary_step calls fly each env in its own mode, until pfb_set_mode or an unmasked
+ * pfb_reset returns the handle to one mode (a masked reset keeps the modes).  Envs 32k .. 32k+31 share a warp: a batch
+ * steps fastest when each such tile flies one mode.                                                                      */
+int pfb_set_modes(PfbHandle h, const int8_t* modes, void* stream);
 /* n_steps × Aviary.step() (aviary.py:480-531).  noise: device [n_steps*updates_per_step][N] raw
  * draws of np_random.normal(*throttle.shape) (motors.py:134-138), or NULL → on-device Philox.        */
 int pfb_aviary_step(PfbHandle h, int n_steps, const float* noise, void* stream);

@@ -171,18 +171,32 @@ class BatchedAviary:
         self._state_fresh = False
 
     def set_mode(self, flight_modes: int | Sequence[int]) -> None:
-        """aviary.py:440-458; one mode per batch (the kernel is specialised on it at compile time)."""
+        """aviary.py:440-458: one mode for every drone, or a list / tuple with one mode per drone.
+
+        A list whose entries differ flies each drone in its own mode until the next ``set_mode(int)`` or ``reset()`` (Aviary
+        handles only; an env flies its ``flight_mode``).  Drones ``32 k .. 32 k + 31`` share one warp: a batch steps fastest
+        when each such tile flies one mode (DESIGN.md §4b)."""
+        lo, hi = (-1, 7) if self.drone_type == "quadx" else ((-1, 0) if self.drone_type == "fixedwing" else (0, 0))
+
+        def check_range(mode: int) -> None:
+            if mode < lo or mode > hi:
+                # quadx.py:259-262, fixedwing.py:216-219, base_drone.py:252-255
+                raise ValueError(f"`mode` must be between {lo} and {hi} or be registered in self.registered_controllers.keys()=dict_keys([]), got {mode}.")
+
         if isinstance(flight_modes, (list, tuple)):
             if len(flight_modes) != self.num_drones:
                 raise AssertionError(f"Expected {self.num_drones} flight_modes, got {len(flight_modes)}.")
-            if len(set(flight_modes)) != 1:
-                raise ValueError("the batched stepper needs one flight mode per batch")
-            flight_modes = flight_modes[0]
+            modes = [int(m) for m in flight_modes]
+            for m in modes:  # every drone's set_mode checks its own mode (aviary.py:455-456)
+                check_range(m)
+            if len(set(modes)) != 1:
+                arr = np.ascontiguousarray(modes, dtype=np.int8)
+                _lib.check(_lib.lib().pfb_set_modes(self._h, arr.ctypes.data_as(C.c_void_p), self._s()))
+                self._state_fresh = False
+                return
+            flight_modes = modes[0]
         mode = int(flight_modes)
-        lo, hi = (-1, 7) if self.drone_type == "quadx" else ((-1, 0) if self.drone_type == "fixedwing" else (0, 0))
-        if mode < lo or mode > hi:
-            # quadx.py:259-262, fixedwing.py:216-219, base_drone.py:252-255
-            raise ValueError(f"`mode` must be between {lo} and {hi} or be registered in self.registered_controllers.keys()=dict_keys([]), got {mode}.")
+        check_range(mode)
         _lib.check(_lib.lib().pfb_set_mode(self._h, mode, self._s()))
         self._state_fresh = False
 

@@ -92,7 +92,12 @@ struct PfbContext {
   // mixed-model QuadX handle (pfb_set_models with k > 1): the tables and d_model_index; nullptr = every env flies `qx`
   QuadXModelSet* qxset;
   uint8_t* d_model_index;
+  // one flight mode per drone (pfb_set_modes; Aviary handles): device [whole tiles * 32], valid while mode == kModePerDrone
+  int8_t* d_modes;
 };
+
+// PfbContext::mode of an Aviary handle whose drones fly the modes in d_modes; pfb_set_mode and a full pfb_reset replace it
+constexpr int kModePerDrone = 0x100;
 
 // Runs BODY with PS = the coefficient-table type of the QuadX kernels and `ps` = the value to pass: the handle's table, or its
 // model set on a mixed-model handle
@@ -256,6 +261,7 @@ int fw_istate_rows();
 int fw_obs_dim(const PfbContext* h);
 int fw_reset(PfbContext* h, const uint8_t* mask, cudaStream_t s);
 int fw_set_mode(PfbContext* h, int mode, cudaStream_t s);
+int fw_set_modes(PfbContext* h, cudaStream_t s);  // after d_modes holds the modes: zero the setpoints, flag the handle
 int fw_aviary_step(PfbContext* h, int n_steps, const float* noise, cudaStream_t s);
 int fw_observe(PfbContext* h, cudaStream_t s);
 int fw_env_reset(PfbContext* h, const uint8_t* mask, const float* noise, cudaStream_t s);

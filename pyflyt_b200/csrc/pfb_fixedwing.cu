@@ -60,6 +60,39 @@ __global__ void __launch_bounds__(kBlock, kMinBlocks)
   fixedwing_store(st, ist, N, i, s);
 }
 
+// k_fw_aviary_step with drone i in flight mode modes[i] (pfb_set_modes): only the command mapping branches on the mode
+template <bool FULL, typename NoiseFn>
+__device__ __forceinline__ void fixedwing_aviary_step_any(const FixedwingParams& p, FixedwingRegs& s, int mode, NoiseFn& noise) {
+  s.flags &= ~(uint32_t)FLAG_CONTACT_ARRAY;
+  noise.begin_step();
+  float cmd[6];
+  if (mode == -1) fixedwing_command<-1>(s, cmd);
+  else fixedwing_command<0>(s, cmd);
+#pragma unroll 1
+  for (int u = 0; u < p.ratio; ++u) fixedwing_substep<FULL>(p, s, cmd, noise.get(u));
+}
+
+template <bool INJECT>
+__global__ void __launch_bounds__(kBlock, kMinBlocks)
+    k_fw_aviary_step_modes(const __grid_constant__ FixedwingParams p, const __grid_constant__ RngParams rng, float* __restrict__ st,
+                           int32_t* __restrict__ ist, const float* __restrict__ setpoint, const int8_t* __restrict__ modes,
+                           const float* __restrict__ noise, int n_steps, uint32_t seq, int64_t N) {
+  int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= N) return;
+  const int mode = modes[i];
+  FixedwingRegs s;
+  fixedwing_load(st, ist, N, i, s);
+#pragma unroll
+  for (int k = 0; k < 6; ++k) s.sp[k] = __ldg(setpoint + (int64_t)6 * i + k);  // Aviary handles: 6-wide setpoints
+  auto nz = make_noise<INJECT>(noise, N, i, rng, seq, TAG_AVIARY, p.noise_loc, p.ratio);
+  if (fixedwing_full_model(p)) {
+    for (int k = 0; k < n_steps; ++k) fixedwing_aviary_step_any<true>(p, s, mode, nz);
+  } else {
+    for (int k = 0; k < n_steps; ++k) fixedwing_aviary_step_any<false>(p, s, mode, nz);
+  }
+  fixedwing_store(st, ist, N, i, s);
+}
+
 __global__ void __launch_bounds__(kBlock) k_fw_observe(const float* __restrict__ st, const int32_t* __restrict__ ist,
                                                        float* __restrict__ drone_state, float* __restrict__ aux,
                                                        uint8_t* __restrict__ contact, int64_t N) {
@@ -358,9 +391,23 @@ int fw_set_mode(PfbContext* h, int mode, cudaStream_t s) {
   return 0;
 }
 
+int fw_set_modes(PfbContext* h, cudaStream_t s) {
+  CUDA_OK(cudaMemsetAsync(h->buf.setpoint, 0, (size_t)h->n * fw_setpoint_dim(h) * sizeof(float), s));  // every drone's set_mode
+  h->mode = kModePerDrone;
+  return 0;
+}
+
 int fw_aviary_step(PfbContext* h, int n_steps, const float* noise, cudaStream_t s) {
   const uint32_t seq = (uint32_t)h->aviary_seq++;
   const int g = grid_for(h->n);
+  if (h->mode == kModePerDrone) {  // pfb_set_modes: Aviary handles only (6-wide setpoints)
+#define FWM_ARGS h->fw, h->rng, h->buf.state, h->buf.istate, h->buf.setpoint, h->d_modes, noise, n_steps, seq, h->n
+    if (noise) k_fw_aviary_step_modes<true><<<g, kBlock, 0, s>>>(FWM_ARGS);
+    else k_fw_aviary_step_modes<false><<<g, kBlock, 0, s>>>(FWM_ARGS);
+#undef FWM_ARGS
+    LAUNCH_CHECK(h);
+    return 0;
+  }
 #define FW_ARGS h->fw, h->rng, h->buf.state, h->buf.istate, h->buf.setpoint, noise, n_steps, seq, fw_setpoint_dim(h), h->n
   if (h->mode == 0) {
     if (noise) k_fw_aviary_step<0, true><<<g, kBlock, 0, s>>>(FW_ARGS);

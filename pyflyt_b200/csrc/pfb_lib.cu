@@ -108,6 +108,44 @@ __global__ void __launch_bounds__(kBlock, kMinBlocks)
   qx_store_any<MODE, TILED>(st, ist, rows, N, i, s, step_count);
 }
 
+// ---- one flight mode per drone (pfb_set_modes; Aviary handles, warp-tiled) ----------------------------------------------
+// Aviary.set_mode(list): QuadX.set_mode(mode[i]) for every drone i, as k_quadx_set_mode does for one mode
+__global__ void __launch_bounds__(kBlock) k_quadx_set_modes(float* __restrict__ st, int rows, float* __restrict__ setpoint,
+                                                            const int8_t* __restrict__ modes, int64_t N) {
+  int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= N) return;
+  QuadXRegs s;
+  int step_count;
+  quadx_load_tile<7, kTileGroupStride>(st + qx_tile_base(i, rows), s, step_count);
+  float4 sp = reinterpret_cast<const float4*>(setpoint)[i];
+  s.sp[0] = sp.x; s.sp[1] = sp.y; s.sp[2] = sp.z; s.sp[3] = sp.w;
+  quadx_set_mode_any(s, modes[i]);
+  quadx_store_tile<7, kTileGroupStride>(st + qx_tile_base(i, rows), s, step_count);
+  reinterpret_cast<float4*>(setpoint)[i] = make_float4(s.sp[0], s.sp[1], s.sp[2], s.sp[3]);
+}
+
+// n_steps x Aviary.step() with drone i in flight mode modes[i].  Every PID row is moved (the mode-7 set); quadx_mask_pid
+// gives each drone the PID memory the uniform kernel of its mode would load, so both store the same words.
+template <bool INJECT, class PS>
+__global__ void __launch_bounds__(kBlock, kMinBlocks)
+    k_quadx_aviary_step_modes(const __grid_constant__ PS ps, const __grid_constant__ RngParams rng, float* __restrict__ st, int rows,
+                              const float* __restrict__ setpoint, const int8_t* __restrict__ modes, const float* __restrict__ noise,
+                              int n_steps, uint32_t seq, int64_t N) {
+  int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= N) return;
+  const QuadXParams& p = qx_model(ps, i);
+  const int mode = modes[i];
+  QuadXRegs s;
+  int step_count;
+  quadx_load_tile<7, kTileGroupStride>(st + qx_tile_base(i, rows), s, step_count);
+  quadx_mask_pid(s, mode);
+  float4 sp = __ldg(reinterpret_cast<const float4*>(setpoint) + i);
+  s.sp[0] = sp.x; s.sp[1] = sp.y; s.sp[2] = sp.z; s.sp[3] = sp.w;
+  auto nz = make_noise<INJECT>(noise, N, i, rng, seq, TAG_AVIARY, qx_model0(ps).noise_loc, qx_model0(ps).ratio);
+  for (int k = 0; k < n_steps; ++k) quadx_aviary_step_any(p, s, mode, nz);
+  quadx_store_tile<7, kTileGroupStride>(st + qx_tile_base(i, rows), s, step_count);
+}
+
 // Aviary.state(i) / aux_state(i) / contact_array  -> row-major API buffers
 template <bool TILED>
 __global__ void __launch_bounds__(kBlock) k_quadx_observe(const float* __restrict__ st, const int32_t* __restrict__ ist, int rows,
@@ -975,6 +1013,7 @@ int pfb_destroy(PfbHandle h) {
   cudaFree(h->d_counters);
   cudaFree(h->d_done_list);
   if (h->d_model_index) cudaFree(h->d_model_index);
+  if (h->d_modes) cudaFree(h->d_modes);
   delete h->qxset;
   if (h->prof_ev) {
     for (int i = 0; i < 2 * h->prof_cap; ++i) cudaEventDestroy(h->prof_ev[i]);
@@ -1051,6 +1090,34 @@ int pfb_set_mode(PfbHandle h, int mode, void* stream) {
   return 0;
 }
 
+int pfb_set_modes(PfbHandle h, const int8_t* modes, void* stream) {
+  if (!h || !modes) return fail("pfb_set_modes: null argument");
+  if (h->env.env_kind != PFB_ENV_NONE)
+    return fail("pfb_set_modes: only Aviary handles fly one flight mode per drone; a handle with an env epilogue flies its env's flight_mode");
+  REQUIRE_BOUND(h);
+  const int lo = is_rk(h) ? 0 : -1, hi = is_rk(h) || is_fw(h) ? 0 : 7;  // quadx.py:259-262, fixedwing.py:216-219, rocket: mode 0 only
+  bool uniform = true;
+  for (int64_t i = 0; i < h->n; ++i) {
+    if (modes[i] < lo || modes[i] > hi)
+      return fail("pfb_set_modes: modes[%lld] = %d, must be between %d and %d for this vehicle kind", (long long)i, (int)modes[i], lo, hi);
+    uniform = uniform && modes[i] == modes[0];
+  }
+  if (uniform) return pfb_set_mode(h, modes[0], stream);  // one mode: the uniform kernels
+  cudaStream_t s = (cudaStream_t)stream;
+  const size_t padded = (size_t)grid_for(h->n) * kBlock;  // whole tiles, like d_model_index
+  if (!h->d_modes) {
+    CUDA_OK(cudaMalloc(&h->d_modes, padded));
+    CUDA_OK(cudaMemsetAsync(h->d_modes, 0, padded, s));
+  }
+  // stream-ordered: a step still queued on `s` reads the previous modes
+  CUDA_OK(cudaMemcpyAsync(h->d_modes, modes, (size_t)h->n, cudaMemcpyHostToDevice, s));
+  if (is_fw(h)) return fw_set_modes(h, s);
+  k_quadx_set_modes<<<grid_for(h->n), kBlock, 0, s>>>(h->buf.state, qx_rows(h), h->buf.setpoint, h->d_modes, h->n);
+  LAUNCH_CHECK(h);
+  h->mode = kModePerDrone;
+  return 0;
+}
+
 int pfb_aviary_step(PfbHandle h, int n_steps, const float* noise, void* stream) {
   REQUIRE_BOUND(h);
   if (n_steps <= 0) return fail("n_steps must be positive");
@@ -1059,8 +1126,16 @@ int pfb_aviary_step(PfbHandle h, int n_steps, const float* noise, void* stream) 
   if (is_rk(h)) return rk_aviary_step(h, n_steps, noise, s);
   const int mode = h->mode;
   const uint32_t seq = (uint32_t)h->aviary_seq++;
-#define AV_ARGS ps, h->rng, h->buf.state, h->buf.istate, qx_rows(h), h->buf.setpoint, noise, n_steps, seq, h->n
   const int g = grid_for(h->n);
+  if (mode == kModePerDrone) {  // pfb_set_modes: Aviary handles only, so always warp-tiled
+#define AVM_ARGS ps, h->rng, h->buf.state, qx_rows(h), h->buf.setpoint, h->d_modes, noise, n_steps, seq, h->n
+    if (noise) { QX_PARAMS_SWITCH(h, (k_quadx_aviary_step_modes<true, PS><<<g, kBlock, 0, s>>>(AVM_ARGS))); }
+    else { QX_PARAMS_SWITCH(h, (k_quadx_aviary_step_modes<false, PS><<<g, kBlock, 0, s>>>(AVM_ARGS))); }
+#undef AVM_ARGS
+    LAUNCH_CHECK(h);
+    return 0;
+  }
+#define AV_ARGS ps, h->rng, h->buf.state, h->buf.istate, qx_rows(h), h->buf.setpoint, noise, n_steps, seq, h->n
   if (is_tiled(h)) {
     if (noise) { QX_PARAMS_SWITCH(h, PFB_MODE_SWITCH(mode, (k_quadx_aviary_step<MODE, true, true, PS><<<g, kBlock, 0, s>>>(AV_ARGS)))); }
     else { QX_PARAMS_SWITCH(h, PFB_MODE_SWITCH(mode, (k_quadx_aviary_step<MODE, false, true, PS><<<g, kBlock, 0, s>>>(AV_ARGS)))); }

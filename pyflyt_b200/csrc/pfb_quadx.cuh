@@ -502,6 +502,38 @@ PFB_HD void quadx_set_mode(QuadXRegs& s) {
   for (int k = 0; k < PID_ZV; ++k) s.pid[k] = 0.0f;  // z_PIDs are not reset by set_mode (quadx.py:196,372)
 }
 
+// ---- one flight mode per drone (pfb_set_modes): the mode is a run-time value -------------------------------------------
+// Runs BODY with `constexpr int M` = the QuadX flight mode `mode` (-1..7; the caller has checked the range)
+#define PFB_QX_MODE_CASES(mode, BODY)               \
+  switch (mode) {                                   \
+    case -1: { constexpr int M = -1; BODY; } break; \
+    case 0: { constexpr int M = 0; BODY; } break;   \
+    case 1: { constexpr int M = 1; BODY; } break;   \
+    case 2: { constexpr int M = 2; BODY; } break;   \
+    case 3: { constexpr int M = 3; BODY; } break;   \
+    case 4: { constexpr int M = 4; BODY; } break;   \
+    case 5: { constexpr int M = 5; BODY; } break;   \
+    case 6: { constexpr int M = 6; BODY; } break;   \
+    default: { constexpr int M = 7; BODY; } break;  \
+  }
+
+// The control tick of a drone in flight mode `mode`.  Only the control tick branches on the mode: the physics substeps after
+// it are the same code for every mode, so a warp whose lanes fly several modes reconverges before them.
+PFB_HD void quadx_update_control_any(const QuadXParams& p, QuadXRegs& s, int mode) {
+  PFB_QX_MODE_CASES(mode, quadx_update_control<M>(p, s));
+}
+
+template <typename NoiseFn>
+PFB_HD void quadx_aviary_step_any(const QuadXParams& p, QuadXRegs& s, int mode, NoiseFn& noise) {
+  s.flags &= ~(uint32_t)FLAG_CONTACT_ARRAY;
+  noise.begin_step();
+  quadx_update_control_any(p, s, mode);
+#pragma unroll 1
+  for (int u = 0; u < p.ratio; ++u) quadx_substep(p, s, noise.get(u));
+}
+
+PFB_HD void quadx_set_mode_any(QuadXRegs& s, int mode) { PFB_QX_MODE_CASES(mode, quadx_set_mode<M>(s)); }
+
 // quadx.py:222-231 + aviary.py:310-311: a freshly constructed drone at its start pose
 PFB_HD void quadx_reset(QuadXRegs& s, float sx, float sy, float sz, float roll, float pitch, float yaw) {
   s.px = (xreal)sx; s.py = (xreal)sy; s.pz = (xreal)sz;
@@ -760,6 +792,28 @@ PFB_HD void quadx_store_tile(float* __restrict__ rec, const QuadXRegs& s, int st
       st_f4(rec + g * GS, v[0], v[1], v[2], v[3]);
     }
   }
+}
+
+// PID words that a step of the uniform MODE kernel leaves as they were (bit k = PID word k).  Its load reads the rows MODE
+// uses and zeroes the other rows of the groups it moves, and its store writes those groups back; the rows of the groups it
+// does not move keep their memory (the z PIDs of a drone that flies mode 0 or 1 between two height-hold phases).
+template <int MODE>
+PFB_HD constexpr uint32_t qx_pid_kept() {
+  uint32_t m = 0u;
+  for (int k = 0; k < PID_WORDS; ++k) {
+    const bool moved = k < PID_P1 || qx_group_used<MODE>(10 + (k - PID_P1) / 4);
+    if (pid_row_used<MODE>(k) || !moved) m |= 1u << k;
+  }
+  return m;
+}
+// After a mode-7 load (every PID row) of a drone in mode `mode`: zero what the uniform kernel of that mode would have loaded
+// as zero, so that the per-drone step stores the same state tensor, word for word, as the uniform kernel of the drone's mode
+PFB_HD void quadx_mask_pid(QuadXRegs& s, int mode) {
+  uint32_t kept = 0u;
+  PFB_QX_MODE_CASES(mode, kept = qx_pid_kept<M>());
+#pragma unroll
+  for (int k = 0; k < PID_WORDS; ++k)
+    if (!((kept >> k) & 1u)) s.pid[k] = 0.0f;
 }
 
 // Round the fp64-carried fields to what the state tensor holds (hi + lo fp32 words) and re-derive R / body velocity:

@@ -139,6 +139,131 @@ def mixed_model_fixtures():
     fly_quadx_mixed("mixed_models_quadx_mode7", 7, opts, pos7, orn, sched7, 300, seed=93)
 
 
+def _setpoint_rows(env):
+    """[n, S] setpoints of every drone; fixed-wing mode 0 keeps 4 (fixedwing.py:224-227), padded here to mode -1's 6"""
+    rows = [np.atleast_1d(np.asarray(d.setpoint, dtype=np.float64)) for d in env.drones]
+    w = max(len(r) for r in rows)
+    return np.array([np.concatenate([r, np.zeros(w - len(r))]) for r in rows])
+
+
+def fly_mixed_modes(name, drone_type, drone_options, start_pos, start_orn, mode_calls, setpoint_fn, n_steps, seed):
+    """Aviary-level flight of several drones in one reference Aviary with one flight mode per drone: ``mode_calls`` =
+    {step_index: [n] modes}, each applied with ``Aviary.set_mode(list)`` before that step (aviary.py:440-458).
+    ``setpoint_fn(step, modes, current)`` returns None or the [n, S] setpoints to apply before the step (after a set_mode call;
+    ``current`` = the drones' setpoints at that point).
+    The fixture stores the modes of every call and the setpoints each call left."""
+    n = len(drone_options)
+    rng = ril.ScriptedNoise(seed)
+    env = Aviary(
+        start_pos=np.array(start_pos, dtype=np.float64),
+        start_orn=np.array(start_orn, dtype=np.float64),
+        drone_type=drone_type,
+        drone_options=[dict(d) for d in drone_options],
+        np_random=rng,
+    )
+    states, auxs, contacts, sps, sp_after = [], [], [], [], []
+    modes = None
+    for i in range(n_steps):
+        if i in mode_calls:
+            modes = [int(m) for m in mode_calls[i]]
+            env.set_mode(modes)
+            sp_after.append(_setpoint_rows(env))
+        sp = setpoint_fn(i, modes, _setpoint_rows(env))
+        if sp is not None:
+            env.set_all_setpoints(np.array(sp, dtype=np.float64))
+        sps.append(_setpoint_rows(env))
+        env.step()
+        states.append(np.array([d.state for d in env.drones]))
+        auxs.append(np.array([d.aux_state for d in env.drones], dtype=np.float64))
+        contacts.append(np.array([bool(env.contact_array[env.planeId, d.Id]) for d in env.drones]))
+    # one reference world: any floor contact would remove every QuadX's rotational drag (quadx.py:508-510)
+    assert not np.any(contacts), f"{name}: a drone touched the floor"
+    steps = sorted(mode_calls)
+    np.savez_compressed(
+        os.path.join(OUT, f"{name}.npz"),
+        kind=f"{drone_type}_mixed_modes",
+        drone_type=drone_type,
+        n_drones=n,
+        drone_options=json.dumps(drone_options),
+        start_pos=np.array(start_pos, dtype=np.float64),
+        start_orn=np.array(start_orn, dtype=np.float64),
+        mode_steps=np.array(steps),
+        modes=np.array([mode_calls[k] for k in steps], dtype=np.int64),
+        setpoint_after_set_mode=np.array(sp_after),
+        setpoints=np.array(sps),
+        noise=np.array(rng.normal_log),
+        state=np.array(states),
+        aux=np.array(auxs),
+        contact=np.array(contacts),
+    )
+    print(name, "final z", np.array(states[-1])[:, 3, 2], "draws", len(rng.normal_log))
+
+
+def mixed_mode_fixtures():
+    """One flight mode per drone.  QuadX: 18 drones, every mode -1..7 on cf2x and on primitive_drone, re-assigned by
+    set_mode(list) at steps 100 and 200: the height-hold drones (modes 2, 3, 4, 7) fly mode 0 or 1 in between and then hold
+    height again with the z-PID memory set_mode keeps (quadx.py:196, 372).  Setpoints come from the ranges of the single-mode
+    fixtures, heights relative to the start.  Fixed-wing: 4 drones, modes -1 / 0 alternating.  No drone touches the floor."""
+    n = 18
+    opts = [dict(drone_model="cf2x" if d % 2 == 0 else "primitive_drone") for d in range(n)]
+    pos = np.array([[10.0 * d, 0.0, 60.0 + 0.5 * d] for d in range(n)])
+    orn = [[0.05 * (d % 5), -0.04 * (d % 4), 0.3 * (d % 7)] for d in range(n)]
+    first = [-1 + d // 2 for d in range(n)]
+    away = {-1: 3, 0: 7, 1: 2, 2: 0, 3: 1, 4: 0, 5: 4, 6: -1, 7: 1}
+    calls = {0: first, 100: [away[m] for m in first], 200: first}
+    table = {  # the first / second setpoint of quadx_<model>_mode<m>; heights and mode-7 positions relative to the start
+        -1: ([0.3, 0.31, 0.32, 0.3], [0.5, 0.5, 0.45, 0.5]),
+        0: ([0.3, -0.2, 0.1, 0.45], [-0.5, 0.4, -0.3, 0.3]),
+        1: ([0.2, -0.1, 0.5, 0.3], [-0.2, 0.2, -0.5, -0.2]),
+        2: ([0.2, -0.2, 0.3, 1.0], [-0.3, 0.1, 0.0, -1.0]),
+        3: ([0.15, -0.1, 0.6, 1.0], [0.0, 0.0, -0.6, -0.5]),
+        4: ([0.8, -0.5, 0.3, 1.0], [-0.6, 0.4, -0.2, -0.5]),
+        5: ([0.8, -0.5, 0.3, 0.4], [-0.6, 0.4, -0.2, -0.3]),
+        6: ([0.9, 0.4, 0.5, 0.3], [-0.5, -0.7, -0.4, -0.2]),
+        7: ([1.0, -1.0, 0.8, 1.0], [-0.5, 0.5, -0.8, -1.0]),
+    }
+
+    def quadx_sp(i, modes, current):
+        if i % 100 == 0:  # a set_mode call's preset is flown for 10 steps; mode -1 keeps the previous setpoint, so it gets pwm now
+            out = current.copy()
+            for d, m in enumerate(modes):
+                if m == -1:
+                    out[d] = table[-1][0]
+            return out
+        if i % 50 != 10 and i % 50 != 0:
+            return None
+        out = np.zeros((n, 4))
+        for d, m in enumerate(modes):
+            out[d] = table[m][(i // 50) % 2]
+            if m in (2, 3, 4, 7):
+                out[d, 3] += pos[d, 2]
+            if m == 7:
+                out[d, :2] += pos[d, :2]
+        return out
+
+    fly_mixed_modes("mixed_modes_quadx", "quadx", opts, pos.tolist(), orn, calls, quadx_sp, 300, seed=95)
+
+    nf = 4
+    fw_opts = [dict(drone_model="fixedwing") for _ in range(nf)]
+    fw_pos = [[40.0 * d, 0.0, 80.0] for d in range(nf)]
+    fw_orn = [[0.05 * d, 0.1, 0.4 * d] for d in range(nf)]
+    fw_modes = [-1 if d % 2 == 0 else 0 for d in range(nf)]
+    r = np.random.default_rng(96)
+
+    def fw_sp(i, modes, current):
+        if i % 40:
+            return None
+        out = np.zeros((nf, 6))
+        for d, m in enumerate(modes):
+            if m == -1:
+                out[d] = np.concatenate([r.uniform(-0.8, 0.8, 5), r.uniform(0.0, 1.0, 1)])
+            else:
+                out[d, :4] = np.concatenate([r.uniform(-0.6, 0.6, 3), r.uniform(0.3, 1.0, 1)])
+        return out
+
+    fly_mixed_modes("mixed_modes_fixedwing", "fixedwing", fw_opts, fw_pos, fw_orn, {0: fw_modes}, fw_sp, 200, seed=97)
+
+
 def wind_fields(wind):
     """npz entries describing an AnalyticWind (absent = still air)"""
     if wind is None:
@@ -762,3 +887,5 @@ if __name__ == "__main__":
         touchdown_fixtures()
     if which in ("all", "mixed"):
         mixed_model_fixtures()
+    if which in ("all", "mixedmodes"):
+        mixed_mode_fixtures()
