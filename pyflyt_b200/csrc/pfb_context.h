@@ -1,5 +1,5 @@
 // pfb_context.h — private to libpyflyt_b200: the handle, error plumbing and launch helpers shared by
-// the per-vehicle translation units (pfb_lib.cu, pfb_fixedwing.cu, ...).
+// the C-ABI (pfb_lib.cu) and the per-vehicle translation units (pfb_quadx.cu, pfb_fixedwing.cu, ...).
 #pragma once
 
 #include <cuda_runtime.h>
@@ -73,13 +73,13 @@ struct PfbContext {
   int64_t launches;
   pfb::QxWaypointParams qwp;
   int sm_count;
-  // QuadX-Hover reset pipeline (pfb_lib.cu, "spare post-reset states"): library-owned spares + the side stream that rebuilds them
+  // spare post-reset states (QuadX-Hover: pfb_quadx.cu; tail-CTA kinds: pfb_tail_step.cuh, rebuilt on the side stream)
   float* d_spare;          // spare post-reset states (env-major records), zero-initialised; nullptr = warm-ups run inline
   int2* d_consumed;        // QuadX-Hover fused rollout: (env, episode to rebuild) for every spare a launch consumed
   int fused_ready;         // every env has its spares kRolloutAhead ahead and the step pipeline is drained (cleared by single steps / resets)
   uint32_t* d_elist;       // QuadX-Hover: [4][N] episode number being built for each done-list entry (builder phase 0 -> phase 1)
-  uint32_t* d_episode;     // QuadX-Hover: [N] episode number of each env's current valid spare (its buffer = episode & 1)
-  cudaStream_t side;       // k_hover_spare runs here, concurrently with the following step launches
+  uint32_t* d_episode;     // QuadX-Hover: [N] episode number of each env's current valid spare (its buffer = episode & kSpareMask)
+  cudaStream_t side;       // tail-CTA kinds: the spare rebuild runs here, concurrently with the following step launches
   cudaEvent_t ev_step;     // recorded on the caller's stream after a step launch; the side stream waits on it
   cudaEvent_t ev_spare[4]; // ev_spare[k % 4]: spares consumed by step k are rebuilt; step k + 2 waits on it
   int64_t side_launches;
@@ -131,6 +131,10 @@ static inline int grid_for(int64_t n) { return (int)((n + kBlock - 1) / kBlock);
     if (_e != cudaSuccess) return fail("kernel launch failed: %s", cudaGetErrorString(_e)); \
     (h)->launches += 1;                                                     \
   } while (0)
+
+// QuadX state layout: warp-tiled (pfb_quadx.cuh) on every QuadX handle except QuadX-Waypoints (field-major rows + istate)
+static inline bool qx_tiled(const PfbContext* h) { return h->model.kind == PFB_KIND_QUADX && h->env.env_kind != PFB_ENV_QUADX_WAYPOINTS; }
+static inline int qx_rows(const PfbContext* h) { return h->env.env_kind == PFB_ENV_MA_QUADX_HOVER ? (int)pfb::QM_ROWS : (int)pfb::QX_ROWS; }
 
 // per-step bookkeeping shared by every env kind (rotating counters and lists, tail CTAs)
 struct StepPlan {
@@ -253,6 +257,19 @@ int tail_env_reset(PfbContext* h, const uint8_t* mask, cudaStream_t s, Reset&& r
   }
   return 0;
 }
+
+// QuadX translation unit (pfb_quadx.cu): Aviary surface, QuadX-Hover and MAQuadXHover
+int qx_reset(PfbContext* h, const uint8_t* mask, cudaStream_t s);
+int qx_set_mode(PfbContext* h, int mode, cudaStream_t s);
+int qx_set_modes(PfbContext* h, cudaStream_t s);  // after d_modes holds the modes
+int qx_aviary_step(PfbContext* h, int n_steps, const float* noise, cudaStream_t s);
+int qx_observe(PfbContext* h, cudaStream_t s);
+int hover_spare_rows();     // floats of d_spare per env
+int hover_consumed_rows();  // entries of d_consumed per env
+int hover_env_reset(PfbContext* h, const uint8_t* mask, const float* noise, cudaStream_t s);
+// `dyn_smem`: dynamic shared memory the step launch requests and never touches (pfb_env_step_mapped; 0 = every CTA resident in one wave)
+int hover_env_step(PfbContext* h, float* actions, const float* noise, bool randact, size_t dyn_smem, cudaStream_t s);
+int hover_env_rollout(PfbContext* h, int n_steps, cudaStream_t s);  // n_steps env steps with on-device actions, fused where it can
 
 // fixedwing translation unit (pfb_fixedwing.cu)
 int fw_build_params(const PfbModel& m, const PfbEnvConfig* env, pfb::FixedwingParams& p, pfb::WaypointParams& w);

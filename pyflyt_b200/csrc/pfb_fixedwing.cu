@@ -1,5 +1,5 @@
 // pfb_fixedwing.cu — Fixedwing kernels (Aviary surface + Fixedwing-Waypoints env) and their launchers.
-// Same structure as the QuadX kernels in pfb_lib.cu: one thread = one env, state in registers between a
+// Same structure as the QuadX kernels in pfb_quadx.cu: one thread = one env, state in registers between a
 // coalesced SoA load and store, obs staged through shared memory, NEXT_STEP autoreset by tail CTAs.
 #include <cmath>
 #include <cstring>

@@ -2,7 +2,7 @@
 // fp32/fp64 precision policy and the control-flow of the CUDA kernels can be studied and unit-tested on
 // a machine without a GPU.  Never linked into, loaded by, or reachable from the product package:
 // libpyflyt_b200.so contains CUDA kernels only and fails loudly without a device.
-// The glue below mirrors the kernels in pfb_lib.cu one-to-one (same loads, same order, same stores).
+// The glue below mirrors the kernels in pfb_quadx.cu one-to-one (same loads, same order, same stores).
 #include <cstdarg>
 #include <cstdio>
 #include <cstring>

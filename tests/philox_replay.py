@@ -1,5 +1,5 @@
 """TEST INFRASTRUCTURE — NumPy restatement of the device-side random streams of libpyflyt_b200 (pyflyt_b200/csrc/pfb_common.cuh:
-philox4x32_10, u32_to_unit_open, box_muller; pfb_noise.cuh: PhiloxNoise; pfb_lib.cu: the RANDACT action mapping).
+philox4x32_10, u32_to_unit_open, box_muller; pfb_noise.cuh: PhiloxNoise; pfb_quadx.cu: the RANDACT action mapping of k_hover_step).
 
 The kernels are stateless: every draw is a pure function of (seed, global env id, call sequence number, stream tag, Aviary
 step).  That lets a test regenerate exactly the noise / action streams the TIMED instantiation of the step kernel consumes
