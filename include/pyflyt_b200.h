@@ -250,7 +250,8 @@ int pfb_create(const PfbModel* model, const PfbEnvConfig* env, int64_t n_envs, i
 int pfb_destroy(PfbHandle h);
 /* env.reset(seed=s) of the reference re-creates np_random: the same seed must give the same episodes.  Re-keys the Philox
  * streams and rewinds every call counter (step / reset / Aviary step numbers, autoreset episode numbers), stream-ordered on
- * `stream`; follow it with pfb_reset / pfb_env_reset.                                                                     */
+ * `stream`.  It invalidates the spare post-reset states (they hold warm-ups of the old streams): an env handle must follow it
+ * with a full pfb_env_reset (mask = NULL), which rebuilds them; an Aviary handle with pfb_reset.                         */
 int pfb_reseed(PfbHandle h, uint64_t seed, void* stream);
 /* Global index of this handle's env 0 (rank * n_envs when the batch is sharded over GPUs): keeps
  * the Philox streams, and therefore every trajectory, independent of the number of ranks.          */

@@ -299,7 +299,8 @@ class BatchedAviary:
 
     def reseed(self, seed: int) -> None:
         """``env.reset(seed=s)``: re-key the random streams and rewind every call counter, so that the same seed replays the same
-        episodes (the reference re-creates ``np_random``, aviary.py:108-117)."""
+        episodes (the reference re-creates ``np_random``, aviary.py:108-117).  The spare post-reset states built from the old
+        streams are dropped: follow with a full ``env_reset()`` (no mask) or ``reset()``."""
         self.seed = int(seed)
         _lib.check(_lib.lib().pfb_reseed(self._h, self.seed, self._s()))
 
@@ -314,9 +315,15 @@ class BatchedAviary:
         return int(_lib.lib().pfb_launch_count(self._h))
 
     # ------------------------------------------------------------------ fused env surface
-    def env_reset(self, mask: torch.Tensor | None = None, noise: torch.Tensor | None = None, targets: torch.Tensor | None = None) -> torch.Tensor:
+    def env_reset(self, mask: torch.Tensor | None = None, noise: torch.Tensor | None = None, targets: torch.Tensor | None = None,
+                  seed: int | None = None) -> torch.Tensor:
         """env.reset() for all / masked envs.  ``targets`` [N, 3*num_targets] installs explicit waypoints
-        (parity tests); by default they are drawn on device like ``WaypointHandler.reset``."""
+        (parity tests); by default they are drawn on device like ``WaypointHandler.reset``.  ``seed``: ``reseed(seed)`` first;
+        that rewinds every env, so it resets the whole batch and takes no ``mask``."""
+        if seed is not None:
+            if mask is not None:
+                raise ValueError("reset(seed=...) re-keys the random streams of every env: it resets the whole batch and takes no mask")
+            self.reseed(seed)
         if targets is not None:
             self._reset_targets = torch.as_tensor(targets, dtype=torch.float32, device=self.device).reshape(self.num_drones, -1).contiguous()
             self._buffers.reset_targets = self._reset_targets.data_ptr()

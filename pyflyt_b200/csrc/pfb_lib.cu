@@ -440,6 +440,10 @@ int pfb_reseed(PfbHandle h, uint64_t seed, void* stream) {
   h->reset_seq = 0;
   CUDA_OK(cudaMemsetAsync(h->d_counters, 0, 8 * sizeof(int32_t), s));
   if (h->d_episode) CUDA_OK(cudaMemsetAsync(h->d_episode, 0, (size_t)h->n * sizeof(uint32_t), s));
+  // Every spare record was drawn from the old key, and the tail kinds keep each env's episode number inside its record: all of
+  // them are invalidated, which rewinds those episode words to 0 (QuadX-Hover's records fail their validity check instead of
+  // being taken as warm-ups of episode numbers the new streams have not drawn).  The full pfb_env_reset that follows rebuilds them.
+  if (h->d_spare) CUDA_OK(cudaMemsetAsync(h->d_spare, 0, h->spare_bytes, s));
   return 0;
 }
 

@@ -91,7 +91,7 @@ class FixedwingWaypointsVecEnv:
         }
 
     def reset(self, *, seed: int | None = None, options: dict | None = None, mask=None, noise=None, targets=None):
-        obs = self.aviary.env_reset(mask=mask, noise=noise, targets=targets)
+        obs = self.aviary.env_reset(mask=mask, noise=noise, targets=targets, seed=seed)
         if mask is None:
             self.aviary.info_bits.zero_()
         return obs, self._info()

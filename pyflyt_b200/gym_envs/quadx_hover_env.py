@@ -110,8 +110,9 @@ class QuadXHoverVecEnv:
         }
 
     def reset(self, *, seed: int | None = None, options: dict | None = None, mask: torch.Tensor | None = None, noise=None):
-        """env.reset() for every env (or the masked ones): quadx_hover_env.py:70-83."""
-        obs = self.aviary.env_reset(mask=mask, noise=noise)
+        """env.reset() for every env (or the masked ones): quadx_hover_env.py:70-83.  ``seed`` re-keys the random streams of the
+        whole batch first (``BatchedAviary.reseed``): the same seed then replays the same episodes."""
+        obs = self.aviary.env_reset(mask=mask, noise=noise, seed=seed)
         if mask is None:
             self.aviary.info_bits.zero_()
         return obs, self._info()

@@ -99,7 +99,7 @@ class QuadXWaypointsVecEnv:
 
     def reset(self, *, seed: int | None = None, options: dict | None = None, mask=None, noise=None, targets=None):
         """``targets``: optional [N, num_targets, 3 or 4] waypoints (x, y, z[, yaw]); default = drawn on device."""
-        obs = self.aviary.env_reset(mask=mask, noise=noise, targets=targets)
+        obs = self.aviary.env_reset(mask=mask, noise=noise, targets=targets, seed=seed)
         if mask is None:
             self.aviary.info_bits.zero_()
         return obs, self._info()

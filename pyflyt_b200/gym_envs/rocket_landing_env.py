@@ -91,7 +91,7 @@ class RocketLandingVecEnv:
         return {"out_of_bounds": (bits & 1).bool(), "fatal_collision": (bits & 2).bool(), "env_complete": (bits & 4).bool()}
 
     def reset(self, *, seed: int | None = None, options: dict | None = None, mask=None, noise=None):
-        obs = self.aviary.env_reset(mask=mask, noise=noise)
+        obs = self.aviary.env_reset(mask=mask, noise=noise, seed=seed)
         if mask is None:
             self.aviary.info_bits.zero_()
         return obs, self._info()

@@ -111,7 +111,7 @@ class MAFixedwingDogfightVecEnv:
         self.aviary.start_orn.copy_(torch.as_tensor(start_orn, dtype=torch.float32, device=self.device).reshape(-1, 3))
 
     def reset(self, *, seed: int | None = None, options: dict | None = None, noise=None):
-        obs = self.aviary.env_reset(noise=noise)
+        obs = self.aviary.env_reset(noise=noise, seed=seed)
         self.aviary.info_bits.zero_()
         return obs, self._info()
 

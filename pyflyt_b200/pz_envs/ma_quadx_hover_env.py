@@ -90,7 +90,7 @@ class MAQuadXHoverVecEnv:
         return {"out_of_bounds": (bits & 1).bool(), "collision": (bits & 2).bool(), "alive": self.alive}
 
     def reset(self, *, seed: int | None = None, options: dict | None = None, noise=None):
-        obs = self.aviary.env_reset(noise=noise)
+        obs = self.aviary.env_reset(noise=noise, seed=seed)
         self.aviary.info_bits.zero_()
         self.alive.fill_(True)
         return obs, self._info()
