@@ -166,10 +166,8 @@ typedef struct PfbEnvConfig {
   /* MAFixedwingDogfight (pz_envs/fixedwing_envs/ma_fixedwing_dogfight_env.py:42-62): an arena is
    * 2*team_size CONSECUTIVE envs of the batch; the first team_size of them are team 0                 */
   int32_t team_size;
-  int32_t inline_reset;      /* autoreset: 1 = integrate every warm-up inside the step launch instead of copying the env's
-                              * spare post-reset state (same results, longer launches; tests).  QuadX-Hover also takes 2 =
-                              * spares as usual, but rebuilt on the CALLER's stream right behind the step launch (no side
-                              * stream: all of a step's work is in order on one stream)                              */
+  int32_t inline_reset;      /* autoreset: 0 = copy the env's spare post-reset state; 1 = integrate every warm-up inside the
+                              * step launch instead (same results, longer launches; tests).  pfb_create refuses other values */
   double damage_per_hit, lethal_distance, lethal_angle, aggressiveness, cooperativeness;
   double spawn_min_radius, spawn_max_radius, spawn_min_height, spawn_max_height;
   int32_t contact_response;  /* Rocket-Landing: 1 = ground / pad contact RESPONSE (sequential-impulse normal + Coulomb friction

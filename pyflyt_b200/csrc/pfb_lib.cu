@@ -68,6 +68,7 @@ int pfb_create(const PfbModel* model, const PfbEnvConfig* env, int64_t n_envs, i
   if (!model || !out) return fail("pfb_create: null argument");
   if (model->abi_version != PFB_ABI_VERSION) return fail("PfbModel ABI %d != library ABI %d", model->abi_version, PFB_ABI_VERSION);
   if (n_envs <= 0) return fail("n_envs must be positive");
+  if (env && env->inline_reset != 0 && env->inline_reset != 1) return fail("inline_reset must be 0 or 1, got %d", env->inline_reset);
   if (model->kind != PFB_KIND_QUADX && model->kind != PFB_KIND_FIXEDWING && model->kind != PFB_KIND_ROCKET)
     return fail("unknown vehicle kind %d", model->kind);
   int count = 0;

@@ -925,7 +925,7 @@ int hover_env_step(PfbContext* h, float* actions, const float* noise, bool randa
   uint32_t* elist_b0 = h->d_elist ? h->d_elist + ((k + 3) % 4) * h->n : nullptr;
   uint32_t* elist_b1 = h->d_elist ? h->d_elist + ((k + 2) % 4) * h->n : nullptr;
   const bool spares = autoreset && h->d_spare != nullptr;
-  const int spare_copy = (spares && h->env.inline_reset != 1) ? 1 : 0;
+  const int spare_copy = (spares && !h->env.inline_reset) ? 1 : 0;
   const int tiles = grid_for(h->n);
   const int builders = spares ? (h->sm_count < tiles ? h->sm_count : tiles) : 0;
   const int grid = tiles + 2 * builders;
@@ -967,7 +967,7 @@ int hover_env_step(PfbContext* h, float* actions, const float* noise, bool randa
 
 // QuadX-Hover with autoreset: n_steps >= kFusedMinSteps run as fused launches of up to kRolloutMaxSteps env steps (k_hover_rollout)
 static bool hover_fused_ok(PfbContext* h) {
-  return h->model.kind == PFB_KIND_QUADX && h->env.env_kind == PFB_ENV_QUADX_HOVER && h->env.autoreset != 0 && h->env.inline_reset == 0 &&
+  return h->model.kind == PFB_KIND_QUADX && h->env.env_kind == PFB_ENV_QUADX_HOVER && h->env.autoreset != 0 && !h->env.inline_reset &&
          h->d_spare != nullptr && h->d_consumed != nullptr && h->noise_dump == nullptr && !(h->prof_ev && h->prof_n < h->prof_cap);
 }
 constexpr int kFusedMinSteps = 4;

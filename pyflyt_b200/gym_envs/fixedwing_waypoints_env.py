@@ -18,14 +18,11 @@ from typing import Literal
 import numpy as np
 import torch
 
-from ..core.aviary import BatchedAviary
-from ..models import PfbEnvConfig
+from ..core.env_base import WaypointsVecEnv, check_env_args, env_config
 from ..models.tables import ENV_FIXEDWING_WAYPOINTS
 
 
-class FixedwingWaypointsVecEnv:
-    metadata = {"render_modes": [], "render_fps": 30}
-
+class FixedwingWaypointsVecEnv(WaypointsVecEnv):
     def __init__(
         self,
         num_envs: int = 1,
@@ -45,67 +42,17 @@ class FixedwingWaypointsVecEnv:
         env_offset: int = 0,
         inline_reset: bool = False,
     ):
-        if 120 % agent_hz != 0:  # fixedwing_base_env.py:47-52
-            lowest = int(120 / (int(120 / agent_hz) + 1))
-            highest = int(120 / int(120 / agent_hz))
-            raise ValueError(f"`agent_hz` must be round denominator of 120, try {lowest} or {highest}.")
-        if render_mode is not None:
-            raise ValueError("rendering is out of scope for the batched stepper (SURVEY.md §2 row 21)")
-        if angle_representation not in ("euler", "quaternion"):
-            raise ValueError(f"angle_representation must be either `euler` or `quaternion`, not {angle_representation}")
+        check_env_args(agent_hz, render_mode, angle_representation)  # fixedwing_base_env.py:47-52
         if flight_mode != 0:
             raise ValueError("Fixedwing-Waypoints is built for flight mode 0 (the env's 4-dim action box)")
         self.num_envs = int(num_envs)
         self.num_targets = int(num_targets)
-        cfg = PfbEnvConfig()
-        cfg.env_kind = ENV_FIXEDWING_WAYPOINTS
-        cfg.flight_mode = 0
-        cfg.env_step_ratio = int(120 / agent_hz)
-        cfg.max_steps = int(agent_hz * max_duration_seconds)
-        cfg.angle_representation = 0 if angle_representation == "euler" else 1
-        cfg.sparse_reward = int(bool(sparse_reward))
-        cfg.autoreset = int(bool(autoreset))
-        cfg.warmup_steps = 10  # fixedwing_base_env.py:187-188
-        cfg.flight_dome_size = float(flight_dome_size)
-        cfg.goal_reach_distance = float(goal_reach_distance)
-        cfg.goal_reach_angle = float("inf")
-        cfg.num_targets = self.num_targets
-        cfg.use_yaw_targets = 0
-        cfg.inline_reset = int(bool(inline_reset))  # tests: spare-copy resets must equal inline ones bit for bit
-        self.config = cfg
+        cfg = env_config(ENV_FIXEDWING_WAYPOINTS, agent_hz=agent_hz, max_duration_seconds=max_duration_seconds,
+                         angle_representation=angle_representation, sparse_reward=sparse_reward, autoreset=autoreset,
+                         flight_dome_size=flight_dome_size, inline_reset=inline_reset, goal_reach_distance=float(goal_reach_distance),
+                         goal_reach_angle=float("inf"), num_targets=self.num_targets, use_yaw_targets=0)
         sp = np.tile(np.array([[0.0, 0.0, 10.0]]), (self.num_envs, 1))  # fixedwing_waypoints_env.py:63
         so = np.zeros((self.num_envs, 3))
-        self.aviary = BatchedAviary(sp, so, drone_type="fixedwing", drone_options=drone_options, seed=seed, device=device, env_config=cfg, env_offset=env_offset)
-        self.device = self.aviary.device
-        self.obs_dim = self.aviary.obs_dim
+        super().__init__(cfg, sp, so, "fixedwing", drone_options=drone_options, seed=seed, device=device, env_offset=env_offset)
         self.action_low, self.action_high = -np.ones(4), np.ones(4)  # fixedwing_base_env.py:79-81
         self.autoreset = bool(autoreset)
-
-    def _info(self):
-        bits = self.aviary.info_bits
-        return {
-            "out_of_bounds": (bits & 1).bool(),
-            "collision": (bits & 2).bool(),
-            "env_complete": (bits & 4).bool(),
-            "num_targets_reached": (bits >> 3).int(),
-        }
-
-    def reset(self, *, seed: int | None = None, options: dict | None = None, mask=None, noise=None, targets=None):
-        obs = self.aviary.env_reset(mask=mask, noise=noise, targets=targets, seed=seed)
-        if mask is None:
-            self.aviary.info_bits.zero_()
-        return obs, self._info()
-
-    def step(self, actions: torch.Tensor, noise=None):
-        a = self.aviary
-        if not (torch.is_tensor(actions) and actions.is_cuda and actions.dtype == torch.float32 and actions.is_contiguous()):
-            a.setpoints.copy_(torch.as_tensor(actions, dtype=torch.float32, device=self.device).reshape(self.num_envs, 4))
-            actions = None
-        a.env_step(actions=actions, noise=noise)
-        return a.obs, a.reward, a.term.bool(), a.trunc.bool(), self._info()
-
-    def rollout(self, n_steps: int) -> None:
-        self.aviary.env_rollout(n_steps)
-
-    def close(self) -> None:
-        self.aviary.disconnect()

@@ -5,7 +5,7 @@ throughput path is the ``*VecEnv`` classes.  Observation layouts follow the refe
 
 * ``QuadXWaypointsEnv`` / ``FixedwingWaypointsEnv``: ``{"attitude": (A,), "target_deltas": (k, T)}`` with k = targets left
   (quadx_waypoints_env.py:95-110, fixedwing_waypoints_env.py:88-101);
-* ``RocketLandingEnv``: flat vector (rocket_landing_env.py:129-188).
+* ``QuadXHoverEnv`` / ``RocketLandingEnv``: flat vector (quadx_hover_env.py:85-116, rocket_landing_env.py:129-188).
 """
 
 from __future__ import annotations
@@ -24,9 +24,7 @@ class _SingleEnv:
 
     def __init__(self, **kwargs):
         kwargs.setdefault("autoreset", False)
-        self._seed = kwargs.pop("seed", None)
-        self._kwargs = kwargs
-        self._vec = self._vec_cls(num_envs=1, seed=self._seed, **kwargs)
+        self._vec = self._vec_cls(num_envs=1, **kwargs)
         self.action_space = spaces.Box(low=self._vec.action_low, high=self._vec.action_high, dtype=np.float64)
         self.observation_space = self._make_observation_space()
 
@@ -44,10 +42,7 @@ class _SingleEnv:
         return obs[0].double().cpu().numpy()
 
     def reset(self, *, seed: None | int = None, options: None | dict[str, Any] = dict()):
-        if seed is not None:  # the same seed must replay the same episode (gymnasium contract; tests/test_gym_envs.py:92-112)
-            self._seed = int(seed)
-            self._vec.aviary.reseed(self._seed)
-        obs, info = self._vec.reset()
+        obs, info = self._vec.reset(seed=seed)  # the same seed replays the same episode (gymnasium's contract)
         info = self._info(info)
         return self._obs(obs, info), info
 
@@ -86,15 +81,17 @@ class _WaypointsMixin:
         return {"attitude": flat[:a], "target_deltas": rows[:k]}
 
 
-def _make(name, vec_import, vehicle=None, action_dim=4, doc=""):
+def _make(name, vec_import, vehicle=None, action_dim=4, doc="", **attrs):
     def _vec_cls(*a, **k):
         mod, cls = vec_import
         return getattr(__import__(mod, fromlist=[cls]), cls)(*a, **k)
 
     bases = (_WaypointsMixin, _SingleEnv) if vehicle else (_SingleEnv,)
-    return type(name, bases, {"_vec_cls": staticmethod(_vec_cls), "_action_dim": action_dim, "_vehicle": vehicle, "__doc__": doc})
+    return type(name, bases, {"_vec_cls": staticmethod(_vec_cls), "_action_dim": action_dim, "_vehicle": vehicle, "__doc__": doc, **attrs})
 
 
+QuadXHoverEnv = _make("QuadXHoverEnv", ("pyflyt_b200.gym_envs.quadx_hover_env", "QuadXHoverVecEnv"),
+                      doc="gym_envs/quadx_envs/quadx_hover_env.py:15-138 for one env.", metadata={"render_modes": [], "render_fps": 30})
 QuadXWaypointsEnv = _make("QuadXWaypointsEnv", ("pyflyt_b200.gym_envs.quadx_waypoints_env", "QuadXWaypointsVecEnv"), "quadx",
                           doc="gym_envs/quadx_envs/quadx_waypoints_env.py:14-212 for one env.")
 FixedwingWaypointsEnv = _make("FixedwingWaypointsEnv", ("pyflyt_b200.gym_envs.fixedwing_waypoints_env", "FixedwingWaypointsVecEnv"), "fixedwing",

@@ -64,10 +64,7 @@ class PyFlytVectorEnv(_Base):
         mod, cls, _ = ENV_TABLE[_stem(env_id)]
         self.spec_id = env_id
         self.output = output
-        self._seed = seed
-        self._kwargs = dict(env_kwargs, device=device)
-        self._cls = getattr(__import__(mod, fromlist=[cls]), cls)
-        self.env = self._cls(num_envs=int(num_envs), seed=seed, autoreset=True, **self._kwargs)
+        self.env = getattr(__import__(mod, fromlist=[cls]), cls)(num_envs=int(num_envs), seed=seed, autoreset=True, device=device, **env_kwargs)
         self.num_envs = int(num_envs)
         self.device = self.env.device
         dt = np.float32
@@ -85,15 +82,11 @@ class PyFlytVectorEnv(_Base):
         return {k: self._out(v) for k, v in info.items()}
 
     def reset(self, *, seed: int | list[int] | None = None, options: dict | None = None):
-        """A seed re-creates the streams: the same seed gives the same episodes (gymnasium's contract, tests/test_gym_envs.py:92-112
-        of the reference)."""
-        if seed is not None:
-            if isinstance(seed, (list, tuple)):
-                seed = int(seed[0])
-            self.env.close()
-            self._seed = int(seed)
-            self.env = self._cls(num_envs=self.num_envs, seed=self._seed, autoreset=True, **self._kwargs)
-        obs, info = self.env.reset()
+        """A seed re-keys the random streams of the batch: the same seed gives the same episodes (gymnasium's contract,
+        tests/test_gym_envs.py:92-112 of the reference).  The zero-copy tensors stay the same buffers across a seeded reset."""
+        if isinstance(seed, (list, tuple)):
+            seed = seed[0]
+        obs, info = self.env.reset(seed=seed)
         return self._out(obs), self._info(info)
 
     def step(self, actions):

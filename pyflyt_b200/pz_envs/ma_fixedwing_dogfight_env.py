@@ -22,13 +22,13 @@ from __future__ import annotations
 import numpy as np
 import torch
 
-from ..core.aviary import BatchedAviary
-from ..models import PfbEnvConfig
+from ..core.env_base import VecEnv, check_env_args, env_config
 from ..models.tables import ENV_DOGFIGHT
 
 
-class MAFixedwingDogfightVecEnv:
+class MAFixedwingDogfightVecEnv(VecEnv):
     metadata = {"render_modes": [], "name": "ma_fixedwing_dogfight"}
+    _info_flags = (("out_of_bounds", 1), ("collision", 2), ("dead", 4), ("team_win", 8))
 
     def __init__(
         self,
@@ -57,12 +57,7 @@ class MAFixedwingDogfightVecEnv:
         env_offset: int = 0,
         inline_reset: bool = False,
     ):
-        if 120 % agent_hz != 0:  # ma_fixedwing_base_env.py:43-48
-            lowest = int(120 / (int(120 / agent_hz) + 1))
-            highest = int(120 / int(120 / agent_hz))
-            raise AssertionError(f"`agent_hz` must be round denominator of 120, try {lowest} or {highest}.")
-        if render_mode is not None:
-            raise ValueError("rendering is out of scope for the batched stepper (SURVEY.md §2 row 21)")
+        check_env_args(agent_hz, render_mode, hz_error=AssertionError)  # ma_fixedwing_base_env.py:43-48
         if not assisted_flight or not flatten_observation:
             raise ValueError("the fused dogfight kernel is built for assisted_flight=True, flatten_observation=True")
         if team_size not in (1, 2):
@@ -71,39 +66,23 @@ class MAFixedwingDogfightVecEnv:
         self.agents_per_arena = 2 * self.team_size
         self.num_agents = self.num_arenas * self.agents_per_arena
         self.possible_agents = [f"uav_{r}" for r in range(self.agents_per_arena)]
-        cfg = PfbEnvConfig()
-        cfg.env_kind = ENV_DOGFIGHT
-        cfg.flight_mode = 0
-        cfg.env_step_ratio = int(120 / agent_hz)
-        cfg.max_steps = int(agent_hz * max_duration_seconds)
-        cfg.angle_representation = 0  # ma_fixedwing_dogfight_env.py:92: "euler"
-        cfg.sparse_reward = int(bool(sparse_reward))
-        cfg.autoreset = int(bool(autoreset))
-        cfg.warmup_steps = 10
-        cfg.flight_dome_size = float(flight_dome_size)
-        cfg.team_size = self.team_size
-        cfg.damage_per_hit, cfg.lethal_distance, cfg.lethal_angle = float(damage_per_hit), float(lethal_distance), float(lethal_angle_radians)
-        cfg.aggressiveness, cfg.cooperativeness = float(aggressiveness), float(cooperativeness)
-        cfg.spawn_min_radius, cfg.spawn_max_radius = float(spawn_min_radius), float(spawn_max_radius)
-        cfg.spawn_min_height, cfg.spawn_max_height = float(spawn_min_height), float(spawn_max_height)
-        cfg.randomize_drop = int(bool(random_spawn))  # draw the spawn on device like _get_start_pos_orn
-        cfg.inline_reset = int(bool(inline_reset))  # tests: spare-copy arena resets must equal inline ones bit for bit
-        self.config = cfg
+        cfg = env_config(ENV_DOGFIGHT, agent_hz=agent_hz, max_duration_seconds=max_duration_seconds,
+                         angle_representation="euler",  # ma_fixedwing_dogfight_env.py:92
+                         sparse_reward=sparse_reward, autoreset=autoreset, flight_dome_size=flight_dome_size, inline_reset=inline_reset,
+                         team_size=self.team_size, damage_per_hit=float(damage_per_hit), lethal_distance=float(lethal_distance),
+                         lethal_angle=float(lethal_angle_radians), aggressiveness=float(aggressiveness),
+                         cooperativeness=float(cooperativeness), spawn_min_radius=float(spawn_min_radius),
+                         spawn_max_radius=float(spawn_max_radius), spawn_min_height=float(spawn_min_height),
+                         spawn_max_height=float(spawn_max_height),
+                         randomize_drop=int(bool(random_spawn)))  # draw the spawn on device like _get_start_pos_orn
         n = self.num_agents
-        self.aviary = BatchedAviary(np.zeros((n, 3)), np.zeros((n, 3)), drone_type="fixedwing", drone_options=dict(drone_model="acrowing"),
-                                    seed=seed, device=device, env_config=cfg, env_offset=env_offset)
-        self.device = self.aviary.device
-        self.obs_dim = self.aviary.obs_dim
+        super().__init__(cfg, np.zeros((n, 3)), np.zeros((n, 3)), "fixedwing", drone_options=dict(drone_model="acrowing"), seed=seed,
+                         device=device, env_offset=env_offset)
 
     def _info(self):
-        bits = self.aviary.info_bits
-        return {
-            "out_of_bounds": (bits & 1).bool(),
-            "collision": (bits & 2).bool(),
-            "dead": (bits & 4).bool(),
-            "team_win": (bits & 8).bool(),
-            "health": self.aviary.state_tensor[30],  # DF_HEALTH row
-        }
+        info = super()._info()
+        info["health"] = self.aviary.state_tensor[30]  # DF_HEALTH row
+        return info
 
     def set_spawn(self, start_pos, start_orn):
         """Explicit spawn poses [num_agents, 3] used by reset() when ``random_spawn=False``."""
@@ -111,20 +90,4 @@ class MAFixedwingDogfightVecEnv:
         self.aviary.start_orn.copy_(torch.as_tensor(start_orn, dtype=torch.float32, device=self.device).reshape(-1, 3))
 
     def reset(self, *, seed: int | None = None, options: dict | None = None, noise=None):
-        obs = self.aviary.env_reset(noise=noise, seed=seed)
-        self.aviary.info_bits.zero_()
-        return obs, self._info()
-
-    def step(self, actions: torch.Tensor, noise=None):
-        a = self.aviary
-        if not (torch.is_tensor(actions) and actions.is_cuda and actions.dtype == torch.float32 and actions.is_contiguous()):
-            a.setpoints.copy_(torch.as_tensor(actions, dtype=torch.float32, device=self.device).reshape(self.num_agents, 4))
-            actions = None
-        a.env_step(actions=actions, noise=noise)
-        return a.obs, a.reward, a.term.bool(), a.trunc.bool(), self._info()
-
-    def rollout(self, n_steps: int) -> None:
-        self.aviary.env_rollout(n_steps)
-
-    def close(self) -> None:
-        self.aviary.disconnect()
+        return self._reset(noise=noise, seed=seed)

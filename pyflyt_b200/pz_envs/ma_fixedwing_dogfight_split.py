@@ -30,7 +30,7 @@ import torch
 import torch.distributed as dist
 
 from ..core.aviary import BatchedAviary
-from ..models import PfbEnvConfig
+from ..core.env_base import env_config
 from ..models.tables import ENV_DOGFIGHT
 
 PAYLOAD = 20
@@ -74,21 +74,12 @@ class MAFixedwingDogfightSplitEnv:
         self.n_local = end - self.first_gid
         self.seed = 0 if seed is None else int(seed)
         self.spawn = (float(spawn_min_radius), float(spawn_max_radius))
-        cfg = PfbEnvConfig()
-        cfg.env_kind = ENV_DOGFIGHT
-        cfg.flight_mode = 0
-        cfg.env_step_ratio = int(120 / agent_hz)
-        cfg.max_steps = int(agent_hz * max_duration_seconds)
-        cfg.angle_representation = 0
-        cfg.sparse_reward = int(bool(sparse_reward))
-        cfg.autoreset = 0
-        cfg.warmup_steps = 10
-        cfg.flight_dome_size = float(flight_dome_size)
-        cfg.team_size = 1
-        cfg.damage_per_hit, cfg.lethal_distance, cfg.lethal_angle = float(damage_per_hit), float(lethal_distance), float(lethal_angle_radians)
-        cfg.aggressiveness, cfg.cooperativeness = float(aggressiveness), float(cooperativeness)
-        cfg.spawn_min_radius, cfg.spawn_max_radius = self.spawn
-        cfg.spawn_min_height, cfg.spawn_max_height = self.spawn
+        cfg = env_config(ENV_DOGFIGHT, agent_hz=agent_hz, max_duration_seconds=max_duration_seconds, angle_representation="euler",
+                         sparse_reward=sparse_reward, autoreset=False, flight_dome_size=flight_dome_size, team_size=1,
+                         damage_per_hit=float(damage_per_hit), lethal_distance=float(lethal_distance), lethal_angle=float(lethal_angle_radians),
+                         aggressiveness=float(aggressiveness), cooperativeness=float(cooperativeness),
+                         spawn_min_radius=self.spawn[0], spawn_max_radius=self.spawn[1],
+                         spawn_min_height=self.spawn[0], spawn_max_height=self.spawn[1])  # (sic) heights take the radius range, as spawn_poses
         self.config = cfg
         n = self.n_local
         # env_offset = first global agent id: the noise streams are keyed by gid, so they do not depend on the world size

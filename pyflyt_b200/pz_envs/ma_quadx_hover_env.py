@@ -22,16 +22,15 @@ from typing import Literal
 import numpy as np
 import torch
 
-from ..core.aviary import BatchedAviary
-from ..models import PfbEnvConfig
-
-ENV_MA_QUADX_HOVER = 6
+from ..core.env_base import AviaryEnv, check_env_args, env_config
+from ..models.tables import ENV_MA_QUADX_HOVER
 
 _DEFAULT_START = np.array([[-1.0, -1.0, 1.0], [1.0, -1.0, 1.0], [-1.0, 1.0, 1.0], [1.0, 1.0, 1.0]])  # ma_quadx_hover_env.py:39-41
 
 
-class MAQuadXHoverVecEnv:
+class MAQuadXHoverVecEnv(AviaryEnv):
     metadata = {"render_modes": [], "name": "ma_quadx_hover"}
+    _info_flags = (("out_of_bounds", 1), ("collision", 2))
 
     def __init__(
         self,
@@ -50,14 +49,7 @@ class MAQuadXHoverVecEnv:
         device: str | torch.device = "cuda:0",
         env_offset: int = 0,
     ):
-        if 120 % agent_hz != 0:  # ma_quadx_base_env.py:47-52
-            lowest = int(120 / (int(120 / agent_hz) + 1))
-            highest = int(120 / int(120 / agent_hz))
-            raise AssertionError(f"`agent_hz` must be round denominator of 120, try {lowest} or {highest}.")
-        if render_mode is not None:
-            raise ValueError("rendering is out of scope for the batched stepper (SURVEY.md §2 row 21)")
-        if angle_representation not in ("euler", "quaternion"):
-            raise ValueError(f"angle_representation must be either `euler` or `quaternion`, not {angle_representation}")
+        check_env_args(agent_hz, render_mode, angle_representation, hz_error=AssertionError)  # ma_quadx_base_env.py:47-52
         start_pos = np.asarray(start_pos, dtype=np.float64).reshape(-1, 3)
         start_orn = np.zeros_like(start_pos) if start_orn is None else np.asarray(start_orn, dtype=np.float64).reshape(-1, 3)
         assert start_orn.shape == start_pos.shape
@@ -65,35 +57,26 @@ class MAQuadXHoverVecEnv:
         self.num_agents = self.num_arenas * self.agents_per_arena
         self.possible_agents = [f"uav_{r}" for r in range(self.agents_per_arena)]
         self.autoreset = bool(autoreset)
-        cfg = PfbEnvConfig()
-        cfg.env_kind = ENV_MA_QUADX_HOVER
-        cfg.flight_mode = int(flight_mode)
-        cfg.env_step_ratio = int(120 / agent_hz)
-        cfg.max_steps = int(agent_hz * max_duration_seconds)
-        cfg.angle_representation = 0 if angle_representation == "euler" else 1
-        cfg.sparse_reward = int(bool(sparse_reward))
-        cfg.autoreset = 0  # arenas are reset from here, with a mask
-        cfg.warmup_steps = 10  # ma_quadx_base_env.py:241-243
-        cfg.flight_dome_size = float(flight_dome_size)
-        self.config = cfg
+        cfg = env_config(ENV_MA_QUADX_HOVER, agent_hz=agent_hz, max_duration_seconds=max_duration_seconds,
+                         angle_representation=angle_representation, sparse_reward=sparse_reward,
+                         autoreset=False,  # arenas are reset from here, with a mask
+                         flight_dome_size=flight_dome_size, flight_mode=int(flight_mode))
         sp, so = np.tile(start_pos, (self.num_arenas, 1)), np.tile(start_orn, (self.num_arenas, 1))
-        self.aviary = BatchedAviary(sp, so, drone_type="quadx", seed=seed, device=device, env_config=cfg, env_offset=env_offset)
-        self.device = self.aviary.device
-        self.obs_dim = self.aviary.obs_dim
+        super().__init__(cfg, sp, so, "quadx", seed=seed, device=device, env_offset=env_offset)
         n = self.num_agents
         self.alive = torch.ones(n, dtype=torch.bool, device=self.device)  # the agents still in self.agents
         self._mask = torch.zeros(n, dtype=torch.uint8, device=self.device)
         self._act = torch.zeros((n, 4), dtype=torch.float32, device=self.device)
 
     def _info(self):
-        bits = self.aviary.info_bits
-        return {"out_of_bounds": (bits & 1).bool(), "collision": (bits & 2).bool(), "alive": self.alive}
+        info = super()._info()
+        info["alive"] = self.alive
+        return info
 
     def reset(self, *, seed: int | None = None, options: dict | None = None, noise=None):
-        obs = self.aviary.env_reset(noise=noise, seed=seed)
-        self.aviary.info_bits.zero_()
+        obs, info = self._reset(noise=noise, seed=seed)
         self.alive.fill_(True)
-        return obs, self._info()
+        return obs, info
 
     def step(self, actions: torch.Tensor, noise=None):
         """``actions`` [num_agents, 4].  Returns (obs, reward, term, trunc, info); rows of culled agents hold their frozen
@@ -122,6 +105,3 @@ class MAQuadXHoverVecEnv:
             info["final_obs"] = a.final_obs      # valid in the rows where info["reset"] is set
             info["reset"] = self._mask.bool()
         return a.obs, reward, term, trunc, info
-
-    def close(self) -> None:
-        self.aviary.disconnect()

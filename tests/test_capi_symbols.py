@@ -51,6 +51,18 @@ def test_no_cpu_fallback(L):
         BatchedAviary(np.zeros((2, 3)), np.zeros((2, 3)))
 
 
+@pytest.mark.parametrize("value", [2, -1])
+def test_create_refuses_inline_reset_other_than_0_or_1(L, value):
+    """``inline_reset`` is a flag; the check comes before the device lookup, so it is the same with and without a GPU."""
+    from engines import hover_config
+
+    env = hover_config(autoreset=True)
+    env.inline_reset = value
+    h = ctypes.c_void_p()
+    assert L.pfb_create(ctypes.byref(build_model("quadx")), ctypes.byref(env), 8, 0, 0, ctypes.byref(h)) != 0 and not h.value
+    assert L.pfb_last_error() == f"inline_reset must be 0 or 1, got {value}".encode()
+
+
 def test_aviary_argument_checks_match_reference_messages():
     import numpy as np
 
