@@ -170,9 +170,12 @@ typedef struct PfbEnvConfig {
                               * step launch instead (same results, longer launches; tests).  pfb_create refuses other values */
   double damage_per_hit, lethal_distance, lethal_angle, aggressiveness, cooperativeness;
   double spawn_min_radius, spawn_max_radius, spawn_min_height, spawn_max_height;
-  int32_t contact_response;  /* Rocket-Landing: 1 = ground / pad contact RESPONSE (sequential-impulse normal + Coulomb friction
-                              * on the collision primitives' corner / rim points; a restatement, see DESIGN.md): a gentle touchdown
-                              * rests on the pad and reaches env_complete (rocket_landing_env.py:231-263).  0 = contact FLAG only  */
+  int32_t contact_response;  /* 1 = ground / pad contact RESPONSE (sequential-impulse normal + Coulomb friction on the collision
+                              * primitives' corner / rim points; a restatement, see DESIGN.md), 0 = contact FLAG only.  Read by
+                              * Rocket-Landing (a gentle touchdown rests on the pad and reaches env_complete,
+                              * rocket_landing_env.py:231-263) and by Aviary handles (env_kind PFB_ENV_NONE: QuadX, fixed-wing and
+                              * rocket drones land on, slide along and rest on the floor).  pfb_create reads no other field of a
+                              * PFB_ENV_NONE config.  The other env kinds ignore it (they terminate on the first contact).         */
   int32_t _pad_cr;
 } PfbEnvConfig;
 

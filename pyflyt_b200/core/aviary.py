@@ -13,6 +13,12 @@ to ``MAX_QUADX_MODELS`` different vehicle tables (``models``), drone ``i`` the t
 at the same ``control_hz``.  Drones ``32 k .. 32 k + 31`` share one warp: a batch runs fastest when each such tile flies one
 model (DESIGN.md §4a).
 
+The floor: the reference's Aviary is a PyBullet world, so a drone that reaches the floor stands on it.  Here, by default, the
+floor only raises ``contact_array`` and a drone keeps falling through ``z = 0`` (the envs end an episode on the first
+contact, so they never need more).  ``contact_response=True`` makes the floor push back on QuadX, fixed-wing and rocket
+drones: contact impulses with Coulomb friction on the corners / rim points of each drone's collision primitives, so drones
+take off from, land on, slide along and rest on the floor (DESIGN.md §4c).
+
 All state is held in caller-visible ``torch`` tensors; the CUDA library (libpyflyt_b200.so) only sees
 raw device pointers.  There is no CPU path.
 """
@@ -56,7 +62,12 @@ class BatchedAviary:
         device: str | torch.device = "cuda:0",
         env_config: PfbEnvConfig | None = None,
         env_offset: int = 0,
+        contact_response: bool = False,
     ):
+        """``contact_response``: the floor pushes back (contact impulses + Coulomb friction) instead of only raising
+        ``contact_array``.  The reference always responds, since every ``Aviary`` is a PyBullet world; here it is opt-in so
+        that a handle built without it steps exactly as before, and so that flight far above the floor never pays for the
+        solver.  Aviary handles only: an env handle (``env_config``) has its own contact policy."""
         start_pos = np.asarray(start_pos, dtype=np.float32)
         start_orn = np.asarray(start_orn, dtype=np.float32)
         # shape checks with the reference's messages (aviary.py:120-131)
@@ -93,6 +104,12 @@ class BatchedAviary:
             control_hz = int(models[0].control_hz)
             self.model = models[0]
             self.models = models
+        if contact_response:
+            if env_config is not None:
+                raise AviaryInitException("contact_response is an Aviary-handle option; an env handle (env_config) keeps its own contact policy.")
+            env_config = PfbEnvConfig()  # env kind NONE: pfb_create reads only contact_response from it
+            env_config.contact_response = 1
+        self.contact_response = bool(contact_response)
         self.env_config = env_config
         self.updates_per_step = int(physics_hz / control_hz)  # aviary.py:288-289 (single control rate)
         self.step_period = 1.0 / control_hz

@@ -132,6 +132,10 @@ static inline int grid_for(int64_t n) { return (int)((n + kBlock - 1) / kBlock);
     (h)->launches += 1;                                                     \
   } while (0)
 
+// An Aviary handle (no env epilogue) whose config asked for the contact RESPONSE: the QuadX and fixed-wing Aviary steps run
+// their CONTACT instantiations.  The rocket carries the switch in RocketParams.contact_response; env handles ignore it.
+static inline bool aviary_contact_response(const PfbContext* h) { return h->env.env_kind == PFB_ENV_NONE && h->env.contact_response != 0; }
+
 // QuadX state layout: warp-tiled (pfb_quadx.cuh) on every QuadX handle except QuadX-Waypoints (field-major rows + istate)
 static inline bool qx_tiled(const PfbContext* h) { return h->model.kind == PFB_KIND_QUADX && h->env.env_kind != PFB_ENV_QUADX_WAYPOINTS; }
 static inline int qx_rows(const PfbContext* h) { return h->env.env_kind == PFB_ENV_MA_QUADX_HOVER ? (int)pfb::QM_ROWS : (int)pfb::QX_ROWS; }

@@ -40,7 +40,8 @@ __global__ void __launch_bounds__(kBlock) k_fw_reset(const __grid_constant__ Fix
     for (int k = 0; k < sp_dim; ++k) setpoint[(int64_t)sp_dim * i + k] = 0.0f;
 }
 
-template <int MODE, bool INJECT>
+// CONTACT: the ground pushes back (Aviary handles with contact_response)
+template <int MODE, bool INJECT, bool CONTACT>
 __global__ void __launch_bounds__(kBlock, kMinBlocks)
     k_fw_aviary_step(const __grid_constant__ FixedwingParams p, const __grid_constant__ RngParams rng, float* __restrict__ st,
                      int32_t* __restrict__ ist, const float* __restrict__ setpoint, const float* __restrict__ noise,
@@ -53,15 +54,15 @@ __global__ void __launch_bounds__(kBlock, kMinBlocks)
   for (int k = 0; k < 6; ++k) s.sp[k] = k < sp_dim ? __ldg(setpoint + (int64_t)sp_dim * i + k) : 0.0f;
   auto nz = make_noise<INJECT>(noise, N, i, rng, seq, TAG_AVIARY, p.noise_loc, p.ratio);
   if (fixedwing_full_model(p)) {  // launch-uniform: all surfaces, no wind -> the one-basic-block substep (pfb_fixedwing.cuh)
-    for (int k = 0; k < n_steps; ++k) fixedwing_aviary_step<MODE, true>(p, s, nz);
+    for (int k = 0; k < n_steps; ++k) fixedwing_aviary_step<MODE, true, CONTACT>(p, s, nz);
   } else {
-    for (int k = 0; k < n_steps; ++k) fixedwing_aviary_step<MODE>(p, s, nz);
+    for (int k = 0; k < n_steps; ++k) fixedwing_aviary_step<MODE, false, CONTACT>(p, s, nz);
   }
   fixedwing_store(st, ist, N, i, s);
 }
 
 // k_fw_aviary_step with drone i in flight mode modes[i] (pfb_set_modes): only the command mapping branches on the mode
-template <bool FULL, typename NoiseFn>
+template <bool FULL, bool CONTACT, typename NoiseFn>
 __device__ __forceinline__ void fixedwing_aviary_step_any(const FixedwingParams& p, FixedwingRegs& s, int mode, NoiseFn& noise) {
   s.flags &= ~(uint32_t)FLAG_CONTACT_ARRAY;
   noise.begin_step();
@@ -69,10 +70,10 @@ __device__ __forceinline__ void fixedwing_aviary_step_any(const FixedwingParams&
   if (mode == -1) fixedwing_command<-1>(s, cmd);
   else fixedwing_command<0>(s, cmd);
 #pragma unroll 1
-  for (int u = 0; u < p.ratio; ++u) fixedwing_substep<FULL>(p, s, cmd, noise.get(u));
+  for (int u = 0; u < p.ratio; ++u) fixedwing_substep<FULL, CONTACT>(p, s, cmd, noise.get(u));
 }
 
-template <bool INJECT>
+template <bool INJECT, bool CONTACT>
 __global__ void __launch_bounds__(kBlock, kMinBlocks)
     k_fw_aviary_step_modes(const __grid_constant__ FixedwingParams p, const __grid_constant__ RngParams rng, float* __restrict__ st,
                            int32_t* __restrict__ ist, const float* __restrict__ setpoint, const int8_t* __restrict__ modes,
@@ -86,9 +87,9 @@ __global__ void __launch_bounds__(kBlock, kMinBlocks)
   for (int k = 0; k < 6; ++k) s.sp[k] = __ldg(setpoint + (int64_t)6 * i + k);  // Aviary handles: 6-wide setpoints
   auto nz = make_noise<INJECT>(noise, N, i, rng, seq, TAG_AVIARY, p.noise_loc, p.ratio);
   if (fixedwing_full_model(p)) {
-    for (int k = 0; k < n_steps; ++k) fixedwing_aviary_step_any<true>(p, s, mode, nz);
+    for (int k = 0; k < n_steps; ++k) fixedwing_aviary_step_any<true, CONTACT>(p, s, mode, nz);
   } else {
-    for (int k = 0; k < n_steps; ++k) fixedwing_aviary_step_any<false>(p, s, mode, nz);
+    for (int k = 0; k < n_steps; ++k) fixedwing_aviary_step_any<false, CONTACT>(p, s, mode, nz);
   }
   fixedwing_store(st, ist, N, i, s);
 }
@@ -400,21 +401,35 @@ int fw_set_modes(PfbContext* h, cudaStream_t s) {
 int fw_aviary_step(PfbContext* h, int n_steps, const float* noise, cudaStream_t s) {
   const uint32_t seq = (uint32_t)h->aviary_seq++;
   const int g = grid_for(h->n);
+  const bool contact = aviary_contact_response(h);
   if (h->mode == kModePerDrone) {  // pfb_set_modes: Aviary handles only (6-wide setpoints)
 #define FWM_ARGS h->fw, h->rng, h->buf.state, h->buf.istate, h->buf.setpoint, h->d_modes, noise, n_steps, seq, h->n
-    if (noise) k_fw_aviary_step_modes<true><<<g, kBlock, 0, s>>>(FWM_ARGS);
-    else k_fw_aviary_step_modes<false><<<g, kBlock, 0, s>>>(FWM_ARGS);
+    if (contact) {
+      if (noise) k_fw_aviary_step_modes<true, true><<<g, kBlock, 0, s>>>(FWM_ARGS);
+      else k_fw_aviary_step_modes<false, true><<<g, kBlock, 0, s>>>(FWM_ARGS);
+    } else {
+      if (noise) k_fw_aviary_step_modes<true, false><<<g, kBlock, 0, s>>>(FWM_ARGS);
+      else k_fw_aviary_step_modes<false, false><<<g, kBlock, 0, s>>>(FWM_ARGS);
+    }
 #undef FWM_ARGS
     LAUNCH_CHECK(h);
     return 0;
   }
 #define FW_ARGS h->fw, h->rng, h->buf.state, h->buf.istate, h->buf.setpoint, noise, n_steps, seq, fw_setpoint_dim(h), h->n
-  if (h->mode == 0) {
-    if (noise) k_fw_aviary_step<0, true><<<g, kBlock, 0, s>>>(FW_ARGS);
-    else k_fw_aviary_step<0, false><<<g, kBlock, 0, s>>>(FW_ARGS);
+  if (contact) {
+    if (h->mode == 0) {
+      if (noise) k_fw_aviary_step<0, true, true><<<g, kBlock, 0, s>>>(FW_ARGS);
+      else k_fw_aviary_step<0, false, true><<<g, kBlock, 0, s>>>(FW_ARGS);
+    } else {
+      if (noise) k_fw_aviary_step<-1, true, true><<<g, kBlock, 0, s>>>(FW_ARGS);
+      else k_fw_aviary_step<-1, false, true><<<g, kBlock, 0, s>>>(FW_ARGS);
+    }
+  } else if (h->mode == 0) {
+    if (noise) k_fw_aviary_step<0, true, false><<<g, kBlock, 0, s>>>(FW_ARGS);
+    else k_fw_aviary_step<0, false, false><<<g, kBlock, 0, s>>>(FW_ARGS);
   } else {
-    if (noise) k_fw_aviary_step<-1, true><<<g, kBlock, 0, s>>>(FW_ARGS);
-    else k_fw_aviary_step<-1, false><<<g, kBlock, 0, s>>>(FW_ARGS);
+    if (noise) k_fw_aviary_step<-1, true, false><<<g, kBlock, 0, s>>>(FW_ARGS);
+    else k_fw_aviary_step<-1, false, false><<<g, kBlock, 0, s>>>(FW_ARGS);
   }
 #undef FW_ARGS
   LAUNCH_CHECK(h);

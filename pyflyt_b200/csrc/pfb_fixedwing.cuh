@@ -202,12 +202,122 @@ PFB_HD bool ground_contact(const ContactParams& cp, float pz, float r20, float r
   return hit;
 }
 
+// ---- contact RESPONSE (opt-in: PfbEnvConfig.contact_response): the arithmetic of oracle/fakebullet/pybullet.py::_solve_contacts
+// and oracle/pfb_oracle.c::solve_contacts, in the BODY frame (the inverse central inertia is constant there): candidate points =
+// 8 per collision primitive (box corners; 4 + 4 cylinder rim points), kContactIterations sweeps, per penetrating point a
+// non-accumulated normal impulse (restitution 0, Baumgarte bias erp * (depth - slop) / dt) then Coulomb friction.  A
+// restatement of a Bullet-like sequential impulse, unpinned (DESIGN.md).  COLD: only called on substeps whose contact flag
+// is up; everything by value so that the caller's registers never have their address taken.
+constexpr int kContactIterations = 8;
+constexpr float kContactErp = 0.2f, kContactSlop = 0.001f, kContactFriction = 0.5f;
+struct ContactVel { float vx, vy, vz, wx, wy, wz; int touched; };
+
+// The primitive list the solver walks: a ContactParams (fixed-wing, rocket: any orientation) or the QuadX table's own
+// shape_kind / shape_dims / shape_at arrays (axis-aligned), read in place so that QuadXParams keeps its layout
+PFB_HD int contact_n_shapes(const ContactParams& c) { return c.n_shapes; }
+PFB_HD int contact_kind(const ContactParams& c, int k) { return c.kind[k]; }
+PFB_HD const float* contact_dims(const ContactParams& c, int k) { return c.dims[k]; }
+// point (lx, ly, lz) of primitive k's own frame, in the base frame
+PFB_HD Vec3 contact_point(const ContactParams& c, int k, float lx, float ly, float lz) {
+  const float* q = c.rot[k];
+  return Vec3{c.at[k][0] + q[0] * lx + q[1] * ly + q[2] * lz, c.at[k][1] + q[3] * lx + q[4] * ly + q[5] * lz, c.at[k][2] + q[6] * lx + q[7] * ly + q[8] * lz};
+}
+PFB_HD int contact_n_shapes(const QuadXParams& p) { return p.n_shapes; }
+PFB_HD int contact_kind(const QuadXParams& p, int k) { return p.shape_kind[k]; }
+PFB_HD const float* contact_dims(const QuadXParams& p, int k) { return p.shape_dims[k]; }
+PFB_HD Vec3 contact_point(const QuadXParams& p, int k, float lx, float ly, float lz) {
+  return Vec3{p.shape_at[k][0] + lx, p.shape_at[k][1] + ly, p.shape_at[k][2] + lz};
+}
+
+template <class Shapes>
+#if defined(__CUDACC__)
+static __host__ __device__ __noinline__
+#else
+inline
+#endif
+ContactVel solve_contacts(const Shapes* cp, float pz, float top, Vec3 n /* world z in the body frame = third row of R */, Vec3 vb,
+                          Vec3 w, float M, Vec3 c, float Ixx, float Ixy, float Ixz, float Iyy, float Iyz, float Izz, float dt) {
+  // inverse of the symmetric central inertia (cofactors)
+  const float c00 = Iyy * Izz - Iyz * Iyz, c01 = Ixz * Iyz - Ixy * Izz, c02 = Ixy * Iyz - Ixz * Iyy;
+  const float c11 = Ixx * Izz - Ixz * Ixz, c12 = Ixy * Ixz - Ixx * Iyz, c22 = Ixx * Iyy - Ixy * Ixy;
+  const float id = 1.0f / (Ixx * c00 + Ixy * c01 + Ixz * c02), iM = 1.0f / M;
+  auto Iinv = [&](Vec3 r) { return Vec3{(c00 * r.x + c01 * r.y + c02 * r.z) * id, (c01 * r.x + c11 * r.y + c12 * r.z) * id, (c02 * r.x + c12 * r.y + c22 * r.z) * id}; };
+  Vec3 vc = vb + cross(w, c);  // COM velocity, body frame
+  int touched = 0;
+  for (int it = 0; it < kContactIterations; ++it) {
+    for (int sh = 0; sh < contact_n_shapes(*cp); ++sh) {
+      const int kind = contact_kind(*cp, sh);
+      if (kind > 1) continue;  // boxes and cylinders
+      const float* dims = contact_dims(*cp, sh);
+      for (int j = 0; j < 8; ++j) {
+        const float sz = (j & 4) ? 1.0f : -1.0f;
+        float lx, ly, lz;
+        if (kind == 0) {
+          lx = ((j & 1) ? 1.0f : -1.0f) * dims[0]; ly = ((j & 2) ? 1.0f : -1.0f) * dims[1]; lz = sz * dims[2];
+        } else {
+          const int a = j & 3;
+          lx = dims[0] * (a == 0 ? 1.0f : (a == 2 ? -1.0f : 0.0f)); ly = dims[0] * (a == 1 ? 1.0f : (a == 3 ? -1.0f : 0.0f));
+          lz = sz * dims[1];
+        }
+        const Vec3 pb = contact_point(*cp, sh, lx, ly, lz);
+        const float depth = top - (pz + dot(n, pb));
+        if (depth <= 0.0f) continue;
+        touched = 1;
+        const Vec3 r = pb - c;
+        Vec3 u = vc + cross(w, r);
+        const Vec3 rn = cross(r, n), Irn = Iinv(rn);
+        const float kn = iM + dot(rn, Irn);
+        const float bias = kContactErp * fmaxf(depth - kContactSlop, 0.0f) / dt;
+        const float jn = fmaxf(0.0f, (bias - dot(u, n)) / kn);
+        if (jn > 0.0f) {
+          vc = vc + (jn * iM) * n;
+          w = w + jn * Irn;
+          u = vc + cross(w, r);
+          const Vec3 ut = u - dot(u, n) * n;
+          const float sp = sqrtf(dot(ut, ut));
+          if (sp > 1e-9f) {
+            const Vec3 t = (1.0f / sp) * ut, rt = cross(r, t), Irt = Iinv(rt);
+            const float kt = iM + dot(rt, Irt);
+            const float jt = fminf(sp / kt, kContactFriction * jn);
+            vc = vc - (jt * iM) * t;
+            w = w - jt * Irt;
+          }
+        }
+      }
+    }
+  }
+  const Vec3 vo = vc - cross(w, c);
+  return ContactVel{vo.x, vo.y, vo.z, w.x, w.y, w.z, touched};
+}
+
+// Contact impulses on the predicted velocities of `s` (world linear velocity, body angular velocity), before its pose is
+// integrated: the solve runs in the body frame of the pose at the START of the substep (rotation s.R, base altitude pz0).
+// M, c, I..: mass, COM offset and inertia about the COM (base frame).
+template <class Shapes, class Regs>
+PFB_HD void apply_contact_impulses(const Shapes* cp, Regs& s, float pz0, float top, float M, Vec3 c, float Ixx, float Ixy, float Ixz,
+                                   float Iyy, float Iyz, float Izz, float dt) {
+  const float m00 = (float)s.R.m00, m01 = (float)s.R.m01, m02 = (float)s.R.m02, m10 = (float)s.R.m10, m11 = (float)s.R.m11,
+              m12 = (float)s.R.m12, m20 = (float)s.R.m20, m21 = (float)s.R.m21, m22 = (float)s.R.m22;
+  const float vwx = (float)s.vx, vwy = (float)s.vy, vwz = (float)s.vz;
+  const Vec3 vbn = Vec3{m00 * vwx + m10 * vwy + m20 * vwz, m01 * vwx + m11 * vwy + m21 * vwz, m02 * vwx + m12 * vwy + m22 * vwz};
+  const ContactVel cv = solve_contacts(cp, pz0, top, Vec3{m20, m21, m22}, vbn, Vec3{s.wx, s.wy, s.wz}, M, c, Ixx, Ixy, Ixz, Iyy, Iyz, Izz, dt);
+  if (cv.touched) {
+    s.vx = (vreal)(m00 * cv.vx + m01 * cv.vy + m02 * cv.vz);
+    s.vy = (vreal)(m10 * cv.vx + m11 * cv.vy + m12 * cv.vz);
+    s.vz = (vreal)(m20 * cv.vx + m21 * cv.vy + m22 * cv.vz);
+    s.wx = cv.wx; s.wy = cv.wy; s.wz = cv.wz;
+  }
+}
+
 // Bullet free-body step for a composite body with COM offset c and full inertia I_O (SURVEY §A.3):
 //   F = M (a_O + wdot x c + w x (w x c)),   T_O = I_O wdot + w x I_O w + M c x a_O
 // F_b / T_b: external force / torque about O in the body frame (without gravity).  State update is the
 // same semi-implicit Euler + body-frame exp-map as the quad.
-template <typename Regs>
-PFB_HD void rigid_step(const RigidParams& rb, float gravity, float dt_f, float vmax_f, Regs& s, Vec3 F, Vec3 T) {
+// CONTACT: contact impulses over `cp` on the predicted velocities when `touching` (the substep's contact flag), before the
+// pose is integrated.
+template <bool CONTACT = false, typename Regs>
+PFB_HD void rigid_step(const RigidParams& rb, float gravity, float dt_f, float vmax_f, Regs& s, Vec3 F, Vec3 T,
+                       const ContactParams* cp = nullptr, bool touching = false) {
   typedef decltype(s.R.m00) RT;  // the body's rotation-matrix precision (fwreal for aircraft, rreal for the rocket)
   const Rot<RT>& R = s.R;
   const float r20 = (float)R.m20, r21 = (float)R.m21, r22 = (float)R.m22;
@@ -244,9 +354,11 @@ PFB_HD void rigid_step(const RigidParams& rb, float gravity, float dt_f, float v
     s.vy = fmin(fmax(s.vy, -vmax), vmax);
     s.vz = fmin(fmax(s.vz, -vmax), vmax);
   }
-  s.px += (xreal)(s.vx * dt);
-  s.py += (xreal)(s.vy * dt);
-  s.pz += (xreal)(s.vz * dt);
+  if (!CONTACT) {  // the contact impulses below change the velocities the positions move with
+    s.px += (xreal)(s.vx * dt);
+    s.py += (xreal)(s.vy * dt);
+    s.pz += (xreal)(s.vz * dt);
+  }
   s.wx = fmaf(sol[3], dt_f, s.wx);
   s.wy = fmaf(sol[4], dt_f, s.wy);
   s.wz = fmaf(sol[5], dt_f, s.wz);
@@ -254,6 +366,18 @@ PFB_HD void rigid_step(const RigidParams& rb, float gravity, float dt_f, float v
     Mat3 Rf{(float)R.m00, (float)R.m01, (float)R.m02, (float)R.m10, (float)R.m11, (float)R.m12, (float)R.m20, (float)R.m21, (float)R.m22};
     Vec3 wc = quadx_clamp_world_rates(vmax_f, Rf, Vec3{s.wx, s.wy, s.wz});
     s.wx = wc.x; s.wy = wc.y; s.wz = wc.z;
+  }
+  if (CONTACT) {
+    if (touching) {  // cold: about the COM c = mc / M, inertia I_O - M (|c|^2 E - c c^T)
+      const float M = rb.mass, iM = 1.0f / M;
+      const Vec3 c = Vec3{rb.mc[0] * iM, rb.mc[1] * iM, rb.mc[2] * iM};
+      const float c2 = dot(c, c);
+      apply_contact_impulses(cp, s, (float)s.pz, 0.0f, M, c, rb.I[0] - M * (c2 - c.x * c.x), rb.I[1] + M * c.x * c.y, rb.I[2] + M * c.x * c.z,
+                             rb.I[4] - M * (c2 - c.y * c.y), rb.I[5] + M * c.y * c.z, rb.I[8] - M * (c2 - c.z * c.z), dt_f);
+    }
+    s.px += (xreal)(s.vx * dt);
+    s.py += (xreal)(s.vy * dt);
+    s.pz += (xreal)(s.vz * dt);
   }
   float h2 = (s.wx * s.wx + s.wy * s.wy + s.wz * s.wz) * (0.25f * dt_f * dt_f);
   float sinc = fmaf(h2, fmaf(h2, fmaf(h2, fmaf(h2, 2.7557319e-6f, -1.9841270e-4f), 8.3333333e-3f), -1.6666667e-1f), 1.0f);
@@ -304,7 +428,8 @@ PFB_HD void fixedwing_command(const FixedwingRegs& s, float* cmd) {
 // pace of its own dependency chain (atan2 -> stall selects -> sincos -> coefficients -> force).  With < 1 warp per scheduler
 // at the batch sizes these vehicles run at (16 384 envs) instruction-level parallelism is the only latency hiding there is:
 // FULL removes the tests at compile time, the surfaces land in ONE basic block and their chains interleave.
-template <bool FULL = false>
+// CONTACT = the ground pushes back (Aviary handles with contact_response): see rigid_step.
+template <bool FULL = false, bool CONTACT = false>
 PFB_HD void fixedwing_substep(const FixedwingParams& p, FixedwingRegs& s, const float* cmd, float xi) {
   Vec3 F = Vec3{0.f, 0.f, 0.f}, T = Vec3{0.f, 0.f, 0.f};
   const Vec3 w = Vec3{s.wx, s.wy, s.wz};
@@ -331,18 +456,18 @@ PFB_HD void fixedwing_substep(const FixedwingParams& p, FixedwingRegs& s, const 
   }
   const bool c = ground_contact(p.contact, (float)s.pz, (float)s.R.m20, (float)s.R.m21, (float)s.R.m22);
   s.flags = (s.flags & ~(uint32_t)FLAG_CONTACT_PREV) | (c ? (FLAG_CONTACT_PREV | FLAG_CONTACT_ARRAY) : 0u);
-  rigid_step(p.rb, p.gravity, p.dt, p.vmax, s, F, T);
+  rigid_step<CONTACT>(p.rb, p.gravity, p.dt, p.vmax, s, F, T, &p.contact, c);
   body_update_state(s);
 }
 
-template <int MODE, bool FULL = false, typename NoiseFn>
+template <int MODE, bool FULL = false, bool CONTACT = false, typename NoiseFn>
 PFB_HD void fixedwing_aviary_step(const FixedwingParams& p, FixedwingRegs& s, NoiseFn& noise) {
   s.flags &= ~(uint32_t)FLAG_CONTACT_ARRAY;
   noise.begin_step();
   float cmd[6];
   fixedwing_command<MODE>(s, cmd);
 #pragma unroll 1
-  for (int u = 0; u < p.ratio; ++u) fixedwing_substep<FULL>(p, s, cmd, noise.get(u));
+  for (int u = 0; u < p.ratio; ++u) fixedwing_substep<FULL, CONTACT>(p, s, cmd, noise.get(u));
 }
 // launch-uniform test for the FULL instantiation
 PFB_HD bool fixedwing_full_model(const FixedwingParams& p) { return p.n_surfaces == kMaxSurfaces && p.wind.kind == 0; }

@@ -71,6 +71,13 @@ int pfb_create(const PfbModel* model, const PfbEnvConfig* env, int64_t n_envs, i
   if (env && env->inline_reset != 0 && env->inline_reset != 1) return fail("inline_reset must be 0 or 1, got %d", env->inline_reset);
   if (model->kind != PFB_KIND_QUADX && model->kind != PFB_KIND_FIXEDWING && model->kind != PFB_KIND_ROCKET)
     return fail("unknown vehicle kind %d", model->kind);
+  // An Aviary handle (env kind NONE) takes ONE field from its config, contact_response; every other handle parameter is
+  // what env == NULL gives
+  int aviary_contact = 0;
+  if (env && env->env_kind == PFB_ENV_NONE) {
+    aviary_contact = env->contact_response ? 1 : 0;
+    env = nullptr;
+  }
   int count = 0;
   cudaError_t e = cudaGetDeviceCount(&count);
   if (e != cudaSuccess || count == 0)
@@ -82,6 +89,7 @@ int pfb_create(const PfbModel* model, const PfbEnvConfig* env, int64_t n_envs, i
   memset(c, 0, sizeof(*c));
   c->model = *model;
   if (env) c->env = *env;
+  else c->env.contact_response = aviary_contact;
   c->n = n_envs;
   c->device = device;
   if (model->kind == PFB_KIND_QUADX) {
@@ -95,6 +103,7 @@ int pfb_create(const PfbModel* model, const PfbEnvConfig* env, int64_t n_envs, i
     }
   } else {
     if (rk_build_params(*model, env, c->rk, c->land) != 0) { delete c; return -1; }
+    if (aviary_contact) c->rk.contact_response = 1;
   }
   c->hover.env_step_ratio = env ? env->env_step_ratio : 1;
   c->hover.max_steps = env ? env->max_steps : 0;

@@ -68,8 +68,8 @@ __global__ void __launch_bounds__(kBlock) k_quadx_set_mode(float* __restrict__ s
   reinterpret_cast<float4*>(setpoint)[i] = make_float4(s.sp[0], s.sp[1], s.sp[2], s.sp[3]);
 }
 
-// n_steps x Aviary.step() (aviary.py:480-531)
-template <int MODE, bool INJECT, bool TILED, class PS>
+// n_steps x Aviary.step() (aviary.py:480-531); CONTACT: the floor pushes back (Aviary handles with contact_response)
+template <int MODE, bool INJECT, bool TILED, class PS, bool CONTACT>
 __global__ void __launch_bounds__(kBlock, kMinBlocks)
     k_quadx_aviary_step(const __grid_constant__ PS ps, const __grid_constant__ RngParams rng,
                         float* __restrict__ st, int32_t* __restrict__ ist, int rows, const float* __restrict__ setpoint,
@@ -83,7 +83,7 @@ __global__ void __launch_bounds__(kBlock, kMinBlocks)
   float4 sp = __ldg(reinterpret_cast<const float4*>(setpoint) + i);
   s.sp[0] = sp.x; s.sp[1] = sp.y; s.sp[2] = sp.z; s.sp[3] = sp.w;
   auto nz = make_noise<INJECT>(noise, N, i, rng, seq, TAG_AVIARY, qx_model0(ps).noise_loc, qx_model0(ps).ratio);
-  for (int k = 0; k < n_steps; ++k) quadx_aviary_step<MODE>(p, s, nz);
+  for (int k = 0; k < n_steps; ++k) quadx_aviary_step<MODE, CONTACT>(p, s, nz);
   qx_store_any<MODE, TILED>(st, ist, rows, N, i, s, step_count);
 }
 
@@ -105,7 +105,7 @@ __global__ void __launch_bounds__(kBlock) k_quadx_set_modes(float* __restrict__ 
 
 // n_steps x Aviary.step() with drone i in flight mode modes[i].  Every PID row is moved (the mode-7 set); quadx_mask_pid
 // gives each drone the PID memory the uniform kernel of its mode would load, so both store the same words.
-template <bool INJECT, class PS>
+template <bool INJECT, class PS, bool CONTACT>
 __global__ void __launch_bounds__(kBlock, kMinBlocks)
     k_quadx_aviary_step_modes(const __grid_constant__ PS ps, const __grid_constant__ RngParams rng, float* __restrict__ st, int rows,
                               const float* __restrict__ setpoint, const int8_t* __restrict__ modes, const float* __restrict__ noise,
@@ -121,7 +121,7 @@ __global__ void __launch_bounds__(kBlock, kMinBlocks)
   float4 sp = __ldg(reinterpret_cast<const float4*>(setpoint) + i);
   s.sp[0] = sp.x; s.sp[1] = sp.y; s.sp[2] = sp.z; s.sp[3] = sp.w;
   auto nz = make_noise<INJECT>(noise, N, i, rng, seq, TAG_AVIARY, qx_model0(ps).noise_loc, qx_model0(ps).ratio);
-  for (int k = 0; k < n_steps; ++k) quadx_aviary_step_any(p, s, mode, nz);
+  for (int k = 0; k < n_steps; ++k) quadx_aviary_step_any<CONTACT>(p, s, mode, nz);
   quadx_store_tile<7, kTileGroupStride>(st + qx_tile_base(i, rows), s, step_count);
 }
 
@@ -865,21 +865,30 @@ int qx_aviary_step(PfbContext* h, int n_steps, const float* noise, cudaStream_t 
   const int mode = h->mode;
   const uint32_t seq = (uint32_t)h->aviary_seq++;
   const int g = grid_for(h->n);
+  const bool contact = aviary_contact_response(h);
   if (mode == kModePerDrone) {  // pfb_set_modes: Aviary handles only, so always warp-tiled
 #define AVM_ARGS ps, h->rng, h->buf.state, qx_rows(h), h->buf.setpoint, h->d_modes, noise, n_steps, seq, h->n
-    if (noise) { QX_PARAMS_SWITCH(h, (k_quadx_aviary_step_modes<true, PS><<<g, kBlock, 0, s>>>(AVM_ARGS))); }
-    else { QX_PARAMS_SWITCH(h, (k_quadx_aviary_step_modes<false, PS><<<g, kBlock, 0, s>>>(AVM_ARGS))); }
+    if (contact) {
+      if (noise) { QX_PARAMS_SWITCH(h, (k_quadx_aviary_step_modes<true, PS, true><<<g, kBlock, 0, s>>>(AVM_ARGS))); }
+      else { QX_PARAMS_SWITCH(h, (k_quadx_aviary_step_modes<false, PS, true><<<g, kBlock, 0, s>>>(AVM_ARGS))); }
+    } else {
+      if (noise) { QX_PARAMS_SWITCH(h, (k_quadx_aviary_step_modes<true, PS, false><<<g, kBlock, 0, s>>>(AVM_ARGS))); }
+      else { QX_PARAMS_SWITCH(h, (k_quadx_aviary_step_modes<false, PS, false><<<g, kBlock, 0, s>>>(AVM_ARGS))); }
+    }
 #undef AVM_ARGS
     LAUNCH_CHECK(h);
     return 0;
   }
 #define AV_ARGS ps, h->rng, h->buf.state, h->buf.istate, qx_rows(h), h->buf.setpoint, noise, n_steps, seq, h->n
-  if (qx_tiled(h)) {
-    if (noise) { QX_PARAMS_SWITCH(h, PFB_MODE_SWITCH(mode, (k_quadx_aviary_step<MODE, true, true, PS><<<g, kBlock, 0, s>>>(AV_ARGS)))); }
-    else { QX_PARAMS_SWITCH(h, PFB_MODE_SWITCH(mode, (k_quadx_aviary_step<MODE, false, true, PS><<<g, kBlock, 0, s>>>(AV_ARGS)))); }
+  if (contact) {  // Aviary handles only, so always warp-tiled
+    if (noise) { QX_PARAMS_SWITCH(h, PFB_MODE_SWITCH(mode, (k_quadx_aviary_step<MODE, true, true, PS, true><<<g, kBlock, 0, s>>>(AV_ARGS)))); }
+    else { QX_PARAMS_SWITCH(h, PFB_MODE_SWITCH(mode, (k_quadx_aviary_step<MODE, false, true, PS, true><<<g, kBlock, 0, s>>>(AV_ARGS)))); }
+  } else if (qx_tiled(h)) {
+    if (noise) { QX_PARAMS_SWITCH(h, PFB_MODE_SWITCH(mode, (k_quadx_aviary_step<MODE, true, true, PS, false><<<g, kBlock, 0, s>>>(AV_ARGS)))); }
+    else { QX_PARAMS_SWITCH(h, PFB_MODE_SWITCH(mode, (k_quadx_aviary_step<MODE, false, true, PS, false><<<g, kBlock, 0, s>>>(AV_ARGS)))); }
   } else {
-    if (noise) { QX_PARAMS_SWITCH(h, PFB_MODE_SWITCH(mode, (k_quadx_aviary_step<MODE, true, false, PS><<<g, kBlock, 0, s>>>(AV_ARGS)))); }
-    else { QX_PARAMS_SWITCH(h, PFB_MODE_SWITCH(mode, (k_quadx_aviary_step<MODE, false, false, PS><<<g, kBlock, 0, s>>>(AV_ARGS)))); }
+    if (noise) { QX_PARAMS_SWITCH(h, PFB_MODE_SWITCH(mode, (k_quadx_aviary_step<MODE, true, false, PS, false><<<g, kBlock, 0, s>>>(AV_ARGS)))); }
+    else { QX_PARAMS_SWITCH(h, PFB_MODE_SWITCH(mode, (k_quadx_aviary_step<MODE, false, false, PS, false><<<g, kBlock, 0, s>>>(AV_ARGS)))); }
   }
 #undef AV_ARGS
   LAUNCH_CHECK(h);

@@ -373,10 +373,18 @@ Vel3 quadx_clamp_world_velocity(vreal vmax, Vel3 v) {
   return v;
 }
 
+// contact RESPONSE over a list of collision primitives (pfb_fixedwing.cuh)
+template <class Shapes, class Regs>
+PFB_HD void apply_contact_impulses(const Shapes* cp, Regs& s, float pz0, float top, float M, Vec3 c, float Ixx, float Ixy, float Ixz,
+                                   float Iyy, float Iyz, float Izz, float dt);
+
 // One physics substep: update_physics (quadx.py:495-510) + stepSimulation + update_state.
 // xi = raw draw of np_random.normal(*throttle.shape)  (one scalar ~ N(4, 1) shared by the motors).
 // Written as straight-line code (selects instead of branches): the kernel is instruction-issue bound
 // and the I-cache-resident hot loop is what the whole env step runs in.
+// CONTACT = the floor pushes back (Aviary handles with contact_response): on a substep whose contact flag is up, contact
+// impulses act on the predicted velocities before the pose is integrated (cold path; COM at the base origin, diagonal inertia).
+template <bool CONTACT = false>
 PFB_HD void quadx_substep(const QuadXParams& p, QuadXRegs& s, float xi) {
   // ---- motors (motors.py:130-155): lag, multiplicative noise, rpm^2 thrust + reaction torque
   float Fz = 0.0f, tx = 0.0f, ty = 0.0f, tz = 0.0f;
@@ -434,9 +442,11 @@ PFB_HD void quadx_substep(const QuadXParams& p, QuadXRegs& s, float xi) {
     Vel3 c = quadx_clamp_world_velocity((vreal)p.vmax, Vel3{s.vx, s.vy, s.vz});
     s.vx = c.x; s.vy = c.y; s.vz = c.z;
   }
-  s.px += (xreal)(s.vx * dt);
-  s.py += (xreal)(s.vy * dt);
-  s.pz += (xreal)(s.vz * dt);
+  if (!CONTACT) {  // the contact impulses below change the velocities the positions move with
+    s.px += (xreal)(s.vx * dt);
+    s.py += (xreal)(s.vy * dt);
+    s.pz += (xreal)(s.vz * dt);
+  }
   s.wx = fmaf(wdx, p.dt, s.wx);
   s.wy = fmaf(wdy, p.dt, s.wy);
   s.wz = fmaf(wdz, p.dt, s.wz);
@@ -444,6 +454,12 @@ PFB_HD void quadx_substep(const QuadXParams& p, QuadXRegs& s, float xi) {
     Mat3 Rf{(float)R.m00, (float)R.m01, (float)R.m02, (float)R.m10, (float)R.m11, (float)R.m12, (float)R.m20, (float)R.m21, (float)R.m22};
     Vec3 w = quadx_clamp_world_rates(p.vmax, Rf, Vec3{s.wx, s.wy, s.wz});
     s.wx = w.x; s.wy = w.y; s.wz = w.z;
+  }
+  if (CONTACT) {
+    if (c) apply_contact_impulses(&p, s, (float)s.pz, 0.0f, 1.0f / p.inv_mass, Vec3{0.f, 0.f, 0.f}, p.Ixx, 0.0f, 0.0f, p.Iyy, 0.0f, p.Izz, p.dt);
+    s.px += (xreal)(s.vx * dt);
+    s.py += (xreal)(s.vy * dt);
+    s.pz += (xreal)(s.vz * dt);
   }
   // ---- attitude: q <- q * dq(w_b dt).  dq = (w sin(h)/|w|, cos h), h = |w| dt / 2.  With
   // h^2 = |w|^2 dt^2 / 4 <= 0.13 (|w| <= sqrt(3) vmax; checked at create) both factors are short even
@@ -474,13 +490,13 @@ PFB_HD void quadx_substep(const QuadXParams& p, QuadXRegs& s, float xi) {
 // Aviary.step(): one control tick + `ratio` physics substeps (aviary.py:506-531 with one drone).
 // Noise protocol: begin_step() prepares the draws of this Aviary step (outside the substep loop),
 // get(u) hands out the draw of substep u.
-template <int MODE, typename NoiseFn>
+template <int MODE, bool CONTACT = false, typename NoiseFn>
 PFB_HD void quadx_aviary_step(const QuadXParams& p, QuadXRegs& s, NoiseFn& noise) {
   s.flags &= ~(uint32_t)FLAG_CONTACT_ARRAY;  // contact_array &= False
   noise.begin_step();
   quadx_update_control<MODE>(p, s);
 #pragma unroll 1
-  for (int u = 0; u < p.ratio; ++u) quadx_substep(p, s, noise.get(u));
+  for (int u = 0; u < p.ratio; ++u) quadx_substep<CONTACT>(p, s, noise.get(u));
 }
 
 // quadx.py:233-373: setpoint preset + PID reset on a mode change
@@ -523,13 +539,13 @@ PFB_HD void quadx_update_control_any(const QuadXParams& p, QuadXRegs& s, int mod
   PFB_QX_MODE_CASES(mode, quadx_update_control<M>(p, s));
 }
 
-template <typename NoiseFn>
+template <bool CONTACT = false, typename NoiseFn>
 PFB_HD void quadx_aviary_step_any(const QuadXParams& p, QuadXRegs& s, int mode, NoiseFn& noise) {
   s.flags &= ~(uint32_t)FLAG_CONTACT_ARRAY;
   noise.begin_step();
   quadx_update_control_any(p, s, mode);
 #pragma unroll 1
-  for (int u = 0; u < p.ratio; ++u) quadx_substep(p, s, noise.get(u));
+  for (int u = 0; u < p.ratio; ++u) quadx_substep<CONTACT>(p, s, noise.get(u));
 }
 
 PFB_HD void quadx_set_mode_any(QuadXRegs& s, int mode) { PFB_QX_MODE_CASES(mode, quadx_set_mode<M>(s)); }

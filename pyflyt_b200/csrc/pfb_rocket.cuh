@@ -89,75 +89,6 @@ PFB_HD void rocket_command(const RocketRegs& s, float* cmd) {
   cmd[4] = s.sp[3]; cmd[5] = s.sp[4]; cmd[6] = s.sp[5]; cmd[7] = s.sp[6];
 }
 
-// ---- contact RESPONSE (PfbEnvConfig.contact_response): the arithmetic of oracle/fakebullet/pybullet.py::_solve_contacts and
-// oracle/pfb_oracle.c::solve_contacts, in the BODY frame (the inverse central inertia is constant there): candidate points =
-// 8 per collision primitive (box corners; 4 + 4 cylinder rim points), kContactIterations sweeps, per penetrating point a
-// non-accumulated normal impulse (restitution 0, Baumgarte bias erp * (depth - slop) / dt) then Coulomb friction.  A
-// restatement of a Bullet-like sequential impulse, unpinned (DESIGN.md).  COLD: only called on substeps whose contact flag
-// is up; everything by value so that the caller's registers never have their address taken.
-constexpr int kContactIterations = 8;
-constexpr float kContactErp = 0.2f, kContactSlop = 0.001f, kContactFriction = 0.5f;
-struct ContactVel { float vx, vy, vz, wx, wy, wz; int touched; };
-#if defined(__CUDACC__)
-static __host__ __device__ __noinline__
-#else
-inline
-#endif
-ContactVel rocket_solve_contacts(const ContactParams* cp, float pz, float top, Vec3 n /* world z in the body frame = third row of R */, Vec3 vb,
-                                 Vec3 w, float M, Vec3 c, float Ixx, float Ixy, float Ixz, float Iyy, float Iyz, float Izz, float dt) {
-  // inverse of the symmetric central inertia (cofactors)
-  const float c00 = Iyy * Izz - Iyz * Iyz, c01 = Ixz * Iyz - Ixy * Izz, c02 = Ixy * Iyz - Ixz * Iyy;
-  const float c11 = Ixx * Izz - Ixz * Ixz, c12 = Ixy * Ixz - Ixx * Iyz, c22 = Ixx * Iyy - Ixy * Ixy;
-  const float id = 1.0f / (Ixx * c00 + Ixy * c01 + Ixz * c02), iM = 1.0f / M;
-  auto Iinv = [&](Vec3 r) { return Vec3{(c00 * r.x + c01 * r.y + c02 * r.z) * id, (c01 * r.x + c11 * r.y + c12 * r.z) * id, (c02 * r.x + c12 * r.y + c22 * r.z) * id}; };
-  Vec3 vc = vb + cross(w, c);  // COM velocity, body frame
-  int touched = 0;
-  for (int it = 0; it < kContactIterations; ++it) {
-    for (int sh = 0; sh < cp->n_shapes; ++sh) {
-      if (cp->kind[sh] > 1) continue;  // boxes and cylinders
-      const float* q = cp->rot[sh];
-      for (int j = 0; j < 8; ++j) {
-        const float sz = (j & 4) ? 1.0f : -1.0f;
-        float lx, ly, lz;
-        if (cp->kind[sh] == 0) {
-          lx = ((j & 1) ? 1.0f : -1.0f) * cp->dims[sh][0]; ly = ((j & 2) ? 1.0f : -1.0f) * cp->dims[sh][1]; lz = sz * cp->dims[sh][2];
-        } else {
-          const int a = j & 3;
-          lx = cp->dims[sh][0] * (a == 0 ? 1.0f : (a == 2 ? -1.0f : 0.0f)); ly = cp->dims[sh][0] * (a == 1 ? 1.0f : (a == 3 ? -1.0f : 0.0f));
-          lz = sz * cp->dims[sh][1];
-        }
-        const Vec3 pb = Vec3{cp->at[sh][0] + q[0] * lx + q[1] * ly + q[2] * lz, cp->at[sh][1] + q[3] * lx + q[4] * ly + q[5] * lz,
-                             cp->at[sh][2] + q[6] * lx + q[7] * ly + q[8] * lz};
-        const float depth = top - (pz + dot(n, pb));
-        if (depth <= 0.0f) continue;
-        touched = 1;
-        const Vec3 r = pb - c;
-        Vec3 u = vc + cross(w, r);
-        const Vec3 rn = cross(r, n), Irn = Iinv(rn);
-        const float kn = iM + dot(rn, Irn);
-        const float bias = kContactErp * fmaxf(depth - kContactSlop, 0.0f) / dt;
-        const float jn = fmaxf(0.0f, (bias - dot(u, n)) / kn);
-        if (jn > 0.0f) {
-          vc = vc + (jn * iM) * n;
-          w = w + jn * Irn;
-          u = vc + cross(w, r);
-          const Vec3 ut = u - dot(u, n) * n;
-          const float sp = sqrtf(dot(ut, ut));
-          if (sp > 1e-9f) {
-            const Vec3 t = (1.0f / sp) * ut, rt = cross(r, t), Irt = Iinv(rt);
-            const float kt = iM + dot(rt, Irt);
-            const float jt = fminf(sp / kt, kContactFriction * jn);
-            vc = vc - (jt * iM) * t;
-            w = w - jt * Irt;
-          }
-        }
-      }
-    }
-  }
-  const Vec3 vo = vc - cross(w, c);
-  return ContactVel{vo.x, vo.y, vo.z, w.x, w.y, w.z, touched};
-}
-
 // one physics substep: update_physics (rocket.py:280-298) + stepSimulation + update_state
 PFB_HD void rocket_substep(const RocketParams& p, RocketRegs& s, const float* cmd, float xi, bool with_pad) {
   Vec3 F = Vec3{0.f, 0.f, 0.f}, T = Vec3{0.f, 0.f, 0.f};
@@ -262,21 +193,9 @@ PFB_HD void rocket_substep(const RocketParams& p, RocketRegs& s, const float* cm
     Vec3 wc = quadx_clamp_world_rates(p.vmax, Rf, Vec3{s.wx, s.wy, s.wz});
     s.wx = wc.x; s.wy = wc.y; s.wz = wc.z;
   }
-  if (p.contact_response && touching) {  // contact impulses on the predicted velocities, before the pose is integrated (cold path)
-    const float m00 = (float)R.m00, m01 = (float)R.m01, m02 = (float)R.m02, m10 = (float)R.m10, m11 = (float)R.m11, m12 = (float)R.m12,
-                m20 = (float)R.m20, m21 = (float)R.m21, m22 = (float)R.m22;
-    const float vwx = (float)s.vx, vwy = (float)s.vy, vwz = (float)s.vz;
-    const Vec3 vbn = Vec3{m00 * vwx + m10 * vwy + m20 * vwz, m01 * vwx + m11 * vwy + m21 * vwz, m02 * vwx + m12 * vwy + m22 * vwz};
-    const ContactVel cv = rocket_solve_contacts(&p.contact, pz0, over_pad ? kPadTop : 0.0f, Vec3{m20, m21, m22}, vbn, Vec3{s.wx, s.wy, s.wz}, M, c,
-                                                Ixx - M * (c2 - c.x * c.x), Ixy + M * c.x * c.y, Ixz + M * c.x * c.z, Iyy - M * (c2 - c.y * c.y),
-                                                Iyz + M * c.y * c.z, Izz - M * (c2 - c.z * c.z), p.dt);
-    if (cv.touched) {
-      s.vx = (vreal)(m00 * cv.vx + m01 * cv.vy + m02 * cv.vz);
-      s.vy = (vreal)(m10 * cv.vx + m11 * cv.vy + m12 * cv.vz);
-      s.vz = (vreal)(m20 * cv.vx + m21 * cv.vy + m22 * cv.vz);
-      s.wx = cv.wx; s.wy = cv.wy; s.wz = cv.wz;
-    }
-  }
+  if (p.contact_response && touching)  // contact impulses on the predicted velocities, before the pose is integrated (cold path)
+    apply_contact_impulses(&p.contact, s, pz0, over_pad ? kPadTop : 0.0f, M, c, Ixx - M * (c2 - c.x * c.x), Ixy + M * c.x * c.y, Ixz + M * c.x * c.z,
+                           Iyy - M * (c2 - c.y * c.y), Iyz + M * c.y * c.z, Izz - M * (c2 - c.z * c.z), p.dt);
   s.px += (xreal)(s.vx * dt); s.py += (xreal)(s.vy * dt); s.pz += (xreal)(s.vz * dt);
   float h2 = (s.wx * s.wx + s.wy * s.wy + s.wz * s.wz) * (0.25f * p.dt * p.dt);
   float sinc = fmaf(h2, fmaf(h2, fmaf(h2, fmaf(h2, 2.7557319e-6f, -1.9841270e-4f), 8.3333333e-3f), -1.6666667e-1f), 1.0f);

@@ -520,6 +520,33 @@ def touchdown_fixtures():
     fly_touchdown("landing_touchdown_hard", seed=83, n_steps=300, descent_rate=2.5)
 
 
+def ground_fixtures():
+    """Aviary-level flights that land on, rest on, slide along and take off from the floor, with the engine's contact RESPONSE
+    switched on (oracle/fakebullet World.contact_response), replayed by BatchedAviary(contact_response=True).  One drone per
+    reference Aviary: the reference drops the rotational drag of every drone of a world once any of them touches
+    (quadx.py:508-510), and each batched drone has a world of its own.  The files are named ground_* so that the replays of
+    the flag-only fixtures (quadx_*, fixedwing_*, rocket_*) do not pick them up."""
+    import pybullet as fb  # oracle/fakebullet
+
+    fb.World.contact_response = True
+    try:
+        # cf2x take-off from the floor (velocity mode 6): climb to ~1 m, hold, descend, settle on the floor for > 2 s
+        fly_quadx("ground_cf2x_takeoff_landing", 6, "cf2x", [0.0, 0.0, 0.01], [0.0, 0.0, 0.0],
+                  {0: [0.0, 0.0, 0.0, 0.5], 240: [0.0, 0.0, 0.0, 0.0], 360: [0.0, 0.0, 0.0, -0.4], 660: [0.0, 0.0, 0.0, -0.2]}, 1000, seed=301)
+        # primitive_drone dropped tilted with the motors idle: a propeller cylinder's rim strikes first, the airframe tips flat
+        fly_quadx("ground_primitive_tilted_drop", -1, "primitive_drone", [0.0, 0.0, 1.5], [0.4, 0.0, 0.0], {0: [0.0, 0.0, 0.0, 0.0]}, 480, seed=302)
+        # cf2x pushed sideways by a tilted thrust burst, then motors idle: it touches down sliding and friction stops it
+        fly_quadx("ground_cf2x_sliding_touchdown", -1, "cf2x", [0.0, 0.0, 0.1], [0.0, 0.35, 0.0],
+                  {0: [0.6, 0.6, 0.6, 0.6], 24: [0.0, 0.0, 0.0, 0.0]}, 600, seed=303)
+        # fixed-wing glide at zero throttle from a few metres: belly landing, slides to rest on its box primitives
+        fly_vehicle("ground_fixedwing_belly_landing", "fixedwing", "fixedwing", 0, [0.0, 0.0, 3.0], [0.0, 0.05, 0.0], {0: [0.0, 0.1, 0.0, 0.0]},
+                    840, seed=304)
+        # rocket dropped a short way onto the bare ground, booster off: it rests on its legs
+        fly_vehicle("ground_rocket_rest", "rocket", "rocket", 0, [0.0, 0.0, 3.0], [0.0, 0.0, 0.0], {0: [0, 0, 0, 0, 0, 0, 0]}, 360, seed=305)
+    finally:
+        fb.World.contact_response = False
+
+
 def fly_dogfight(name, seed, n_steps, action_seed, team_size=1, sparse=False, action_scale=0.6, lethal_distance=20.0, lethal_angle=0.07,
                  spawn_min_radius=10.0, spawn_max_radius=50.0, damage_per_hit=0.003, pitch_bias=0.0):
     """MAFixedwingDogfightEnv (pz_envs/fixedwing_envs/ma_fixedwing_dogfight_env.py) with scripted actions; a new
@@ -889,3 +916,5 @@ if __name__ == "__main__":
         mixed_model_fixtures()
     if which in ("all", "mixedmodes"):
         mixed_mode_fixtures()
+    if which in ("all", "ground"):
+        ground_fixtures()
