@@ -255,7 +255,8 @@ int pfb_destroy(PfbHandle h);
  * with a full pfb_env_reset (mask = NULL), which rebuilds them; an Aviary handle with pfb_reset.                         */
 int pfb_reseed(PfbHandle h, uint64_t seed, void* stream);
 /* Global index of this handle's env 0 (rank * n_envs when the batch is sharded over GPUs): keeps
- * the Philox streams, and therefore every trajectory, independent of the number of ranks.          */
+ * the Philox streams, and therefore every trajectory, independent of the number of ranks.  Call it before the first
+ * pfb_env_reset: the spare post-reset states are keyed to the env ids they were built for.          */
 int pfb_set_env_offset(PfbHandle h, uint64_t first_global_env);
 
 /* Several vehicle models in one QuadX handle (Aviary(drone_options=[...]) with one dict per drone, aviary.py:75,196-199):
@@ -267,7 +268,10 @@ int pfb_set_env_offset(PfbHandle h, uint64_t first_global_env);
 int pfb_set_models(PfbHandle h, const PfbModel* models, int k, const uint8_t* index_host);
 
 /* Aviary.register_wind_field_function for an analytic field (NULL or kind PFB_WIND_NONE: still air).  Takes effect from the
- * next call on; every vehicle kind.                                                                                  */
+ * next call on; every vehicle kind.  PFB_WIND_POWER needs alpha >= 0; alpha = 0 is stored as PFB_WIND_CONSTANT (0^0 = 1).
+ * On an env handle that keeps spare post-reset states (autoreset), a field that differs from the current one costs a device
+ * synchronisation: every spare is marked invalid, so that each env's next reset integrates its warm-up in the new air,
+ * under the same episode number, and the spares are rebuilt from there on (the spare and inline_reset paths stay equal).  */
 int pfb_set_wind(PfbHandle h, const PfbWind* wind);
 int pfb_sizeof_wind(void);
 

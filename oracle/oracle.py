@@ -43,6 +43,7 @@ def lib() -> C.CDLL:
         L.orc_df_get_actions.argtypes = [vp, dp]
         L.orc_df_set_actions.argtypes = [vp, C.POINTER(C.c_uint8), dp]
         L.orc_set_wind.argtypes = [vp, vp]
+        L.orc_wind_field.argtypes = [vp, i64, dp, dp]
         L.orc_reset.argtypes = [vp, u8p]
         L.orc_set_mode.argtypes = [vp, C.c_int]
         L.orc_set_setpoints.argtypes = [vp, dp, C.c_int]
@@ -112,6 +113,13 @@ class Oracle:
         else:
             w = wind.as_struct()
             lib().orc_set_wind(self._h, C.byref(w))
+
+    def wind_field(self, pos):
+        """the field set with set_wind at world points pos[m][3] -> [m][3]"""
+        p = np.ascontiguousarray(pos, dtype=np.float64).reshape(-1, 3)
+        out = np.zeros_like(p)
+        lib().orc_wind_field(self._h, len(p), _dp(p), _dp(out))
+        return out
 
     def set_setpoints(self, sp):
         sp = np.ascontiguousarray(sp, dtype=np.float64)

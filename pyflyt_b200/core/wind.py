@@ -6,7 +6,7 @@ parameter block the CUDA kernels evaluate in place of that callback (``PfbWind``
 
     wind(x, y, z) = base * f(z)
       constant   f = 1
-      power      f = (max(z, 0) / z_ref) ** alpha
+      power      f = (max(z, 0) / z_ref) ** alpha      # alpha >= 0; alpha = 0 is the constant profile (0 ** 0 = 1)
       log        f = ln(max(z, z0) / z0) / ln(z_ref / z0)
       exp        f = exp(z / z_ref)          # tests/test_core.py:275-278 of the reference: base = (0, 0, 1), z_ref = 1
 """
@@ -30,6 +30,8 @@ class AnalyticWind:
             raise ValueError(f"wind kind must be one of {sorted(KINDS)}, got {kind!r}")
         if z_ref <= 0.0 or (kind == "log" and not (0.0 < z0 < z_ref)):
             raise ValueError("z_ref must be positive and, for the log profile, 0 < z0 < z_ref")
+        if kind == "power" and not alpha >= 0.0:  # a negative exponent makes the wind infinite at the floor
+            raise ValueError(f"the power-law profile needs alpha >= 0, got {alpha}")
         self.kind, self.base = kind, np.asarray(base, dtype=np.float64).reshape(3)
         self.z_ref, self.alpha, self.z0 = float(z_ref), float(alpha), float(z0)
 

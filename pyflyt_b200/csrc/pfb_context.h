@@ -274,6 +274,8 @@ int hover_env_reset(PfbContext* h, const uint8_t* mask, const float* noise, cuda
 // `dyn_smem`: dynamic shared memory the step launch requests and never touches (pfb_env_step_mapped; 0 = every CTA resident in one wave)
 int hover_env_step(PfbContext* h, float* actions, const float* noise, bool randact, size_t dyn_smem, cudaStream_t s);
 int hover_env_rollout(PfbContext* h, int n_steps, cudaStream_t s);  // n_steps env steps with on-device actions, fused where it can
+// with the device idle: finish the half-built spares, empty their queue and mark every spare record invalid (pfb_set_wind)
+int hover_invalidate_spares(PfbContext* h, cudaStream_t s);
 
 // fixedwing translation unit (pfb_fixedwing.cu)
 int fw_build_params(const PfbModel& m, const PfbEnvConfig* env, pfb::FixedwingParams& p, pfb::WaypointParams& w);
@@ -288,6 +290,7 @@ int fw_observe(PfbContext* h, cudaStream_t s);
 int fw_env_reset(PfbContext* h, const uint8_t* mask, const float* noise, cudaStream_t s);
 int fw_env_step(PfbContext* h, float* actions, const float* noise, bool randact, cudaStream_t s);
 int fw_spare_rows();
+int fw_spare_valid_row();  // float offset of the valid word in a spare record
 
 // rocket translation unit (pfb_rocket.cu)
 int rk_build_params(const PfbModel& m, const PfbEnvConfig* env, pfb::RocketParams& p, pfb::LandingParams& l);
@@ -302,6 +305,7 @@ int rk_observe(PfbContext* h, cudaStream_t s);
 int rk_env_reset(PfbContext* h, const uint8_t* mask, const float* noise, cudaStream_t s);
 int rk_env_step(PfbContext* h, float* actions, const float* noise, bool randact, cudaStream_t s);
 int rk_spare_rows();
+int rk_spare_valid_row();  // float offset of the valid word in a spare record
 
 // dogfight translation unit (pfb_dogfight.cu): fixedwing vehicles, arenas of 2*team_size adjacent envs
 int df_build_params(const PfbEnvConfig* env, pfb::DogfightParams& d);
@@ -309,6 +313,7 @@ int df_obs_dim(const PfbContext* h);
 int df_env_reset(PfbContext* h, const uint8_t* mask, const float* noise, cudaStream_t s);
 int df_env_step(PfbContext* h, float* actions, const float* noise, bool randact, cudaStream_t s);
 int df_spare_rows();
+int df_spare_valid_row();  // float offset of the valid word in a spare record
 int df_split_physics(PfbContext* h, const float* actions, const float* noise, float* payload, const uint64_t* peers, int world, int64_t slot0,
                      const uint64_t* peer_flags, int rank, int epoch, int first, int do_reset, int sub, cudaStream_t s);
 int df_split_combat(PfbContext* h, const float* table, int64_t first_gid, int64_t num_arenas, int last, const int* wait_flags, int world, int epoch,
@@ -319,5 +324,6 @@ int qwp_state_rows();
 int qwp_istate_rows();
 int qwp_obs_dim(const PfbContext* h);
 int qwp_spare_rows();
+int qwp_spare_valid_row();  // float offset of the valid word in a spare record
 int qwp_env_reset(PfbContext* h, const uint8_t* mask, const float* noise, cudaStream_t s);
 int qwp_env_step(PfbContext* h, float* actions, const float* noise, bool randact, cudaStream_t s);

@@ -56,6 +56,7 @@ enum { DSP_HITS = FW_ROWS, DSP_VALID = FW_ROWS + 1, DSP_FLAGS = FW_ROWS + 2, DSP
 static_assert(FW_ROWS + 4 <= DSP_OBS && DSP_OBS + 23 + 14 * 3 <= DSP_ROWS, "spare record too small");
 constexpr int kDfObsPast = 19;  // index of past_actions inside the observation (3 + 3 + 3 + 3 + 5 + 1 + 1)
 int df_spare_rows() { return DSP_ROWS; }
+int df_spare_valid_row() { return DSP_VALID; }
 
 struct DfAgent {
   float health, acc_reward;

@@ -242,6 +242,7 @@ __device__ __forceinline__ void wp_reset_env(const FixedwingParams& p, const Way
 // new_distance
 enum { WSP_ROWS = 64 };
 int fw_spare_rows() { return WSP_ROWS; }
+int fw_spare_valid_row() { return FW_ROWS + SPARE_VALID; }
 
 // the Fixedwing-Waypoints env for tail_step (pfb_tail_step.cuh)
 template <bool INJECT, bool RANDACT>

@@ -360,7 +360,9 @@ int pfb_set_wind(PfbHandle h, const PfbWind* wind) {
     if (wind->kind < PFB_WIND_CONSTANT || wind->kind > PFB_WIND_EXP) return fail("unknown wind kind %d", wind->kind);
     if (!(wind->z_ref > 0.0)) return fail("wind z_ref must be positive");
     if (wind->kind == PFB_WIND_LOG && !(wind->z0 > 0.0 && wind->z0 < wind->z_ref)) return fail("log wind profile needs 0 < z0 < z_ref");
-    w.kind = wind->kind;
+    if (wind->kind == PFB_WIND_POWER && !(wind->alpha >= 0.0)) return fail("power-law wind profile needs alpha >= 0, got %g", wind->alpha);
+    // alpha = 0 is the constant profile for every z (0^0 = 1); the kernels' exp2(alpha * log2(z)) would give 0 * -inf = NaN at z <= 0
+    w.kind = (wind->kind == PFB_WIND_POWER && wind->alpha == 0.0) ? PFB_WIND_CONSTANT : wind->kind;
     w.bx = (float)wind->base[0]; w.by = (float)wind->base[1]; w.bz = (float)wind->base[2];
     w.inv_zref = (float)(1.0 / wind->z_ref);
     w.alpha = (float)wind->alpha;
@@ -369,6 +371,22 @@ int pfb_set_wind(PfbHandle h, const PfbWind* wind) {
       w.inv_z0 = (float)(1.0 / wind->z0);
       w.inv_log = (float)(1.0 / log(wind->z_ref / wind->z0));
     }
+  }
+  if (h->d_spare && memcmp(&w, &h->qx.wind, sizeof(w)) != 0) {
+    // The spare post-reset states were integrated in the old air.  Nothing may still be building them; then every record is
+    // marked invalid but keeps its episode number, so each env's next reset integrates its warm-up inline, under the episode
+    // number the spare would have had, in the new air, and the rebuilds that follow it use the new air too.
+    CUDA_OK(cudaSetDevice(h->device));
+    if (h->side) CUDA_OK(cudaStreamSynchronize(h->side));
+    CUDA_OK(cudaDeviceSynchronize());
+    if (h->env.env_kind == PFB_ENV_QUADX_HOVER) {
+      if (hover_invalidate_spares(h, 0)) return -1;
+    } else {
+      const int valid = is_df(h) ? df_spare_valid_row() : is_rk(h) ? rk_spare_valid_row() : is_qwp(h) ? qwp_spare_valid_row() : fw_spare_valid_row();
+      const size_t rows = (size_t)(is_df(h) ? df_spare_rows() : is_rk(h) ? rk_spare_rows() : is_qwp(h) ? qwp_spare_rows() : fw_spare_rows());
+      CUDA_OK(cudaMemset2DAsync(h->d_spare + valid, rows * sizeof(float), 0, sizeof(float), (size_t)h->n, 0));
+    }
+    CUDA_OK(cudaDeviceSynchronize());
   }
   h->qx.wind = w;
   if (h->qxset)

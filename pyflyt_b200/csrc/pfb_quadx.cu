@@ -1020,6 +1020,27 @@ static int hover_rollout_fused(PfbContext* h, int n_steps, cudaStream_t s) {
   return 0;
 }
 
+// The spares whose first half the last step launch integrated are finished (so that episode[] names each env's next spare) and
+// taken off the queue the next launch would finish them from; the envs finished on the last launch stay queued, so that launch
+// builds their next spares.  Then every record fails its validity check: each env's next reset runs the cold path under
+// episode[i], the number the spare path would have used, and the builders / k_hover_spare_ahead replace the records.
+int hover_invalidate_spares(PfbContext* h, cudaStream_t s) {
+  const uint64_t k = h->step_seq;
+  if (k >= 2) {
+    const int tiles = grid_for(h->n);
+    const int builders = h->sm_count < tiles ? h->sm_count : tiles;
+    QX_PARAMS_SWITCH(h, PFB_MODE_SWITCH(h->hover.flight_mode, (k_hover_drain<MODE, PS><<<builders, kBlock, 0, s>>>(
+                                                                   ps, h->hover, h->rng, h->d_counters + ((k + 2) % 4), h->d_done_list + ((k + 2) % 4) * h->n,
+                                                                   h->d_elist + ((k + 2) % 4) * h->n, h->buf.start_pos, h->buf.start_orn, h->d_spare,
+                                                                   h->d_episode, builders, h->n))));
+    LAUNCH_CHECK(h);
+    CUDA_OK(cudaMemsetAsync(h->d_counters + ((k + 2) % 4), 0, sizeof(int32_t), s));
+  }
+  CUDA_OK(cudaMemset2DAsync(h->d_spare + SP_VALID, SP_ROWS * sizeof(float), 0, sizeof(float), (size_t)kSpareBufs * h->n, s));
+  h->fused_ready = 0;
+  return 0;
+}
+
 int hover_env_rollout(PfbContext* h, int n_steps, cudaStream_t s) {
   if (n_steps >= kFusedMinSteps && hover_fused_ok(h)) return hover_rollout_fused(h, n_steps, s);
   for (int k = 0; k < n_steps; ++k)

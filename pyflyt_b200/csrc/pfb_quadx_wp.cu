@@ -162,6 +162,7 @@ __device__ __forceinline__ void qw_reset_env(const QuadXParams& p, const QxWaypo
 // new_distance and yaw error
 enum { QSP_ROWS = 128 };
 int qwp_spare_rows() { return QSP_ROWS; }
+int qwp_spare_valid_row() { return QW_ROWS + SPARE_VALID; }
 
 // the QuadX-Waypoints env for tail_step (pfb_tail_step.cuh)
 template <int MODE, bool INJECT, bool RANDACT, class PS>

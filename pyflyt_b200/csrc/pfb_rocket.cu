@@ -200,6 +200,7 @@ constexpr int kLandBlocks = 8;
 // ---- spare post-reset states (pfb_tail_step.cuh): a record holds the RK_* state words
 enum { LSP_ROWS = 64 };
 int rk_spare_rows() { return LSP_ROWS; }
+int rk_spare_valid_row() { return RK_ROWS + SPARE_VALID; }
 
 // the Rocket-Landing env for tail_step (pfb_tail_step.cuh)
 template <bool INJECT, bool RANDACT>

@@ -26,10 +26,13 @@ def scenario(num_arenas, steps, seed=5):
     return pos, orn, nz0, acts, nz
 
 
-def run(num_arenas, steps, device, single_rank=False, exchange="nccl"):
+def run(num_arenas, steps, device, single_rank=False, exchange="nccl", wind=None):
+    """``wind``: an AnalyticWind registered on the rank's Aviary before the reset, or None"""
     pos, orn, nz0, acts, nz = scenario(num_arenas, steps)
     env = MAFixedwingDogfightSplitEnv(num_arenas, seed=3, device=device, lethal_distance=150.0, lethal_angle_radians=1.0, damage_per_hit=0.05,
                                       single_rank=single_rank, exchange=exchange)
+    if wind is not None:
+        env.aviary.register_wind_field(wind)
     lo, hi = env.first_gid, env.first_gid + env.n_local
     dev = env.device
     out = [env.reset(pos, orn, noise=torch.as_tensor(nz0[:, lo:hi].copy(), device=dev)).clone()]

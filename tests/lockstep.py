@@ -12,6 +12,10 @@ An env whose termination decision sits within fp32 rounding of its threshold tak
 the two follow different episodes, so it is dropped from the comparison and counted as a flip.  ``Run.check()`` holds the
 flips, the "loose" envs and the worst differences to the per-kind bars of test_timed_path_parity.py; a flip budget never goes
 below 2, so small batches are not held to a zero-flip bar.
+
+Every driver takes an optional wind schedule ``{env step: AnalyticWind | None}``: each entry is registered on the handle's
+Aviary and set on the oracle before that env step (the step's index in the driver's loop; entry 0 before ``env.reset()``),
+so a wind can be present from the start, or registered, changed and cleared between autoresets.
 """
 from __future__ import annotations
 
@@ -95,6 +99,14 @@ def oracle_config(env):
     return c
 
 
+def _apply_wind(wind, k, env, orc):
+    """the schedule's entry for env step k, if any, on the handle and on the oracle (whose set_wind refreshes the link air
+    velocities, as the kernels derive them from the state in every substep)"""
+    if wind and k in wind:
+        env.aviary.register_wind_field(wind[k])
+        orc.set_wind(wind[k])
+
+
 def _autoreset_noise(streams, episode, idx, n):
     rz = np.zeros((20, n))
     rz[:, idx] = streams.autoreset_noise(episode[idx], envs=idx)
@@ -106,7 +118,7 @@ def hover_oracle(env, n):
     return OracleEngine(build_model("quadx", "cf2x"), oracle_config(env), n, np.tile([[0.0, 0.0, 1.0]], (n, 1)), np.zeros((n, 3)))
 
 
-def hover_step(env, seed: int, steps: int, *, env_offset: int = 0, reset_seq: int = 0, episode0: int = 1, obs_bar: float = 1e-4) -> Run:
+def hover_step(env, seed: int, steps: int, *, env_offset: int = 0, reset_seq: int = 0, episode0: int = 1, obs_bar: float = 1e-4, wind: dict | None = None) -> Run:
     """Single-step launches (``rollout(1)``: on-device RANDACT actions, compared bit for bit with the replay), the kernel's noise
     dumped and compared with the replay, the oracle reset on the kernel's schedule."""
     import torch
@@ -117,12 +129,15 @@ def hover_step(env, seed: int, steps: int, *, env_offset: int = 0, reset_seq: in
     av.set_noise_dump(dump)
     streams = Streams(seed, n, env_offset=env_offset, noise_loc=4.0)
     orc = hover_oracle(env, n)
+    _apply_wind(wind, 0, env, orc)
     obs_g, _ = env.reset()
     obs_o = orc.o.env_reset(noise=streams.user_reset_noise(reset_seq).astype(np.float64))
     run.reset_obs = float(np.abs(obs_g.double().cpu().numpy() - obs_o).max())
     episode = np.full(n, episode0, dtype=np.int64)
     done_prev = np.zeros(n, dtype=bool)
     for k in range(steps):
+        if k:
+            _apply_wind(wind, k, env, orc)
         env.rollout(1)
         act_g = av.setpoints.cpu().numpy()
         act = streams.actions(k, mode)
@@ -149,7 +164,7 @@ def hover_step(env, seed: int, steps: int, *, env_offset: int = 0, reset_seq: in
     return run
 
 
-def hover_fused(env, seed: int, chunks, *, env_offset: int = 0, reset_seq: int = 0, episode0: int = 1, obs_bar: float = 1e-4) -> Run:
+def hover_fused(env, seed: int, chunks, *, env_offset: int = 0, reset_seq: int = 0, episode0: int = 1, obs_bar: float = 1e-4, wind: dict | None = None) -> Run:
     """The fused rollout (chunks of >= 4 env steps: k_hover_rollout with spares kept three ahead): the oracle runs step by step
     on the replayed actions and noise and resets on its OWN terminations; at the end of every chunk the step counters, flags,
     observations and rewards must agree.  An env off the oracle's schedule counts as a flip."""
@@ -157,6 +172,7 @@ def hover_fused(env, seed: int, chunks, *, env_offset: int = 0, reset_seq: int =
     run = Run("hover fused", n, obs_bar, obs_bar, 2000)
     streams = Streams(seed, n, env_offset=env_offset, noise_loc=4.0)
     orc = hover_oracle(env, n)
+    _apply_wind(wind, 0, env, orc)
     obs_g, _ = env.reset()
     obs_o = orc.o.env_reset(noise=streams.user_reset_noise(reset_seq).astype(np.float64))
     run.reset_obs = float(np.abs(obs_g.double().cpu().numpy() - obs_o).max())
@@ -164,7 +180,10 @@ def hover_fused(env, seed: int, chunks, *, env_offset: int = 0, reset_seq: int =
     done_prev = np.zeros(n, dtype=bool)
     steps_o = np.zeros(n, dtype=np.int64)
     k = 0
+    assert not wind or set(wind) <= {0, *np.cumsum(chunks)[:-1].tolist()}, "the wind can only change between fused launches"
     for chunk in chunks:
+        if k:
+            _apply_wind(wind, k, env, orc)
         env.rollout(chunk)
         assert np.array_equal(av.setpoints.cpu().numpy(), streams.actions(k + chunk - 1, mode))  # the last step's actions, written back
         for _ in range(chunk):
@@ -188,7 +207,7 @@ def hover_fused(env, seed: int, chunks, *, env_offset: int = 0, reset_seq: int =
 
 
 # ------------------------------------------------------------------------------------------------------- QuadX-Waypoints
-def quadx_waypoints(env, seed: int, steps: int, *, env_offset: int = 0, reset_seq: int = 0, episode0: int = 1, rng_seed: int = 5) -> Run:
+def quadx_waypoints(env, seed: int, steps: int, *, env_offset: int = 0, reset_seq: int = 0, episode0: int = 1, rng_seed: int = 5, wind: dict | None = None) -> Run:
     """Scripted actions; device-drawn waypoints (and yaw targets) replayed into the oracle."""
     import torch
 
@@ -200,6 +219,7 @@ def quadx_waypoints(env, seed: int, steps: int, *, env_offset: int = 0, reset_se
         run = Run("quadx-waypoints", n, 5e-4, 5e-3, 500)
     streams = Streams(seed, n, env_offset=env_offset, noise_loc=4.0)
     orc = OracleEngine(build_model("quadx", "cf2x"), oracle_config(env), n, np.tile([[0.0, 0.0, 1.0]], (n, 1)), np.zeros((n, 3)))
+    _apply_wind(wind, 0, env, orc)
     obs_g, _ = env.reset()
     tg = streams.waypoint_targets(0x80000000 | reset_seq, T, dome, min_height=0.1, yaw=yaw)
     obs_o = orc.o.env_reset(noise=streams.user_reset_noise(reset_seq).astype(np.float64), targets=tg.astype(np.float64).reshape(n, -1))
@@ -208,6 +228,8 @@ def quadx_waypoints(env, seed: int, steps: int, *, env_offset: int = 0, reset_se
     episode = np.full(n, episode0, dtype=np.int64)
     done_prev = np.zeros(n, dtype=bool)
     for k in range(steps):
+        if k:
+            _apply_wind(wind, k, env, orc)
         if mode == 7:
             act = _f(rng.uniform([-2.0, -2.0, -1.0, 0.5], [2.0, 2.0, 1.0, 3.0], (n, 4)))
         else:
@@ -233,13 +255,15 @@ def quadx_waypoints(env, seed: int, steps: int, *, env_offset: int = 0, reset_se
 
 
 # ---------------------------------------------------------------------------------------------------- Fixedwing-Waypoints
-def fixedwing_waypoints(env, seed: int, steps: int, *, env_offset: int = 0, reset_seq: int = 0, episode0: int = 1) -> Run:
+def fixedwing_waypoints(env, seed: int, steps: int, *, env_offset: int = 0, reset_seq: int = 0, episode0: int = 1, obs_bar: float = 5e-3,
+                        wind: dict | None = None) -> Run:
     """On-device RANDACT actions (U(-1, 1)^4, compared bit for bit with the replay on every env that stepped); device-drawn
     waypoints replayed into the oracle."""
     av, n, T, dome = env.aviary, env.num_envs, env.config.num_targets, env.config.flight_dome_size
-    run = Run("fixedwing-waypoints", n, 5e-3, 5e-3, 1000)  # target deltas are O(100 m) fp32 numbers
+    run = Run("fixedwing-waypoints", n, obs_bar, 5e-3, 1000)  # target deltas are O(100 m) fp32 numbers
     streams = Streams(seed, n, env_offset=env_offset, noise_loc=1.0)
     orc = OracleEngine(build_model("fixedwing", "fixedwing"), oracle_config(env), n, np.tile([[0.0, 0.0, 10.0]], (n, 1)), np.zeros((n, 3)))
+    _apply_wind(wind, 0, env, orc)
     obs_g, _ = env.reset()
     tg = streams.waypoint_targets(0x80000000 | reset_seq, T, dome, min_height=0.5)
     obs_o = orc.o.env_reset(noise=streams.user_reset_noise(reset_seq).astype(np.float64), targets=tg.astype(np.float64).reshape(n, -1))
@@ -247,6 +271,8 @@ def fixedwing_waypoints(env, seed: int, steps: int, *, env_offset: int = 0, rese
     episode = np.full(n, episode0, dtype=np.int64)
     done_prev = np.zeros(n, dtype=bool)
     for k in range(steps):
+        if k:
+            _apply_wind(wind, k, env, orc)
         env.rollout(1)
         act = streams.uniform_actions(k)
         assert np.array_equal(av.setpoints.cpu().numpy()[~done_prev], act[~done_prev]), k  # a resetting env draws no action
@@ -269,7 +295,7 @@ def fixedwing_waypoints(env, seed: int, steps: int, *, env_offset: int = 0, rese
 
 
 # --------------------------------------------------------------------------------------------------------- Rocket-Landing
-def rocket_landing(env, seed: int, steps: int, *, env_offset: int = 0, reset_seq: int = 0, episode0: int = 1, rng_seed: int = 3) -> Run:
+def rocket_landing(env, seed: int, steps: int, *, env_offset: int = 0, reset_seq: int = 0, episode0: int = 1, rng_seed: int = 3, wind: dict | None = None) -> Run:
     """Scripted actions; device-drawn randomised drops replayed into the oracle.  The crash step's observation and reward stay
     out of the comparison (a stiff impulse iteration on an 80 m/s impact: see test_timed_path_parity.py); envs that carry a
     stall-branch offset are counted as loose."""
@@ -281,6 +307,7 @@ def rocket_landing(env, seed: int, steps: int, *, env_offset: int = 0, reset_seq
     sp, so = streams.drop_poses(0x80000000 | reset_seq, ceiling, 200.0)
     sp, so = sp.astype(np.float64), so.astype(np.float64)
     orc = OracleEngine(build_model("rocket", "rocket", starting_fuel_ratio=0.05), oracle_config(env), n, sp, so)
+    _apply_wind(wind, 0, env, orc)
     obs_g, _ = env.reset()
     obs_o = orc.o.env_reset(noise=streams.user_reset_noise(reset_seq).astype(np.float64))
     run.reset_obs = float(np.abs(obs_g.double().cpu().numpy() - obs_o).max())
@@ -288,6 +315,8 @@ def rocket_landing(env, seed: int, steps: int, *, env_offset: int = 0, reset_seq
     episode = np.full(n, episode0, dtype=np.int64)
     done_prev = np.zeros(n, dtype=bool)
     for k in range(steps):
+        if k:
+            _apply_wind(wind, k, env, orc)
         act = _f(rng.uniform([-1, -1, -1, 0, 0, -1, -1], [1, 1, 1, 1, 1, 1, 1], (n, 7)))
         env.step(torch.as_tensor(act, dtype=torch.float32, device=av.device))
         og, rg, teg, trg, ig = _host(av)
@@ -329,7 +358,7 @@ def dogfight_spawns(streams: Streams, seq, rmin=10.0, rmax=50.0, A=2):
     return _f(pos), _f(orn)
 
 
-def dogfight(env, seed: int, steps: int, *, env_offset: int = 0, reset_seq: int = 0, episode0: int = 1, rng_seed: int = 8) -> Run:
+def dogfight(env, seed: int, steps: int, *, env_offset: int = 0, reset_seq: int = 0, episode0: int = 1, rng_seed: int = 8, wind: dict | None = None) -> Run:
     """1-vs-1 arenas, scripted actions, device-drawn spawns replayed into the oracle; an arena is re-spawned once both of its
     agents have left, and a flipped decision drops the whole arena."""
     import torch
@@ -339,6 +368,7 @@ def dogfight(env, seed: int, steps: int, *, env_offset: int = 0, reset_seq: int 
     streams = Streams(seed, n, env_offset=env_offset, noise_loc=1.0)
     sp, so = dogfight_spawns(streams, 0x80000000 | reset_seq)
     orc = OracleEngine(build_model("fixedwing", "acrowing"), oracle_config(env), n, sp, so)
+    _apply_wind(wind, 0, env, orc)
     obs_g, _ = env.reset()
     obs_o = orc.o.env_reset(noise=streams.user_reset_noise(reset_seq).astype(np.float64))
     run.reset_obs = float(np.abs(obs_g.double().cpu().numpy() - obs_o).max())
@@ -348,6 +378,8 @@ def dogfight(env, seed: int, steps: int, *, env_offset: int = 0, reset_seq: int 
     arena_reset = np.zeros(n, dtype=bool)  # per agent: its arena is re-spawned on this call
     pairs = lambda m: (m.reshape(-1, 2).all(axis=1)[:, None] & np.ones((1, 2), dtype=bool)).reshape(-1)  # noqa: E731
     for k in range(steps):
+        if k:
+            _apply_wind(wind, k, env, orc)
         act = _f(np.clip(rng.uniform(-1, 1, (n, 4)) * 0.4 + np.array([0.0, 0.15, 0.0, 0.0]) * (np.arange(n) % 5 == 0)[:, None], -1, 1))
         env.step(torch.as_tensor(act, dtype=torch.float32, device=av.device))
         og, rg, teg, trg, _ = _host(av)
