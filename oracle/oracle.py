@@ -44,6 +44,7 @@ def lib() -> C.CDLL:
         L.orc_df_set_actions.argtypes = [vp, C.POINTER(C.c_uint8), dp]
         L.orc_set_wind.argtypes = [vp, vp]
         L.orc_wind_field.argtypes = [vp, i64, dp, dp]
+        L.orc_surface_wrench.argtypes = [vp, C.c_int, i64, dp, dp, dp, dp, dp]
         L.orc_reset.argtypes = [vp, u8p]
         L.orc_set_mode.argtypes = [vp, C.c_int]
         L.orc_set_setpoints.argtypes = [vp, dp, C.c_int]
@@ -73,6 +74,19 @@ def _dp(a):
 
 def _u8(a):
     return None if a is None else a.ctypes.data_as(C.POINTER(C.c_uint8))
+
+
+def surface_wrench(model, si: int, actuation, vb, w):
+    """Lifting surface ``si`` of ``model`` on its own, in fp64: actuation[n] (after the lag), base-origin velocity vb[n][3]
+    and body rate w[n][3] (base frame, still air) -> force F[n][3] and torque T[n][3] about the base origin, base frame."""
+    L = lib()
+    act = np.ascontiguousarray(actuation, dtype=np.float64).reshape(-1)
+    vb = np.ascontiguousarray(vb, dtype=np.float64).reshape(-1, 3)
+    w = np.ascontiguousarray(w, dtype=np.float64).reshape(-1, 3)
+    assert len(vb) == len(act) and len(w) == len(act)
+    F, T = np.zeros((len(act), 3)), np.zeros((len(act), 3))
+    L.orc_surface_wrench(C.byref(model), int(si), len(act), _dp(act), _dp(vb), _dp(w), _dp(F), _dp(T))
+    return F, T
 
 
 class Oracle:

@@ -168,9 +168,12 @@ PFB_HD void surface_force(const SurfaceParams& sf, float& act, float cmd, Vec3 v
   float CM = -CN * (0.25f - 0.175f * (1.0f - aeff_m * 0.63661977236758134308f));
   // _jitted_compute_force_torque (lifting_surfaces.py:450-498); sin/cos(alpha) straight from the components
   float Q_area = sf.q_area * speed2;
+  // below FLT_MIN (in-plane airspeed under ~1e-19 m/s, where Q_area is ~1e-38 too) the force takes alpha = 0's direction:
+  // fast_rsqrt would flush a subnormal h2 to 0 on the device and return +inf
   float h2 = lifting * lifting + forward * forward;
-  float inv_h = h2 > 0.0f ? fast_rsqrt(h2) : 0.0f;
-  float sa = -lifting * inv_h, ca = h2 > 0.0f ? forward * inv_h : 1.0f;
+  const bool h_normal = h2 >= kFltMin;
+  float inv_h = h_normal ? fast_rsqrt(h2) : 0.0f;
+  float sa = -lifting * inv_h, ca = h_normal ? forward * inv_h : 1.0f;
   float lift = Cl * Q_area, drag = Cd * Q_area;
   float fn = lift * ca + drag * sa;
   float fp = lift * sa - drag * ca;

@@ -354,24 +354,14 @@ int pfb_sizeof_wind(void) { return (int)sizeof(PfbWind); }
 
 int pfb_set_wind(PfbHandle h, const PfbWind* wind) {
   if (!h) return fail("null handle");
-  WindParams w;
-  memset(&w, 0, sizeof(w));
   if (wind && wind->kind != PFB_WIND_NONE) {
     if (wind->kind < PFB_WIND_CONSTANT || wind->kind > PFB_WIND_EXP) return fail("unknown wind kind %d", wind->kind);
     if (!(wind->z_ref > 0.0)) return fail("wind z_ref must be positive");
     if (wind->kind == PFB_WIND_LOG && !(wind->z0 > 0.0 && wind->z0 < wind->z_ref)) return fail("log wind profile needs 0 < z0 < z_ref");
     if (wind->kind == PFB_WIND_POWER && !(wind->alpha >= 0.0)) return fail("power-law wind profile needs alpha >= 0, got %g", wind->alpha);
-    // alpha = 0 is the constant profile for every z (0^0 = 1); the kernels' exp2(alpha * log2(z)) would give 0 * -inf = NaN at z <= 0
-    w.kind = (wind->kind == PFB_WIND_POWER && wind->alpha == 0.0) ? PFB_WIND_CONSTANT : wind->kind;
-    w.bx = (float)wind->base[0]; w.by = (float)wind->base[1]; w.bz = (float)wind->base[2];
-    w.inv_zref = (float)(1.0 / wind->z_ref);
-    w.alpha = (float)wind->alpha;
-    if (wind->kind == PFB_WIND_LOG) {
-      w.z0 = (float)wind->z0;
-      w.inv_z0 = (float)(1.0 / wind->z0);
-      w.inv_log = (float)(1.0 / log(wind->z_ref / wind->z0));
-    }
   }
+  WindParams w;
+  pfb_narrow_wind(wind, w);
   if (h->d_spare && memcmp(&w, &h->qx.wind, sizeof(w)) != 0) {
     // The spare post-reset states were integrated in the old air.  Nothing may still be building them; then every record is
     // marked invalid but keeps its episode number, so each env's next reset integrates its warm-up inline, under the episode

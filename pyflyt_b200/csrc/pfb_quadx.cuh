@@ -179,12 +179,16 @@ PFB_HD void quadx_update_state(QuadXRegs& s) {
   s.vb.z = (float)(R.m02 * vx + R.m12 * vy + R.m22 * vz);
 }
 
-// atan2 without the IEEE-division / denormal slow paths: |error| < 2e-7 rad (tests/test_hostsim_parity.py).
-// Octant reduction to a = min/max in [0,1], odd minimax polynomial for atan(a), quadrant fix-ups.
+// atan2 without the IEEE-division / denormal slow paths: |error| < 4e-7 rad for max(|x|, |y|) in [FLT_MIN, 2^126)
+// (tests/test_device_math.py).  Octant reduction to a = min/max in [0,1], odd minimax polynomial for atan(a), quadrant fix-ups.
+// A subnormal max takes a = 0, the nearest multiple of pi/2 in its octant pair (|error| <= pi/4): fast_rcp would flush it to 0
+// on the device and overflow on the host, and mn * inf is NaN.  Only a link at rest in still air reaches it, where the
+// surface force is ~1e-38 N.  Outside the domain: max >= 2^126 gives a = 0 on the device (the reciprocal is subnormal and
+// flushed), and atan2_f(+-0, -0) = +-0 where IEEE atan2 gives +-pi.
 PFB_HD float atan2_f(float y, float x) {
   float ax = fabsf(x), ay = fabsf(y);
   float mx = fmaxf(ax, ay), mn = fminf(ax, ay);
-  float a = mx > 0.0f ? fast_div(mn, mx) : 0.0f;
+  float a = mx >= kFltMin ? fast_div(mn, mx) : 0.0f;
   float t = a * a;
   float r = 0.00282363896258175373077393f;
   r = fmaf(r, t, -0.0159569028764963150024414f);

@@ -8,6 +8,23 @@
 #include "../../include/pyflyt_b200.h"
 #include "pfb_quadx.cuh"
 
+// PfbWind (validated: kind 1..4, z_ref > 0, 0 < z0 < z_ref for the log profile, alpha >= 0) -> the fp32 block every
+// vehicle's parameter table carries.  NULL or PFB_WIND_NONE is still air.
+static void pfb_narrow_wind(const PfbWind* wind, pfb::WindParams& w) {
+  memset(&w, 0, sizeof(w));
+  if (!wind || wind->kind == PFB_WIND_NONE) return;
+  // alpha = 0 is the constant profile for every z (0^0 = 1); the kernels' exp2(alpha * log2(z)) would give 0 * -inf = NaN at z <= 0
+  w.kind = (wind->kind == PFB_WIND_POWER && wind->alpha == 0.0) ? PFB_WIND_CONSTANT : wind->kind;
+  w.bx = (float)wind->base[0]; w.by = (float)wind->base[1]; w.bz = (float)wind->base[2];
+  w.inv_zref = (float)(1.0 / wind->z_ref);
+  w.alpha = (float)wind->alpha;
+  if (wind->kind == PFB_WIND_LOG) {
+    w.z0 = (float)wind->z0;
+    w.inv_z0 = (float)(1.0 / wind->z0);
+    w.inv_log = (float)(1.0 / log(wind->z_ref / wind->z0));
+  }
+}
+
 static int build_quadx_params(const PfbModel& m, pfb::QuadXParams& q) {
   memset(&q, 0, sizeof(q));
   if (m.n_motors != 4) return fail("quadx model must have 4 motors, got %d", m.n_motors);

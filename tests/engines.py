@@ -23,6 +23,50 @@ if ROOT not in sys.path:
 from pyflyt_b200.models import PfbEnvConfig, build_model  # noqa: E402
 
 
+def euler_zyx_ref(q, lock=None):
+    """(roll, pitch, yaw) of the quaternion q = (x, y, z, w) in fp64, as p.getEulerFromQuaternion gives them
+    (btQuaternion::getEulerZYX with its +-0.99999 gimbal-lock branch).  ``lock`` True / False forces the gimbal-lock / regular
+    branch (a quaternion whose sarg rounds to either side of the snap)."""
+    import math
+
+    x, y, z, w = (float(v) for v in q)
+    sarg = -2.0 * (x * z - w * y)
+    if lock is None:
+        lock = abs(sarg) >= 0.99999
+    if lock:
+        if sarg < 0.0:
+            return 0.0, -0.5 * math.pi, 2.0 * math.atan2(x, -y)
+        return 0.0, 0.5 * math.pi, 2.0 * math.atan2(-x, y)
+    sarg = min(max(sarg, -1.0), 1.0)
+    return (math.atan2(2.0 * (y * z + w * x), w * w - x * x - y * y + z * z), math.asin(sarg),
+            math.atan2(2.0 * (x * y + w * z), w * w + x * x - y * y - z * z))
+
+
+def quat_from_euler_ref(roll, pitch, yaw):
+    """p.getQuaternionFromEuler (btQuaternion::setEulerZYX) in fp64 -> (x, y, z, w)."""
+    import math
+
+    cy, sy, cp, sp = math.cos(yaw / 2), math.sin(yaw / 2), math.cos(pitch / 2), math.sin(pitch / 2)
+    cr, sr = math.cos(roll / 2), math.sin(roll / 2)
+    return np.array([sr * cp * cy - cr * sp * sy, cr * sp * cy + sr * cp * sy, cr * cp * sy - sr * sp * cy, cr * cp * cy + sr * sp * sy])
+
+
+def quat_observation_ref(q):
+    """The reference's quaternion observation getQuaternionFromEuler(getEulerFromQuaternion(q)) (quadx_base_env.py:243), fp64."""
+    return quat_from_euler_ref(*euler_zyx_ref(q))
+
+
+def sign_rule_quaternions():
+    """24 000 unit quaternions [n][4] (x, y, z, w), fp64: 20 000 uniform on the sphere, then 4 000 from Euler angles with large
+    roll / yaw and steep pitch (where the observation's w_e < 0) up to near gimbal lock, each with a random sign."""
+    rng = np.random.default_rng(3)
+    qs = rng.normal(size=(20000, 4))
+    eul = np.column_stack([rng.uniform(-np.pi, np.pi, 4000), rng.uniform(-1.5705, 1.5705, 4000), rng.uniform(-np.pi, np.pi, 4000)])
+    extra = [quat_from_euler_ref(r, p, y) * rng.choice([-1.0, 1.0]) for r, p, y in eul]
+    qs = np.vstack([qs, np.array(extra)])
+    return qs / np.linalg.norm(qs, axis=1, keepdims=True)
+
+
 def hover_config(flight_mode=0, angle_representation="quaternion", sparse=False, dome=3.0, agent_hz=40, max_duration=10.0, autoreset=False):
     e = PfbEnvConfig()
     e.env_kind = 1

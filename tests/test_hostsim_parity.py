@@ -69,42 +69,16 @@ def test_observation_quaternion_sign_rule():
     """The kernel reports +-q with the sign getQuaternionFromEuler(getEulerFromQuaternion(q)) would give
     (quadx_base_env.py:243), without evaluating any trigonometric function outside gimbal lock."""
     import ctypes as C
-    import math
 
-    from engines import hostsim_lib
+    from engines import hostsim_lib, quat_observation_ref, sign_rule_quaternions
 
     L = hostsim_lib()
-
-    def ref(q):  # the reference's round trip, fp64 (btQuaternion::getEulerZYX / setEulerZYX)
-        x, y, z, w = q
-        sarg = -2.0 * (x * z - w * y)
-        if sarg <= -0.99999:
-            roll, pitch, yaw = 0.0, -0.5 * math.pi, 2.0 * math.atan2(x, -y)
-        elif sarg >= 0.99999:
-            roll, pitch, yaw = 0.0, 0.5 * math.pi, 2.0 * math.atan2(-x, y)
-        else:
-            pitch = math.asin(sarg)
-            roll = math.atan2(2.0 * (y * z + w * x), w * w - x * x - y * y + z * z)
-            yaw = math.atan2(2.0 * (x * y + w * z), w * w + x * x - y * y - z * z)
-        cy, sy, cp, sp, cr, sr = math.cos(yaw / 2), math.sin(yaw / 2), math.cos(pitch / 2), math.sin(pitch / 2), math.cos(roll / 2), math.sin(roll / 2)
-        return np.array([sr * cp * cy - cr * sp * sy, cr * sp * cy + sr * cp * sy, cr * cp * sy - sr * sp * cy, cr * cp * cy + sr * sp * sy])
-
-    rng = np.random.default_rng(3)
-    qs = rng.normal(size=(20000, 4))
-    # include large roll/yaw with steep pitch (where w_e < 0 happens) and near-gimbal-lock attitudes
-    eul = np.column_stack([rng.uniform(-np.pi, np.pi, 4000), rng.uniform(-1.5705, 1.5705, 4000), rng.uniform(-np.pi, np.pi, 4000)])
-    extra = []
-    for r, p, y in eul:
-        cy, sy, cp, sp, cr, sr = math.cos(y / 2), math.sin(y / 2), math.cos(p / 2), math.sin(p / 2), math.cos(r / 2), math.sin(r / 2)
-        q = np.array([sr * cp * cy - cr * sp * sy, cr * sp * cy + sr * cp * sy, cr * cp * sy - sr * sp * cy, cr * cp * cy + sr * sp * sy])
-        extra.append(q * rng.choice([-1.0, 1.0]))
-    qs = np.vstack([qs, np.array(extra)])
-    qs /= np.linalg.norm(qs, axis=1, keepdims=True)
+    qs = sign_rule_quaternions()
     out = np.zeros(4, dtype=np.float32)
     worst, negatives = 0.0, 0
     for q in qs:
         L.hs_obs_quat(q.ctypes.data_as(C.POINTER(C.c_double)), out.ctypes.data_as(C.POINTER(C.c_float)))
-        r = ref(q)
+        r = quat_observation_ref(q)
         negatives += int(r[3] < 0)
         worst = max(worst, float(np.abs(out - r).max()))
     assert negatives > 50  # the w_e < 0 branch is exercised

@@ -81,7 +81,10 @@ def test_hover_philox_autoreset_matches_oracle(n, steps, randact):
     print(f"\n[timed-path parity] {n} envs x {steps} steps: {n_done} episodes finished, {n_resets} autoresets, flips {n_flip}; "
           f"max |obs| {worst_obs:.2e}, max |reward| {worst_rew:.2e}, max |noise dump - replay| {worst_noise:.2e}")
     assert n_resets > n  # every env was reset more than once on average
-    assert worst_noise < 5e-4  # the device Box-Muller uses __logf / __sincosf / sqrt.approx: ~2e-4 absolute on N(4, 1) draws
+    # the device Box-Muller (__logf / __sincosf / sqrt.approx) is within 2.2e-4 of fp64 over every u1 and every u2
+    # (tests/test_device_math.py::test_box_muller_device); the worst is at u1 = 1 - 2^-24, where __logf's absolute error is
+    # comparable to -ln u1 = 6e-8 and r = sqrt(-2 ln u1) = 3.5e-4 carries it as a square root
+    assert worst_noise < 5e-4
     assert n_flip <= max(2, n // 4096)
     assert worst_obs < 1e-4 and worst_rew < 1e-4
     env.close()
