@@ -249,6 +249,20 @@ int pfb_model_from_files(int kind, const char* urdf_path, const char* yaml_path,
 int pfb_create(const PfbModel* model, const PfbEnvConfig* env, int64_t n_envs, int device, uint64_t seed,
                PfbHandle* out);
 int pfb_destroy(PfbHandle h);
+/* Aviary(drone_type=[...]) with drones of several kinds (aviary.py:139-190): drone i flies models[model_index[i]] (host array
+ * of n entries, each < k).  Every table has the same physics_hz and control_hz; at most PFB_MAX_QUADX_MODELS QuadX tables,
+ * one fixed-wing and one rocket table.  aviary_cfg: NULL, or a PFB_ENV_NONE config of which only contact_response is read.
+ * The handle is an Aviary handle (the env entry points, pfb_set_models and pfb_set_base_velocity refuse it) with:
+ *   state     pfb_state_floats() floats, carved by the library into one region per kind (PFB_LAYOUT_BY_KIND): QuadX
+ *             warp-tiled, then fixed-wing and rocket field-major, each on a 128-byte boundary; istate [pfb_istate_rows][N];
+ *   setpoint  [N][7] (pfb_setpoint_dim): drone i reads its own length (QuadX 4, fixed-wing 6, rocket 7), the rest is zero
+ *             after pfb_reset / pfb_set_mode;
+ *   aux_state [N][9] (pfb_aux_dim), zero past the drone's own aux length (QuadX 4, fixed-wing 6, rocket 9);
+ *   obs       [N][6] (pfb_obs_dim): pfb_observe_state writes the hi and lo fp32 words of each drone's position there.
+ * pfb_aviary_step steps every kind in ONE launch.  Drone i draws the noise drone i of a single-kind handle with the same seed
+ * draws (Philox stream of env id i, column i of injected noise), so its trajectory is that drone's in such a handle.       */
+int pfb_create_mixed(const PfbModel* models, int k, const uint8_t* model_index, int64_t n, const PfbEnvConfig* aviary_cfg, int device,
+                     uint64_t seed, PfbHandle* out);
 /* env.reset(seed=s) of the reference re-creates np_random: the same seed must give the same episodes.  Re-keys the Philox
  * streams and rewinds every call counter (step / reset / Aviary step numbers, autoreset episode numbers), stream-ordered on
  * `stream`.  It invalidates the spare post-reset states (they hold warm-ups of the old streams): an env handle must follow it
@@ -284,6 +298,7 @@ int pfb_state_rows(PfbHandle h);     /* F of PfbBuffers.state                   
  * allocate (tiles are padded to 32 envs); step_count and the flag word live in rows 17 / 18 of the tile as int32 bits.  */
 #define PFB_LAYOUT_FIELD_MAJOR 0
 #define PFB_LAYOUT_WARP_TILED 1
+#define PFB_LAYOUT_BY_KIND 2 /* a mixed-kind handle (pfb_create_mixed): one region per vehicle kind, in that kind's layout */
 int pfb_state_layout(PfbHandle h);
 int64_t pfb_state_floats(PfbHandle h);
 int pfb_istate_rows(PfbHandle h);    /* I of PfbBuffers.istate                                        */

@@ -65,6 +65,7 @@ def lib() -> C.CDLL:
     vp, i64, u64, i32 = C.c_void_p, C.c_int64, C.c_uint64, C.c_int
     L.pfb_last_error.restype = C.c_char_p
     L.pfb_create.argtypes = [vp, vp, i64, i32, u64, C.POINTER(vp)]
+    L.pfb_create_mixed.argtypes = [vp, i32, vp, i64, vp, i32, u64, C.POINTER(vp)]
     L.pfb_model_from_files.argtypes = [i32, C.c_char_p, C.c_char_p, C.c_double, C.c_double, vp]
     L.pfb_destroy.argtypes = [vp]
     L.pfb_set_env_offset.argtypes = [vp, u64]
@@ -110,7 +111,7 @@ def check(rc: int) -> None:
 
 EXPORTS = [
     "pfb_last_error", "pfb_abi_version", "pfb_sizeof_model", "pfb_sizeof_env_config", "pfb_sizeof_buffers",
-    "pfb_model_from_files", "pfb_create", "pfb_destroy", "pfb_set_env_offset", "pfb_state_rows", "pfb_state_layout", "pfb_state_floats", "pfb_set_noise_dump", "pfb_reseed", "pfb_set_wind", "pfb_sizeof_wind", "pfb_set_models",
+    "pfb_model_from_files", "pfb_create", "pfb_create_mixed", "pfb_destroy", "pfb_set_env_offset", "pfb_state_rows", "pfb_state_layout", "pfb_state_floats", "pfb_set_noise_dump", "pfb_reseed", "pfb_set_wind", "pfb_sizeof_wind", "pfb_set_models",
     "pfb_istate_rows", "pfb_setpoint_dim",
     "pfb_obs_dim", "pfb_aux_dim", "pfb_bind", "pfb_reset", "pfb_set_mode", "pfb_set_modes", "pfb_aviary_step", "pfb_observe_state",
     "pfb_set_base_velocity",

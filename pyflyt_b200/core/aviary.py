@@ -19,6 +19,15 @@ contact, so they never need more).  ``contact_response=True`` makes the floor pu
 drones: contact impulses with Coulomb friction on the corners / rim points of each drone's collision primitives, so drones
 take off from, land on, slide along and rest on the floor (DESIGN.md §4c).
 
+``drone_type`` may be a list with one kind per drone, as in the reference (aviary.py:139-190, examples/core/08_mixed_drones.py):
+a batch then flies QuadX, fixed-wing and rocket drones together, all stepped by one CUDA launch (DESIGN.md §4d).  Every drone
+keeps its own kind's surface: ``set_setpoint(i, sp)`` takes drone ``i``'s own setpoint length (QuadX 4, fixed-wing 4 or 6,
+rocket 7) and ``state(i)`` / ``aux_state(i)`` return its own aux length (4, 6 or 9); ``setpoints`` is ``[N, 7]`` and
+``all_aux_states`` a list of ``N`` tensors.  Each kind's drones take their tables from their own ``drone_options`` entries (up
+to ``MAX_QUADX_MODELS`` QuadX models, one fixed-wing and one rocket model), and every drone runs at one ``control_hz``.  Such
+a batch is an Aviary only: no ``env_config``, no ``set_base_velocity``, no ``state_row``.  Drone ``i`` draws the random stream
+drone ``i`` of a single-kind batch with the same seed draws, so it flies exactly as it would there.
+
 All state is held in caller-visible ``torch`` tensors; the CUDA library (libpyflyt_b200.so) only sees
 raw device pointers.  There is no CPU path.
 """
@@ -32,7 +41,19 @@ import numpy as np
 import torch
 
 from .. import _lib
-from ..models import ModelSetError, PfbEnvConfig, PfbModel, build_model, build_model_set
+from ..models import ModelSetError, PfbEnvConfig, PfbModel, build_mixed_model_set, build_model, build_model_set
+
+_KINDS = ("quadx", "fixedwing", "rocket")
+_MODE_RANGE = {"quadx": (-1, 7), "fixedwing": (-1, 0), "rocket": (0, 0)}  # quadx.py:259-262, fixedwing.py:216-219, base_drone.py:252-255
+_SETPOINT_LEN = {"quadx": (4,), "fixedwing": (4, 6), "rocket": (7,)}
+_AUX_LEN = {"quadx": 4, "fixedwing": 6, "rocket": 9}
+
+
+def _check_mode(kind: str, mode: int) -> None:
+    lo, hi = _MODE_RANGE[kind]
+    if mode < lo or mode > hi:
+        # quadx.py:259-262, fixedwing.py:216-219, base_drone.py:252-255
+        raise ValueError(f"`mode` must be between {lo} and {hi} or be registered in self.registered_controllers.keys()=dict_keys([]), got {mode}.")
 
 
 class AviaryInitException(Exception):
@@ -75,15 +96,31 @@ class BatchedAviary:
             raise AviaryInitException(f"start_pos must be shape (n, 3), currently {start_pos.shape}.")
         if start_orn.shape != start_pos.shape:
             raise AviaryInitException(f"start_orn must be same shape as start_pos, currently {start_orn.shape}.")
+        kinds = None  # one vehicle kind per drone (a list that holds more than one kind), else None
         if isinstance(drone_type, (tuple, list)):
             if len(set(drone_type)) != 1:
-                raise AviaryInitException("the batched stepper runs one vehicle kind per batch; build one BatchedAviary per kind.")
-            drone_type = drone_type[0]
-        if drone_type not in ("quadx", "fixedwing", "rocket"):
+                # the reference's checks and messages (aviary.py:140-148, 178-186)
+                if len(drone_type) != start_pos.shape[0]:
+                    raise AviaryInitException(
+                        f"If multiple `drone_types` are used, must have same number of `drone_types` ({len(drone_type)}) as number of drones ({start_pos.shape[0]})."
+                    )
+                if not all(dt in _KINDS for dt in drone_type):
+                    raise AviaryInitException(f"One of types in `drone_type` {drone_type} is not amongst known types {dict.fromkeys(_KINDS).keys()}.")
+                if env_config is not None:
+                    raise AviaryInitException("a batch of several vehicle kinds is an Aviary only; an env handle (env_config) flies one kind.")
+                kinds = [str(k) for k in drone_type]
+            else:
+                drone_type = drone_type[0]
+        if kinds is None and drone_type not in ("quadx", "fixedwing", "rocket"):
             raise AviaryInitException(f"Can't find `drone_type` {drone_type} amongst known types ['quadx', 'fixedwing', 'rocket'].")
         # one options dict per drone (aviary.py:75, 196-199): the distinct vehicle tables + the model index of every drone
         models, index = None, None
-        if drone_options is not None and not isinstance(drone_options, dict):
+        if kinds is not None:
+            try:
+                models, index = build_mixed_model_set(kinds, drone_options, physics_hz, int(start_pos.shape[0]))
+            except ModelSetError as e:
+                raise AviaryInitException(str(e)) from None
+        elif drone_options is not None and not isinstance(drone_options, dict):
             try:
                 models, index = build_model_set(drone_type, drone_options, physics_hz, int(start_pos.shape[0]))
             except ModelSetError as e:
@@ -92,7 +129,8 @@ class BatchedAviary:
             raise _lib.PfbError("pyflyt_b200 needs a CUDA device (H100, sm_90a); there is no CPU fallback.")
         self.device = torch.device(device)
         self.num_drones = int(start_pos.shape[0])
-        self.drone_type = drone_type
+        self.drone_type = drone_type if kinds is None else kinds
+        self.kinds = kinds
         self.physics_hz = int(physics_hz)
         self.physics_period = 1.0 / physics_hz
         if models is None:
@@ -118,10 +156,16 @@ class BatchedAviary:
         L = _lib.lib()
         self._h = C.c_void_p()
         dev_index = self.device.index if self.device.index is not None else torch.cuda.current_device()
-        _lib.check(L.pfb_create(C.byref(self.model), C.byref(env_config) if env_config is not None else None, self.num_drones, dev_index, self.seed, C.byref(self._h)))
+        if kinds is not None:  # drone i flies models[index[i]], each kind its own sub-batch inside the handle
+            tables = (PfbModel * len(models))(*models)
+            idx = np.ascontiguousarray(index, dtype=np.uint8)
+            _lib.check(L.pfb_create_mixed(tables, len(models), idx.ctypes.data_as(C.c_void_p), self.num_drones,
+                                          C.byref(env_config) if env_config is not None else None, dev_index, self.seed, C.byref(self._h)))
+        else:
+            _lib.check(L.pfb_create(C.byref(self.model), C.byref(env_config) if env_config is not None else None, self.num_drones, dev_index, self.seed, C.byref(self._h)))
         _lib.check(L.pfb_set_env_offset(self._h, int(env_offset)))
         n, dev = self.num_drones, self.device
-        if len(self.models) > 1:  # drone i flies self.models[model_index[i]]; one table keeps the handle as pfb_create made it
+        if kinds is None and len(self.models) > 1:  # drone i flies self.models[model_index[i]]; one table keeps the handle as pfb_create made it
             tables = (PfbModel * len(models))(*models)
             idx = np.ascontiguousarray(index, dtype=np.uint8)
             _lib.check(L.pfb_set_models(self._h, tables, len(models), idx.ctypes.data_as(C.c_void_p)))
@@ -133,7 +177,11 @@ class BatchedAviary:
         # persistent state: fp32 SoA, field-major [F][N] or warp-tiled [N/32][F/4][32][4] (include/pyflyt_b200.h)
         self.state_rows = int(L.pfb_state_rows(self._h))
         self.tiled = int(L.pfb_state_layout(self._h)) == 1
-        if self.tiled:
+        if kinds is not None:  # one flat buffer; the library carves it into one region per kind, each in that kind's layout
+            self.state_tensor = torch.zeros((int(L.pfb_state_floats(self._h)),), **f32)
+            self._setpoint_len = [_SETPOINT_LEN[k] for k in kinds]
+            self._aux_len = [_AUX_LEN[k] for k in kinds]
+        elif self.tiled:
             self.state_tensor = torch.zeros((int(L.pfb_state_floats(self._h)) // (self.state_rows * 32), self.state_rows // 4, 32, 4), **f32)
         else:
             self.state_tensor = torch.zeros((self.state_rows, n), **f32)
@@ -193,6 +241,9 @@ class BatchedAviary:
         A list whose entries differ flies each drone in its own mode until the next ``set_mode(int)`` or ``reset()`` (Aviary
         handles only; an env flies its ``flight_mode``).  Drones ``32 k .. 32 k + 31`` share one warp: a batch steps fastest
         when each such tile flies one mode (DESIGN.md §4b)."""
+        if self.kinds is not None:
+            self._set_mode_mixed(flight_modes)
+            return
         lo, hi = (-1, 7) if self.drone_type == "quadx" else ((-1, 0) if self.drone_type == "fixedwing" else (0, 0))
 
         def check_range(mode: int) -> None:
@@ -217,10 +268,49 @@ class BatchedAviary:
         _lib.check(_lib.lib().pfb_set_mode(self._h, mode, self._s()))
         self._state_fresh = False
 
+    def _set_mode_mixed(self, flight_modes) -> None:
+        """``set_mode`` of a batch of several kinds.  Every drone's mode is checked against its own kind's range first, and the
+        first invalid one raises its kind's ``ValueError`` with nothing changed.  (The reference's loop, aviary.py:454-458, would
+        already have set the mode of the drones before that one.)"""
+        n = self.num_drones
+        if isinstance(flight_modes, (list, tuple)):
+            if len(flight_modes) != n:
+                raise AssertionError(f"Expected {n} flight_modes, got {len(flight_modes)}.")
+            modes = [int(m) for m in flight_modes]
+        else:
+            modes = [int(flight_modes)] * n
+        for kind, m in zip(self.kinds, modes):
+            _check_mode(kind, m)
+        if isinstance(flight_modes, (list, tuple)):
+            arr = np.ascontiguousarray(modes, dtype=np.int8)
+            _lib.check(_lib.lib().pfb_set_modes(self._h, arr.ctypes.data_as(C.c_void_p), self._s()))
+        else:
+            _lib.check(_lib.lib().pfb_set_mode(self._h, modes[0], self._s()))
+        self._state_fresh = False
+
+    def _setpoint_row(self, index: int, setpoint) -> torch.Tensor:
+        """Drone ``index``'s setpoint of its own length, zero-padded to the 7 columns of a batch of several kinds."""
+        sp = torch.as_tensor(setpoint, dtype=torch.float32).reshape(-1)
+        allowed = self._setpoint_len[index]
+        if sp.numel() not in allowed:
+            raise ValueError(f"drone {index} is a {self.kinds[index]}: its setpoint has length {' or '.join(map(str, allowed))}, got {sp.numel()}.")
+        row = torch.zeros(self.setpoint_dim, dtype=torch.float32)
+        row[: sp.numel()] = sp
+        return row
+
     def set_setpoint(self, index: int, setpoint) -> None:
+        if self.kinds is not None:
+            self.setpoints[index] = self._setpoint_row(index, setpoint).to(self.device)
+            return
         self.setpoints[index] = torch.as_tensor(setpoint, dtype=torch.float32, device=self.device)
 
     def set_all_setpoints(self, setpoints) -> None:
+        """A batch of several kinds takes a padded ``[N, 7]`` array or a sequence of ``N`` per-drone setpoints (aviary.py:477-478
+        indexes ``setpoints[i]``)."""
+        if self.kinds is not None and not (hasattr(setpoints, "shape") and tuple(setpoints.shape) == (self.num_drones, self.setpoint_dim)):
+            if len(setpoints) != self.num_drones:
+                raise ValueError(f"Expected {self.num_drones} setpoints, got {len(setpoints)}.")
+            setpoints = torch.stack([self._setpoint_row(i, sp) for i, sp in enumerate(setpoints)])
         self.setpoints.copy_(torch.as_tensor(setpoints, dtype=torch.float32, device=self.device))
 
     def step(self, n_steps: int = 1, noise: torch.Tensor | None = None) -> None:
@@ -239,6 +329,7 @@ class BatchedAviary:
 
     def set_base_velocity(self, lin_vel: torch.Tensor, ang_vel: torch.Tensor) -> None:
         """``p.resetBaseVelocity`` for every drone (used by rocket_base_env.py:228): [N, 3] world-frame tensors."""
+        self._single_kind("set_base_velocity")
         lin = torch.as_tensor(lin_vel, dtype=torch.float32, device=self.device).reshape(self.num_drones, 3).contiguous()
         ang = torch.as_tensor(ang_vel, dtype=torch.float32, device=self.device).reshape(self.num_drones, 3).contiguous()
         _lib.check(_lib.lib().pfb_set_base_velocity(self._h, C.c_void_p(lin.data_ptr()), C.c_void_p(ang.data_ptr()), self._s()))
@@ -256,14 +347,20 @@ class BatchedAviary:
         return self._drone_state.view(self.num_drones, 4, 3)
 
     @property
-    def all_aux_states(self) -> torch.Tensor:
+    def all_aux_states(self) -> torch.Tensor | list[torch.Tensor]:
+        """(N, A) tensor; a batch of several kinds returns a list of ``N`` tensors of each drone's own aux length (aviary.py:396-411)."""
         self._refresh()
+        if self.kinds is not None:
+            return [self._aux_state[i, : self._aux_len[i]] for i in range(self.num_drones)]
         return self._aux_state
 
     def state(self, index: int) -> torch.Tensor:
         return self.all_states[index]
 
     def aux_state(self, index: int) -> torch.Tensor:
+        if self.kinds is not None:
+            self._refresh()
+            return self._aux_state[index, : self._aux_len[index]]
         return self.all_aux_states[index]
 
     @property
@@ -273,8 +370,13 @@ class BatchedAviary:
         return self._contact.bool()
 
     # ------------------------------------------------------------------ raw state access (tests, debugging)
+    def _single_kind(self, what: str) -> None:
+        if self.kinds is not None:
+            raise NotImplementedError(f"{what} is not available on a batch of several vehicle kinds (drone_type={sorted(set(self.kinds))}).")
+
     def state_row(self, row: int) -> torch.Tensor:
         """[N] fp32 copy-free view (field-major) or gathered copy (warp-tiled) of state row ``row``."""
+        self._single_kind("state_row (a kind-specific state layout)")
         if not self.tiled:
             return self.state_tensor[row]
         return self.state_tensor[:, row // 4, :, row % 4].reshape(-1)[: self.num_drones]
@@ -286,6 +388,9 @@ class BatchedAviary:
     @property
     def precise_positions(self) -> torch.Tensor:
         """(N, 3) float64 world positions as the kernels carry them: hi + lo fp32 words of the state tensor."""
+        if self.kinds is not None:  # pfb_observe_state writes the hi and lo words into obs [N, 6]
+            self._refresh()
+            return self.obs[:, :3].double() + self.obs[:, 3:6].double()
         lo = {"quadx": 25, "fixedwing": 19, "rocket": 22}[self.drone_type]
         return torch.stack([self.state_row(k).double() + self.state_row(lo + k).double() for k in range(3)], dim=1)
 
@@ -324,6 +429,7 @@ class BatchedAviary:
     def set_noise_dump(self, buf: torch.Tensor | None) -> None:
         """Test aid: ``buf`` [env_step_ratio * updates_per_step, N] fp32 receives every motor-noise draw of the following
         QuadX-Hover ``env_step`` calls (None = off)."""
+        self._single_kind("set_noise_dump")
         self._noise_dump = buf
         _lib.check(_lib.lib().pfb_set_noise_dump(self._h, None if buf is None else C.c_void_p(buf.data_ptr())))
 
@@ -337,6 +443,7 @@ class BatchedAviary:
         """env.reset() for all / masked envs.  ``targets`` [N, 3*num_targets] installs explicit waypoints
         (parity tests); by default they are drawn on device like ``WaypointHandler.reset``.  ``seed``: ``reseed(seed)`` first;
         that rewinds every env, so it resets the whole batch and takes no ``mask``."""
+        self._single_kind("env_reset")
         if seed is not None:
             if mask is not None:
                 raise ValueError("reset(seed=...) re-keys the random streams of every env: it resets the whole batch and takes no mask")
@@ -357,6 +464,7 @@ class BatchedAviary:
 
     def env_step(self, actions: torch.Tensor | None = None, noise: torch.Tensor | None = None) -> None:
         """One fused env.step() for every env; ``actions`` [N, S] fp32 on this device (None = ``self.setpoints``)."""
+        self._single_kind("env_step")
         act = None
         if actions is not None:
             assert actions.is_cuda and actions.dtype == torch.float32 and actions.is_contiguous()
@@ -383,6 +491,7 @@ class BatchedAviary:
     def dogfight_physics(self, payload: torch.Tensor, actions: torch.Tensor | None = None, noise: torch.Tensor | None = None,
                          first: bool = False, do_reset: bool = False, aviary_index: int = 0) -> None:
         """Split dogfight, half 1: integrate one Aviary step (or reset + warm-up) and publish ``payload`` [N, 20]."""
+        self._single_kind("dogfight_physics")
         act = None if actions is None else C.c_void_p(actions.data_ptr())
         nz = None if noise is None else C.c_void_p(noise.data_ptr())
         _lib.check(_lib.lib().pfb_dogfight_physics(self._h, act, nz, C.c_void_p(payload.data_ptr()), int(first), int(do_reset), int(aviary_index), self._s()))
@@ -393,6 +502,7 @@ class BatchedAviary:
                               peer_flags: torch.Tensor | None = None, rank: int = 0, epoch: int = 0) -> None:
         """Split dogfight, half 1 with the exchange fused in: every payload is stored straight into all ranks' tables
         (``peer_tables``: int64 device tensor of ``world`` peer-mapped base pointers)."""
+        self._single_kind("dogfight_physics_peer")
         act = None if actions is None else C.c_void_p(actions.data_ptr())
         nz = None if noise is None else C.c_void_p(noise.data_ptr())
         fl = None if peer_flags is None else C.c_void_p(peer_flags.data_ptr())
@@ -403,6 +513,7 @@ class BatchedAviary:
     def dogfight_combat_wait(self, table: torch.Tensor, first_global_agent: int, num_arenas: int, last: int, flags: torch.Tensor,
                              world: int, epoch: int) -> None:
         """Split dogfight, half 2, waiting in-kernel until every rank's physics kernel has raised its flag to ``epoch``."""
+        self._single_kind("dogfight_combat_wait")
         _lib.check(_lib.lib().pfb_dogfight_combat_wait(self._h, C.c_void_p(table.data_ptr()), int(first_global_agent), int(num_arenas), int(last),
                                                        C.c_void_p(flags.data_ptr()), int(world), int(epoch), self._s()))
         self._state_fresh = False
@@ -410,6 +521,7 @@ class BatchedAviary:
     def dogfight_split_step(self, actions: torch.Tensor, peer_tables: torch.Tensor, peer_flags: torch.Tensor, tables: torch.Tensor,
                             flags: torch.Tensor, world: int, rank: int, epoch0: int, first_global_agent: int, num_arenas: int) -> None:
         """A whole env step of the split dogfight (fused exchange, in-kernel signalling) in one library call."""
+        self._single_kind("dogfight_split_step")
         _lib.check(_lib.lib().pfb_dogfight_split_step(self._h, C.c_void_p(actions.data_ptr()), C.c_void_p(peer_tables.data_ptr()),
                                                       C.c_void_p(peer_flags.data_ptr()), C.c_void_p(tables.data_ptr()), C.c_void_p(flags.data_ptr()),
                                                       int(world), int(rank), int(epoch0), int(first_global_agent), int(num_arenas), self._s()))
@@ -417,6 +529,7 @@ class BatchedAviary:
 
     def dogfight_combat(self, table: torch.Tensor, first_global_agent: int, num_arenas: int, last: int) -> None:
         """Split dogfight, half 2: combat state from the all-gathered payload ``table`` [2 * num_arenas, 20]."""
+        self._single_kind("dogfight_combat")
         _lib.check(_lib.lib().pfb_dogfight_combat(self._h, C.c_void_p(table.data_ptr()), int(first_global_agent), int(num_arenas), int(last), self._s()))
         self._state_fresh = False
 
@@ -436,6 +549,8 @@ class BatchedAviary:
 
     def env_step_mapped(self, actions: torch.Tensor, obs: torch.Tensor, reward: torch.Tensor, term: torch.Tensor, trunc: torch.Tensor) -> None:
         """Zero-copy end-to-end step: the kernel reads ``actions`` from and writes the results into PINNED host tensors."""
+        self._single_kind("env_step_mapped")
+        self._single_kind("env_rollout")
         for t in (actions, obs, reward, term, trunc):
             assert not t.is_cuda and t.is_contiguous() and t.is_pinned()
         _lib.check(_lib.lib().pfb_env_step_mapped(self._h, C.c_void_p(actions.data_ptr()), C.c_void_p(obs.data_ptr()), C.c_void_p(reward.data_ptr()), C.c_void_p(term.data_ptr()), C.c_void_p(trunc.data_ptr()), self._s()))
@@ -443,6 +558,7 @@ class BatchedAviary:
 
     def env_step_host(self, actions: torch.Tensor, obs: torch.Tensor, reward: torch.Tensor, term: torch.Tensor, trunc: torch.Tensor) -> None:
         """Pinned-host in, pinned-host out (the end-to-end path bench.py times)."""
+        self._single_kind("env_step_host")
         for t in (actions, obs, reward, term, trunc):
             assert not t.is_cuda and t.is_contiguous()
         _lib.check(_lib.lib().pfb_env_step_host(self._h, C.c_void_p(actions.data_ptr()), C.c_void_p(obs.data_ptr()), C.c_void_p(reward.data_ptr()), C.c_void_p(term.data_ptr()), C.c_void_p(trunc.data_ptr()), self._s()))

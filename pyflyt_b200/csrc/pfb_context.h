@@ -94,6 +94,8 @@ struct PfbContext {
   uint8_t* d_model_index;
   // one flight mode per drone (pfb_set_modes; Aviary handles): device [whole tiles * 32], valid while mode == kModePerDrone
   int8_t* d_modes;
+  // mixed-kind Aviary handle (pfb_create_mixed, pfb_mixed.cu): one sub-handle per vehicle kind; nullptr = one kind
+  struct MixedKinds* mixed;
 };
 
 // PfbContext::mode of an Aviary handle whose drones fly the modes in d_modes; pfb_set_mode and a full pfb_reset replace it
@@ -318,6 +320,21 @@ int df_split_physics(PfbContext* h, const float* actions, const float* noise, fl
                      const uint64_t* peer_flags, int rank, int epoch, int first, int do_reset, int sub, cudaStream_t s);
 int df_split_combat(PfbContext* h, const float* table, int64_t first_gid, int64_t num_arenas, int last, const int* wait_flags, int world, int epoch,
                     cudaStream_t s);
+
+// mixed-kind Aviary handles (pfb_mixed.cu): what the C-ABI entry points run when h->mixed is set
+int mx_state_rows(const PfbContext* h);
+int mx_istate_rows(const PfbContext* h);
+int64_t mx_state_floats(const PfbContext* h);
+int mx_bind(PfbContext* h, const PfbBuffers* b);
+int mx_reset(PfbContext* h, const uint8_t* mask, cudaStream_t s);
+int mx_set_mode(PfbContext* h, int mode, cudaStream_t s);
+int mx_set_modes(PfbContext* h, const int8_t* modes, cudaStream_t s);
+int mx_aviary_step(PfbContext* h, int n_steps, const float* noise, cudaStream_t s);
+int mx_observe(PfbContext* h, cudaStream_t s);
+int mx_set_wind(PfbContext* h, const PfbWind* wind);
+int mx_reseed(PfbContext* h, uint64_t seed, cudaStream_t s);
+int64_t mx_launches(const PfbContext* h);  // launches of the sub-handles (their resets and mode changes)
+void mx_destroy(PfbContext* h);
 
 // QuadX-Waypoints translation unit (pfb_quadx_wp.cu)
 int qwp_state_rows();

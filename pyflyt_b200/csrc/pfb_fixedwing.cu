@@ -61,18 +61,7 @@ __global__ void __launch_bounds__(kBlock, kMinBlocks)
   fixedwing_store(st, ist, N, i, s);
 }
 
-// k_fw_aviary_step with drone i in flight mode modes[i] (pfb_set_modes): only the command mapping branches on the mode
-template <bool FULL, bool CONTACT, typename NoiseFn>
-__device__ __forceinline__ void fixedwing_aviary_step_any(const FixedwingParams& p, FixedwingRegs& s, int mode, NoiseFn& noise) {
-  s.flags &= ~(uint32_t)FLAG_CONTACT_ARRAY;
-  noise.begin_step();
-  float cmd[6];
-  if (mode == -1) fixedwing_command<-1>(s, cmd);
-  else fixedwing_command<0>(s, cmd);
-#pragma unroll 1
-  for (int u = 0; u < p.ratio; ++u) fixedwing_substep<FULL, CONTACT>(p, s, cmd, noise.get(u));
-}
-
+// k_fw_aviary_step with drone i in flight mode modes[i] (pfb_set_modes; step body fixedwing_aviary_step_any)
 template <bool INJECT, bool CONTACT>
 __global__ void __launch_bounds__(kBlock, kMinBlocks)
     k_fw_aviary_step_modes(const __grid_constant__ FixedwingParams p, const __grid_constant__ RngParams rng, float* __restrict__ st,

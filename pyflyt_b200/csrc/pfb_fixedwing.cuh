@@ -472,6 +472,17 @@ PFB_HD void fixedwing_aviary_step(const FixedwingParams& p, FixedwingRegs& s, No
 #pragma unroll 1
   for (int u = 0; u < p.ratio; ++u) fixedwing_substep<FULL, CONTACT>(p, s, cmd, noise.get(u));
 }
+// fixedwing_aviary_step with the flight mode a run-time value (one mode per drone): only the command mapping branches on it
+template <bool FULL, bool CONTACT, typename NoiseFn>
+PFB_HD void fixedwing_aviary_step_any(const FixedwingParams& p, FixedwingRegs& s, int mode, NoiseFn& noise) {
+  s.flags &= ~(uint32_t)FLAG_CONTACT_ARRAY;
+  noise.begin_step();
+  float cmd[6];
+  if (mode == -1) fixedwing_command<-1>(s, cmd);
+  else fixedwing_command<0>(s, cmd);
+#pragma unroll 1
+  for (int u = 0; u < p.ratio; ++u) fixedwing_substep<FULL, CONTACT>(p, s, cmd, noise.get(u));
+}
 // launch-uniform test for the FULL instantiation
 PFB_HD bool fixedwing_full_model(const FixedwingParams& p) { return p.n_surfaces == kMaxSurfaces && p.wind.kind == 0; }
 

@@ -193,6 +193,7 @@ int pfb_create(const PfbModel* model, const PfbEnvConfig* env, int64_t n_envs, i
 int pfb_destroy(PfbHandle h) {
   if (!h) return 0;
   cudaSetDevice(h->device);
+  mx_destroy(h);
   if (h->d_spare) {
     if (h->side) {
       cudaStreamSynchronize(h->side);
@@ -230,23 +231,27 @@ static inline bool is_rk(PfbHandle h) { return h->model.kind == PFB_KIND_ROCKET;
 static inline bool is_qwp(PfbHandle h) { return h->model.kind == PFB_KIND_QUADX && h->env.env_kind == PFB_ENV_QUADX_WAYPOINTS; }
 static inline bool is_ma(PfbHandle h) { return h->model.kind == PFB_KIND_QUADX && h->env.env_kind == PFB_ENV_MA_QUADX_HOVER; }
 static inline bool is_df(PfbHandle h) { return h->model.kind == PFB_KIND_FIXEDWING && h->env.env_kind == PFB_ENV_DOGFIGHT; }
-int pfb_state_rows(PfbHandle h) { return is_rk(h) ? rk_state_rows() : (is_fw(h) ? fw_state_rows() : (is_qwp(h) ? qwp_state_rows() : qx_rows(h))); }
-int pfb_state_layout(PfbHandle h) { return h && qx_tiled(h) ? PFB_LAYOUT_WARP_TILED : PFB_LAYOUT_FIELD_MAJOR; }
+// A mixed-kind handle (pfb_create_mixed) carves its state buffer by kind: rows of the widest kind present, PFB_LAYOUT_BY_KIND,
+// setpoints and aux of the widest kind (rocket), and its obs buffer receives the hi / lo position words of pfb_observe_state
+int pfb_state_rows(PfbHandle h) { if (h && h->mixed) return mx_state_rows(h); return is_rk(h) ? rk_state_rows() : (is_fw(h) ? fw_state_rows() : (is_qwp(h) ? qwp_state_rows() : qx_rows(h))); }
+int pfb_state_layout(PfbHandle h) { if (h && h->mixed) return PFB_LAYOUT_BY_KIND; return h && qx_tiled(h) ? PFB_LAYOUT_WARP_TILED : PFB_LAYOUT_FIELD_MAJOR; }
 int64_t pfb_state_floats(PfbHandle h) {
   if (!h) return 0;
+  if (h->mixed) return mx_state_floats(h);
   if (qx_tiled(h)) return ((h->n + kTileLanes - 1) / kTileLanes) * qx_tile_floats(qx_rows(h));  // padded to whole tiles
   return (int64_t)pfb_state_rows(h) * h->n;
 }
-int pfb_istate_rows(PfbHandle h) { return is_rk(h) ? rk_istate_rows() : (is_fw(h) ? fw_istate_rows() : (is_qwp(h) ? qwp_istate_rows() : QI_ROWS)); }
-int pfb_setpoint_dim(PfbHandle h) { return is_rk(h) ? 7 : ((is_fw(h) && h->env.env_kind == PFB_ENV_NONE) ? 6 : 4); }
-int pfb_obs_dim(PfbHandle h) { return is_df(h) ? df_obs_dim(h) : is_rk(h) ? rk_obs_dim(h) : (is_fw(h) ? fw_obs_dim(h) : (is_qwp(h) ? qwp_obs_dim(h) : (h->hover.angle_representation == 0 ? 20 : 21) + (is_ma(h) ? 3 : 0))); }
-int pfb_aux_dim(PfbHandle h) { return is_rk(h) ? 9 : (is_fw(h) ? 6 : 4); }
+int pfb_istate_rows(PfbHandle h) { if (h && h->mixed) return mx_istate_rows(h); return is_rk(h) ? rk_istate_rows() : (is_fw(h) ? fw_istate_rows() : (is_qwp(h) ? qwp_istate_rows() : QI_ROWS)); }
+int pfb_setpoint_dim(PfbHandle h) { if (h && h->mixed) return 7; return is_rk(h) ? 7 : ((is_fw(h) && h->env.env_kind == PFB_ENV_NONE) ? 6 : 4); }
+int pfb_obs_dim(PfbHandle h) { if (h && h->mixed) return 6; return is_df(h) ? df_obs_dim(h) : is_rk(h) ? rk_obs_dim(h) : (is_fw(h) ? fw_obs_dim(h) : (is_qwp(h) ? qwp_obs_dim(h) : (h->hover.angle_representation == 0 ? 20 : 21) + (is_ma(h) ? 3 : 0))); }
+int pfb_aux_dim(PfbHandle h) { if (h && h->mixed) return 9; return is_rk(h) ? 9 : (is_fw(h) ? 6 : 4); }
 
 int pfb_bind(PfbHandle h, const PfbBuffers* b) {
   if (!h || !b) return fail("pfb_bind: null argument");
   if (!b->state || !b->istate || !b->setpoint || !b->start_pos || !b->start_orn)
     return fail("pfb_bind: state, istate, setpoint, start_pos and start_orn are mandatory");
   if (((uintptr_t)b->setpoint & 15) || ((uintptr_t)b->state & 15)) return fail("pfb_bind: buffers must be 16-byte aligned");
+  if (h->mixed && mx_bind(h, b)) return -1;
   h->buf = *b;
   h->bound = true;
   return 0;
@@ -262,6 +267,7 @@ int pfb_reset(PfbHandle h, const uint8_t* mask, void* stream) {
   if (h) h->fused_ready = 0;
   REQUIRE_BOUND(h);
   cudaStream_t s = (cudaStream_t)stream;
+  if (h->mixed) return mx_reset(h, mask, s);
   if (is_fw(h)) return fw_reset(h, mask, s);
   if (is_rk(h)) return rk_reset(h, mask, s);
   return qx_reset(h, mask, s);
@@ -270,6 +276,7 @@ int pfb_reset(PfbHandle h, const uint8_t* mask, void* stream) {
 int pfb_set_mode(PfbHandle h, int mode, void* stream) {
   REQUIRE_BOUND(h);
   cudaStream_t s = (cudaStream_t)stream;
+  if (h->mixed) return mx_set_mode(h, mode, s);
   if (is_fw(h)) return fw_set_mode(h, mode, s);
   if (is_rk(h)) return rk_set_mode(h, mode, s);
   return qx_set_mode(h, mode, s);
@@ -280,6 +287,7 @@ int pfb_set_modes(PfbHandle h, const int8_t* modes, void* stream) {
   if (h->env.env_kind != PFB_ENV_NONE)
     return fail("pfb_set_modes: only Aviary handles fly one flight mode per drone; a handle with an env epilogue flies its env's flight_mode");
   REQUIRE_BOUND(h);
+  if (h->mixed) return mx_set_modes(h, modes, (cudaStream_t)stream);
   const int lo = is_rk(h) ? 0 : -1, hi = is_rk(h) || is_fw(h) ? 0 : 7;  // quadx.py:259-262, fixedwing.py:216-219, rocket: mode 0 only
   bool uniform = true;
   for (int64_t i = 0; i < h->n; ++i) {
@@ -304,6 +312,7 @@ int pfb_aviary_step(PfbHandle h, int n_steps, const float* noise, void* stream) 
   REQUIRE_BOUND(h);
   if (n_steps <= 0) return fail("n_steps must be positive");
   cudaStream_t s = (cudaStream_t)stream;
+  if (h->mixed) return mx_aviary_step(h, n_steps, noise, s);
   if (is_fw(h)) return fw_aviary_step(h, n_steps, noise, s);
   if (is_rk(h)) return rk_aviary_step(h, n_steps, noise, s);
   return qx_aviary_step(h, n_steps, noise, s);
@@ -312,18 +321,21 @@ int pfb_aviary_step(PfbHandle h, int n_steps, const float* noise, void* stream) 
 int pfb_set_base_velocity(PfbHandle h, const float* lin_vel, const float* ang_vel, void* stream) {
   REQUIRE_BOUND(h);
   if (!lin_vel || !ang_vel) return fail("pfb_set_base_velocity: null argument");
+  if (h->mixed) return fail("pfb_set_base_velocity is not available on a mixed-kind handle");
   if (is_rk(h)) return rk_set_velocity(h, lin_vel, ang_vel, (cudaStream_t)stream);
   return fail("pfb_set_base_velocity is only built for the rocket (the one vehicle whose env calls resetBaseVelocity)");
 }
 
 int pfb_observe_state(PfbHandle h, void* stream) {
   REQUIRE_BOUND(h);
+  if (h->mixed) return mx_observe(h, (cudaStream_t)stream);
   if (is_fw(h)) return fw_observe(h, (cudaStream_t)stream);
   if (is_rk(h)) return rk_observe(h, (cudaStream_t)stream);
   return qx_observe(h, (cudaStream_t)stream);
 }
 
 static int require_env(PfbHandle h) {
+  if (h->mixed) return fail("a mixed-kind handle is an Aviary handle: the env entry points fly one vehicle kind");
   if (h->env.env_kind == PFB_ENV_NONE) return fail("handle was created without an env epilogue");
   if (!h->buf.obs || !h->buf.reward || !h->buf.term || !h->buf.trunc) return fail("obs/reward/term/trunc buffers are not bound");
   return 0;
@@ -360,6 +372,7 @@ int pfb_set_wind(PfbHandle h, const PfbWind* wind) {
     if (wind->kind == PFB_WIND_LOG && !(wind->z0 > 0.0 && wind->z0 < wind->z_ref)) return fail("log wind profile needs 0 < z0 < z_ref");
     if (wind->kind == PFB_WIND_POWER && !(wind->alpha >= 0.0)) return fail("power-law wind profile needs alpha >= 0, got %g", wind->alpha);
   }
+  if (h->mixed) return mx_set_wind(h, wind);
   WindParams w;
   pfb_narrow_wind(wind, w);
   if (h->d_spare && memcmp(&w, &h->qx.wind, sizeof(w)) != 0) {
@@ -388,6 +401,7 @@ int pfb_set_wind(PfbHandle h, const PfbWind* wind) {
 
 int pfb_set_models(PfbHandle h, const PfbModel* models, int k, const uint8_t* index_host) {
   if (!h || !models || !index_host) return fail("pfb_set_models: null argument");
+  if (h->mixed) return fail("pfb_set_models: a mixed-kind handle takes its models at pfb_create_mixed");
   if (h->model.kind != PFB_KIND_QUADX) return fail("pfb_set_models: only QuadX handles fly several vehicle models");
   if (is_ma(h)) return fail("pfb_set_models: MAQuadXHover handles fly one vehicle model");
   if (k < 1 || k > PFB_MAX_QUADX_MODELS) return fail("pfb_set_models: k = %d, must be in 1..%d", k, PFB_MAX_QUADX_MODELS);
@@ -449,6 +463,7 @@ int pfb_reseed(PfbHandle h, uint64_t seed, void* stream) {
   if (!h) return fail("null handle");
   CUDA_OK(cudaSetDevice(h->device));
   cudaStream_t s = (cudaStream_t)stream;
+  if (h->mixed) return mx_reseed(h, seed, s);
   if (h->side) CUDA_OK(cudaStreamSynchronize(h->side));  // no spare rebuild of the old streams may still be in flight
   h->rng.k0 = (uint32_t)seed;
   h->rng.k1 = (uint32_t)(seed >> 32);
@@ -602,7 +617,7 @@ int pfb_dogfight_split_step(PfbHandle h, const float* actions, const uint64_t* p
   return 0;
 }
 
-int64_t pfb_launch_count(PfbHandle h) { return h ? h->launches : 0; }
+int64_t pfb_launch_count(PfbHandle h) { return h ? h->launches + (h->mixed ? mx_launches(h) : 0) : 0; }
 
 int pfb_profile_begin(PfbHandle h, int capacity) {
   if (!h) return fail("null handle");

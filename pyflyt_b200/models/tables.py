@@ -417,6 +417,43 @@ def build_model_set(kind: str, drone_options, physics_hz: int, n: int) -> tuple[
     return tables, remap[index].astype(np.uint8)
 
 
+KINDS = ("quadx", "fixedwing", "rocket")  # PFB_KIND_QUADX, PFB_KIND_FIXEDWING, PFB_KIND_ROCKET
+
+
+def build_mixed_model_set(kinds, drone_options, physics_hz: int, n: int) -> tuple[list[PfbModel], np.ndarray]:
+    """Per-drone vehicle tables for ``n`` drones of several kinds: ``kinds[i]`` is drone ``i``'s ``drone_type``.
+
+    ``drone_options`` is what the reference's ``Aviary`` takes: ``None`` or one dict for every drone, or a sequence of ``n``
+    dicts, one per drone.  The sub-sequence of each kind goes through ``build_model_set`` (so each kind keeps its limits: up to
+    ``MAX_QUADX_MODELS`` QuadX tables, one fixed-wing and one rocket table).  Returns ``(tables, index)``: the QuadX tables,
+    then the fixed-wing table, then the rocket table (those present), and a uint8 array ``[n]``, drone ``i`` flies
+    ``tables[index[i]]``.  Every drone must run at the same ``control_hz`` (one launch steps them all with one substep count)."""
+    kinds = list(kinds)
+    if len(kinds) != n:
+        raise ModelSetError(f"If multiple `drone_types` are used, must have same number of `drone_types` ({len(kinds)}) as number of drones ({n}).")
+    per_drone = not (drone_options is None or isinstance(drone_options, dict))
+    if per_drone:
+        seq = list(drone_options)
+        if len(seq) != n:  # aviary.py:150-153
+            raise ModelSetError(
+                f"If multiple `drone_options` ({len(seq)}) are used, must have same number of `drone_options` as number of drones ({n})."
+            )
+    tables: list[PfbModel] = []
+    index = np.zeros(n, dtype=np.int64)
+    for kind in KINDS:
+        ids = [i for i, k in enumerate(kinds) if k == kind]
+        if not ids:
+            continue
+        opts = [seq[i] for i in ids] if per_drone else drone_options
+        t, idx = build_model_set(kind, opts, physics_hz, len(ids))
+        index[ids] = idx.astype(np.int64) + len(tables)
+        tables.extend(t)
+    rates = sorted({float(m.control_hz) for m in tables})
+    if len(rates) > 1:
+        raise ModelSetError(f"every drone of a batch needs the same control_hz (one substep ratio per batch); got {[int(r) for r in rates]}.")
+    return tables, index.astype(np.uint8)
+
+
 def model_from_files(kind: str, urdf_path: str, yaml_path: str, physics_hz: int = 240, control_hz: int = 120, **options) -> PfbModel:
     """The same table built INSIDE the C-ABI (``pfb_model_from_files``, pyflyt_b200/csrc/pfb_model_files.cu) from a
     ``<model>.urdf`` + ``<model>.yaml`` pair in the reference's layout (base_drone.py:104-110): what a non-Python caller uses.

@@ -264,6 +264,122 @@ def mixed_mode_fixtures():
     fly_mixed_modes("mixed_modes_fixedwing", "fixedwing", fw_opts, fw_pos, fw_orn, {0: fw_modes}, fw_sp, 200, seed=97)
 
 
+def _padded_rows(rows, w):
+    rows = [np.atleast_1d(np.asarray(r, dtype=np.float64)) for r in rows]
+    return np.array([np.concatenate([r, np.zeros(w - len(r))]) for r in rows])
+
+
+def fly_mixed_kinds(name, drone_type, drone_options, start_pos, start_orn, mode_calls, setpoint_fn, n_steps, seed):
+    """Aviary-level flight of QuadX, fixed-wing and rocket drones in ONE reference Aviary (``drone_type`` a list,
+    aviary.py:139-190, as examples/core/08_mixed_drones.py does): ``mode_calls`` = {step_index: [n] modes}, each applied with
+    ``Aviary.set_mode(list)`` before that step; ``setpoint_fn(step, modes)`` returns None or a list of ``n`` per-drone
+    setpoints of each drone's own length, applied with ``set_all_setpoints`` (aviary.py:470-478 indexes ``setpoints[i]``).
+    Every drone draws one normal per physics step (its motors or its booster), in drone order, so the recorded draws are
+    [step][substep][drone].  Setpoints are stored padded to 7 columns, aux states to 9."""
+    n = len(drone_type)
+    rng = ril.ScriptedNoise(seed)
+    env = Aviary(
+        start_pos=np.array(start_pos, dtype=np.float64),
+        start_orn=np.array(start_orn, dtype=np.float64),
+        drone_type=list(drone_type),
+        drone_options=[dict(d) for d in drone_options],
+        np_random=rng,
+    )
+    states, auxs, contacts, sps, sp_after = [], [], [], [], []
+    modes = None
+    for i in range(n_steps):
+        if i in mode_calls:
+            modes = [int(m) for m in mode_calls[i]]
+            env.set_mode(modes)
+            sp_after.append(_padded_rows([d.setpoint for d in env.drones], 7))
+        sp = setpoint_fn(i, modes)
+        if sp is not None:
+            env.set_all_setpoints([np.array(r, dtype=np.float64) for r in sp])
+        sps.append(_padded_rows([d.setpoint for d in env.drones], 7))
+        env.step()
+        states.append(np.array([d.state for d in env.drones]))
+        auxs.append(_padded_rows([d.aux_state for d in env.drones], 9))
+        contacts.append(np.array([bool(env.contact_array[env.planeId, d.Id]) for d in env.drones]))
+    # one reference world: any floor contact would remove every QuadX's rotational drag (quadx.py:508-510), a coupling that
+    # separate worlds cannot have
+    assert not np.any(contacts), f"{name}: a drone touched the floor"
+    steps = sorted(mode_calls)
+    T = n_steps
+    noise = np.array(rng.normal_log)
+    assert noise.size == T * int(env.updates_per_step) * n, (noise.size, T, n)
+    np.savez_compressed(
+        os.path.join(OUT, f"{name}.npz"),
+        kind="mixed_kinds",
+        drone_type=json.dumps(list(drone_type)),
+        n_drones=n,
+        drone_options=json.dumps(drone_options),
+        start_pos=np.array(start_pos, dtype=np.float64),
+        start_orn=np.array(start_orn, dtype=np.float64),
+        mode_steps=np.array(steps),
+        modes=np.array([mode_calls[k] for k in steps], dtype=np.int64),
+        setpoint_after_set_mode=np.array(sp_after),
+        setpoints=np.array(sps),
+        noise=noise,
+        state=np.array(states),
+        aux=np.array(auxs),
+        contact=np.array(contacts),
+    )
+    print(name, "final z", np.array(states[-1])[:, 3, 2], "draws", noise.size)
+
+
+def mixed_kind_fixtures():
+    """Rockets, QuadX and fixed-wing drones in one Aviary (the reference's tests/test_core.py::test_mixed_drones with more drones
+    and commands).  Rockets upright (roll pi / 2), ignited, with finlet, throttle and gimbal commands; QuadX cf2x and
+    primitive_drone in modes 0 and 7; fixed-wing in modes 0 and -1, all re-assigned by a second set_mode(list) at step 150.
+    1: the kinds grouped; 2: interleaved r, q, f, q, r, f, ...  No drone touches the floor."""
+    qx_opts = [dict(drone_model="cf2x"), dict(drone_model="primitive_drone")]
+
+    def scenario(name, kinds, seed):
+        n = len(kinds)
+        opts, first, second = [], [], []
+        nq = nf = 0
+        for k in kinds:
+            if k == "quadx":
+                opts.append(dict(qx_opts[nq % 2]))
+                first.append(0 if (nq // 2) % 2 == 0 else 7)
+                nq += 1
+            elif k == "fixedwing":
+                opts.append(dict(drone_model="fixedwing"))
+                first.append(0 if nf % 2 == 0 else -1)
+                nf += 1
+            else:
+                opts.append(dict(drone_model="rocket"))
+                first.append(0)
+        second = [{0: 7, 7: 0, -1: 0}.get(m, m) if k != "rocket" else 0 for k, m in zip(kinds, first)]
+        second = [(-1 if m == 0 else 0) if k == "fixedwing" else m for k, m in zip(kinds, second)]
+        pos = np.array([[12.0 * d, 0.0, {"quadx": 40.0, "fixedwing": 80.0, "rocket": 60.0}[k] + 0.5 * d] for d, k in enumerate(kinds)])
+        orn = [[np.pi / 2, 0.0, 0.2 * (d % 3)] if k == "rocket" else [0.05 * (d % 3), -0.04 * (d % 2), 0.3 * (d % 5)] for d, k in enumerate(kinds)]
+        r = np.random.default_rng(seed)
+
+        def sp_fn(i, modes):
+            if i % 50 != 10:
+                return None
+            out = []
+            for d, (k, m) in enumerate(zip(kinds, modes)):
+                if k == "rocket":
+                    out.append(np.concatenate([r.uniform(-0.5, 0.5, 3), [1.0, r.uniform(0.3, 0.8)], r.uniform(-0.3, 0.3, 2)]))
+                elif k == "fixedwing":
+                    if m == -1:
+                        out.append(np.concatenate([r.uniform(-0.6, 0.6, 5), r.uniform(0.3, 1.0, 1)]))
+                    else:
+                        out.append(np.concatenate([r.uniform(-0.5, 0.5, 3), r.uniform(0.3, 1.0, 1)]))
+                elif m == 7:
+                    out.append(np.array([pos[d, 0] + r.uniform(-1, 1), pos[d, 1] + r.uniform(-1, 1), r.uniform(-0.8, 0.8), pos[d, 2] + r.uniform(-1, 1)]))
+                else:
+                    out.append(np.concatenate([r.uniform(-0.3, 0.3, 3), r.uniform(0.3, 0.45, 1)]))
+            return out
+
+        fly_mixed_kinds(name, kinds, opts, pos.tolist(), orn, {0: first, 150: second}, sp_fn, 300, seed=seed)
+
+    scenario("mixed_kinds_grouped", ["rocket"] * 2 + ["quadx"] * 4 + ["fixedwing"] * 2, 101)
+    scenario("mixed_kinds_interleaved", ["rocket", "quadx", "fixedwing", "quadx", "rocket", "fixedwing", "quadx", "fixedwing", "rocket", "quadx"], 102)
+
+
 def wind_fields(wind):
     """npz entries describing an AnalyticWind (absent = still air)"""
     if wind is None:
@@ -918,3 +1034,5 @@ if __name__ == "__main__":
         mixed_mode_fixtures()
     if which in ("all", "ground"):
         ground_fixtures()
+    if which in ("all", "mixedkinds"):
+        mixed_kind_fixtures()
