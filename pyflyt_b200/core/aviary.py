@@ -156,7 +156,7 @@ class BatchedAviary:
         L = _lib.lib()
         self._h = C.c_void_p()
         dev_index = self.device.index if self.device.index is not None else torch.cuda.current_device()
-        if kinds is not None:  # drone i flies models[index[i]], each kind its own sub-batch inside the handle
+        if kinds is not None:  # drone i flies models[index[i]], each kind in its own region of the state buffer
             tables = (PfbModel * len(models))(*models)
             idx = np.ascontiguousarray(index, dtype=np.uint8)
             _lib.check(L.pfb_create_mixed(tables, len(models), idx.ctypes.data_as(C.c_void_p), self.num_drones,
@@ -240,52 +240,29 @@ class BatchedAviary:
 
         A list whose entries differ flies each drone in its own mode until the next ``set_mode(int)`` or ``reset()`` (Aviary
         handles only; an env flies its ``flight_mode``).  Drones ``32 k .. 32 k + 31`` share one warp: a batch steps fastest
-        when each such tile flies one mode (DESIGN.md §4b)."""
-        if self.kinds is not None:
-            self._set_mode_mixed(flight_modes)
-            return
-        lo, hi = (-1, 7) if self.drone_type == "quadx" else ((-1, 0) if self.drone_type == "fixedwing" else (0, 0))
+        when each such tile flies one mode (DESIGN.md §4b).
 
-        def check_range(mode: int) -> None:
-            if mode < lo or mode > hi:
-                # quadx.py:259-262, fixedwing.py:216-219, base_drone.py:252-255
-                raise ValueError(f"`mode` must be between {lo} and {hi} or be registered in self.registered_controllers.keys()=dict_keys([]), got {mode}.")
-
+        Every drone's mode is checked against its own kind's range first, and the first invalid one raises its kind's
+        ``ValueError`` with nothing changed.  (On a batch of several kinds the reference's loop, aviary.py:454-458, would already
+        have set the mode of the drones before that one.)"""
+        kinds = self.kinds if self.kinds is not None else [self.drone_type] * self.num_drones
         if isinstance(flight_modes, (list, tuple)):
             if len(flight_modes) != self.num_drones:
                 raise AssertionError(f"Expected {self.num_drones} flight_modes, got {len(flight_modes)}.")
             modes = [int(m) for m in flight_modes]
-            for m in modes:  # every drone's set_mode checks its own mode (aviary.py:455-456)
-                check_range(m)
-            if len(set(modes)) != 1:
+            for kind, m in zip(kinds, modes):  # every drone's set_mode checks its own mode (aviary.py:455-456)
+                _check_mode(kind, m)
+            # one mode on a single-kind batch: the uniform kernels; a batch of several kinds keeps one mode per drone
+            if self.kinds is not None or len(set(modes)) != 1:
                 arr = np.ascontiguousarray(modes, dtype=np.int8)
                 _lib.check(_lib.lib().pfb_set_modes(self._h, arr.ctypes.data_as(C.c_void_p), self._s()))
                 self._state_fresh = False
                 return
             flight_modes = modes[0]
         mode = int(flight_modes)
-        check_range(mode)
+        for kind in dict.fromkeys(kinds):  # the kinds in drone order: the first drone that refuses raises
+            _check_mode(kind, mode)
         _lib.check(_lib.lib().pfb_set_mode(self._h, mode, self._s()))
-        self._state_fresh = False
-
-    def _set_mode_mixed(self, flight_modes) -> None:
-        """``set_mode`` of a batch of several kinds.  Every drone's mode is checked against its own kind's range first, and the
-        first invalid one raises its kind's ``ValueError`` with nothing changed.  (The reference's loop, aviary.py:454-458, would
-        already have set the mode of the drones before that one.)"""
-        n = self.num_drones
-        if isinstance(flight_modes, (list, tuple)):
-            if len(flight_modes) != n:
-                raise AssertionError(f"Expected {n} flight_modes, got {len(flight_modes)}.")
-            modes = [int(m) for m in flight_modes]
-        else:
-            modes = [int(flight_modes)] * n
-        for kind, m in zip(self.kinds, modes):
-            _check_mode(kind, m)
-        if isinstance(flight_modes, (list, tuple)):
-            arr = np.ascontiguousarray(modes, dtype=np.int8)
-            _lib.check(_lib.lib().pfb_set_modes(self._h, arr.ctypes.data_as(C.c_void_p), self._s()))
-        else:
-            _lib.check(_lib.lib().pfb_set_mode(self._h, modes[0], self._s()))
         self._state_fresh = False
 
     def _setpoint_row(self, index: int, setpoint) -> torch.Tensor:

@@ -5,6 +5,8 @@
 #include <cuda_runtime.h>
 
 #include <cstdint>
+#include <cstring>
+#include <new>
 #include <type_traits>
 
 #include "../../include/pyflyt_b200.h"
@@ -94,9 +96,45 @@ struct PfbContext {
   uint8_t* d_model_index;
   // one flight mode per drone (pfb_set_modes; Aviary handles): device [whole tiles * 32], valid while mode == kModePerDrone
   int8_t* d_modes;
-  // mixed-kind Aviary handle (pfb_create_mixed, pfb_mixed.cu): one sub-handle per vehicle kind; nullptr = one kind
+  // mixed-kind Aviary handle (pfb_create_mixed, pfb_mixed.cu): the drones of each kind and their slots; nullptr = one kind
   struct MixedKinds* mixed;
 };
+
+// The device lookup, then a zeroed handle for n drones / envs on `device` with its Philox key and counters, which `setup(c)`
+// completes (0 or the result of fail()).  On every failure path everything allocated is freed and *out is left alone.
+template <class Setup>
+int pfb_new_context(int64_t n, int device, uint64_t seed, PfbContext** out, Setup&& setup) {
+  int count = 0;
+  cudaError_t e = cudaGetDeviceCount(&count);
+  if (e != cudaSuccess || count == 0)
+    return fail("no CUDA device: libpyflyt_b200 has no CPU fallback (%s)", e != cudaSuccess ? cudaGetErrorString(e) : "0 devices");
+  if (device < 0 || device >= count) return fail("device %d out of range (have %d)", device, count);
+  CUDA_OK(cudaSetDevice(device));
+  cudaDeviceProp prop;
+  CUDA_OK(cudaGetDeviceProperties(&prop, device));
+  PfbContext* c = new (std::nothrow) PfbContext();
+  if (!c) return fail("out of host memory");
+  memset(c, 0, sizeof(*c));
+  c->n = n;
+  c->device = device;
+  c->sm_count = prop.multiProcessorCount;
+  c->rng.k0 = (uint32_t)seed;
+  c->rng.k1 = (uint32_t)(seed >> 32);
+  e = cudaMalloc(&c->d_counters, 8 * sizeof(int32_t));  // [0..3] rotating autoreset counters, [4] ticket of the split dogfight
+  if (e == cudaSuccess) e = cudaMemset(c->d_counters, 0, 8 * sizeof(int32_t));
+  const int rc = e != cudaSuccess ? fail("allocating the counters failed: %s", cudaGetErrorString(e)) : setup(c);
+  if (rc) {
+    pfb_destroy(c);
+    return -1;
+  }
+  *out = c;
+  return 0;
+}
+
+// pfb_lib.cu: the coefficient tables of k QuadX models that one handle flies (one substep ratio, dt and motor count), and
+// their installation as the handle's model set with its current wind and the per-drone index (n entries, padded to whole tiles)
+int pfb_quadx_tables(const PfbModel* models, int k, pfb::QuadXParams* tables);
+int pfb_install_quadx_set(PfbContext* h, const pfb::QuadXParams* tables, int k, const uint8_t* index_host, int64_t n);
 
 // PfbContext::mode of an Aviary handle whose drones fly the modes in d_modes; pfb_set_mode and a full pfb_reset replace it
 constexpr int kModePerDrone = 0x100;
@@ -176,6 +214,11 @@ static inline StepPlan plan_step(PfbContext* h) {
 // pfb_lib.cu: a masked user reset on an autoreset handle removes the masked envs / arenas from the pending done list
 int pfb_drop_masked_done(PfbContext* h, const uint8_t* mask, cudaStream_t s);
 
+// The flight modes each vehicle kind flies, by PFB_KIND_*: QuadX -1..7 (quadx.py:259-262), fixed-wing -1..0 (fixedwing.py:216-219),
+// rocket 0 only (base_drone.py:252-255)
+constexpr int kModeLo[3] = {-1, -1, 0};
+constexpr int kModeHi[3] = {7, 0, 0};
+
 // Runs BODY with `constexpr int MODE` = the QuadX flight mode `mode`
 #define PFB_MODE_SWITCH(mode, BODY)                         \
   switch (mode) {                                           \
@@ -188,7 +231,7 @@ int pfb_drop_masked_done(PfbContext* h, const uint8_t* mask, cudaStream_t s);
     case 5: { constexpr int MODE = 5; BODY; } break;        \
     case 6: { constexpr int MODE = 6; BODY; } break;        \
     case 7: { constexpr int MODE = 7; BODY; } break;        \
-    default: return fail("`mode` must be between -1 and 7, got %d", mode); \
+    default: return fail("`mode` must be between %d and %d, got %d", kModeLo[PFB_KIND_QUADX], kModeHi[PFB_KIND_QUADX], mode); \
   }
 
 // ---- host side of the tail-CTA env kinds (pfb_tail_step.cuh): QuadX-Waypoints, Fixedwing-Waypoints, Rocket-Landing, Dogfight ----
@@ -300,7 +343,6 @@ int rk_state_rows();
 int rk_istate_rows();
 int rk_obs_dim(const PfbContext* h);
 int rk_reset(PfbContext* h, const uint8_t* mask, cudaStream_t s);
-int rk_set_mode(PfbContext* h, int mode, cudaStream_t s);
 int rk_set_velocity(PfbContext* h, const float* lin, const float* ang, cudaStream_t s);
 int rk_aviary_step(PfbContext* h, int n_steps, const float* noise, cudaStream_t s);
 int rk_observe(PfbContext* h, cudaStream_t s);
@@ -325,15 +367,11 @@ int df_split_combat(PfbContext* h, const float* table, int64_t first_gid, int64_
 int mx_state_rows(const PfbContext* h);
 int mx_istate_rows(const PfbContext* h);
 int64_t mx_state_floats(const PfbContext* h);
-int mx_bind(PfbContext* h, const PfbBuffers* b);
 int mx_reset(PfbContext* h, const uint8_t* mask, cudaStream_t s);
 int mx_set_mode(PfbContext* h, int mode, cudaStream_t s);
 int mx_set_modes(PfbContext* h, const int8_t* modes, cudaStream_t s);
 int mx_aviary_step(PfbContext* h, int n_steps, const float* noise, cudaStream_t s);
 int mx_observe(PfbContext* h, cudaStream_t s);
-int mx_set_wind(PfbContext* h, const PfbWind* wind);
-int mx_reseed(PfbContext* h, uint64_t seed, cudaStream_t s);
-int64_t mx_launches(const PfbContext* h);  // launches of the sub-handles (their resets and mode changes)
 void mx_destroy(PfbContext* h);
 
 // QuadX-Waypoints translation unit (pfb_quadx_wp.cu)

@@ -4,8 +4,7 @@
 #include <cmath>
 #include <cstring>
 
-#include "pfb_context.h"
-#include "pfb_noise.cuh"
+#include "pfb_aviary.cuh"
 #include "pfb_tail_step.cuh"
 
 using namespace pfb;
@@ -31,11 +30,7 @@ __global__ void __launch_bounds__(kBlock) k_fw_reset(const __grid_constant__ Fix
   int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= N) return;
   if (mask && !mask[i]) return;
-  FixedwingRegs s;
-  fixedwing_reset(p, s, start_pos[3 * i], start_pos[3 * i + 1], start_pos[3 * i + 2], start_orn[3 * i], start_orn[3 * i + 1],
-                  start_orn[3 * i + 2]);
-  fixedwing_store(st, ist, N, i, s);
-  ist[(int64_t)FI_STEP * N + i] = 0;
+  fw_reset_drone(p, st, ist, N, i, start_pos, start_orn, i);
   if (setpoint)  // the caller's buffer is [N][sp_dim]: 6 on the Aviary surface, 4 behind an env
     for (int k = 0; k < sp_dim; ++k) setpoint[(int64_t)sp_dim * i + k] = 0.0f;
 }
@@ -69,18 +64,7 @@ __global__ void __launch_bounds__(kBlock, kMinBlocks)
                            const float* __restrict__ noise, int n_steps, uint32_t seq, int64_t N) {
   int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= N) return;
-  const int mode = modes[i];
-  FixedwingRegs s;
-  fixedwing_load(st, ist, N, i, s);
-#pragma unroll
-  for (int k = 0; k < 6; ++k) s.sp[k] = __ldg(setpoint + (int64_t)6 * i + k);  // Aviary handles: 6-wide setpoints
-  auto nz = make_noise<INJECT>(noise, N, i, rng, seq, TAG_AVIARY, p.noise_loc, p.ratio);
-  if (fixedwing_full_model(p)) {
-    for (int k = 0; k < n_steps; ++k) fixedwing_aviary_step_any<true, CONTACT>(p, s, mode, nz);
-  } else {
-    for (int k = 0; k < n_steps; ++k) fixedwing_aviary_step_any<false, CONTACT>(p, s, mode, nz);
-  }
-  fixedwing_store(st, ist, N, i, s);
+  fw_aviary_step_drone<INJECT, CONTACT, 6>(p, rng, st, ist, N, i, modes, setpoint, noise, N, i, n_steps, seq);  // Aviary handles: 6-wide setpoints
 }
 
 __global__ void __launch_bounds__(kBlock) k_fw_observe(const float* __restrict__ st, const int32_t* __restrict__ ist,
@@ -88,15 +72,13 @@ __global__ void __launch_bounds__(kBlock) k_fw_observe(const float* __restrict__
                                                        uint8_t* __restrict__ contact, int64_t N) {
   int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= N) return;
-  FixedwingRegs s;
-  fixedwing_load(st, ist, N, i, s);
-  float o[12], a[6];
-  fixedwing_drone_state(s, o, a);
+  float o[12], a[6], hi[3], lo[3];
+  const bool c = fw_query_drone(st, ist, N, i, o, a, hi, lo);
   if (drone_state)
     for (int k = 0; k < 12; ++k) drone_state[12 * i + k] = o[k];
   if (aux)
     for (int k = 0; k < 6; ++k) aux[6 * i + k] = a[k];
-  if (contact) contact[i] = (s.flags & FLAG_CONTACT_ARRAY) ? 1 : 0;
+  if (contact) contact[i] = c ? 1 : 0;
 }
 
 // ---------------------------------------------------------------------------------------------------
@@ -374,8 +356,6 @@ int fw_reset(PfbContext* h, const uint8_t* mask, cudaStream_t s) {
 }
 
 int fw_set_mode(PfbContext* h, int mode, cudaStream_t s) {
-  if (mode < -1 || mode > 0)  // fixedwing.py:216-219
-    return fail("`mode` must be between -1 and 0 or be registered in self.registered_controllers.keys()=dict_keys([]), got %d.", mode);
   if (mode == -1 && fw_setpoint_dim(h) < 6) return fail("mode -1 needs the 6-wide setpoint buffer of the Aviary surface");
   CUDA_OK(cudaMemsetAsync(h->buf.setpoint, 0, (size_t)h->n * fw_setpoint_dim(h) * sizeof(float), s));  // fixedwing.py:224-227
   h->mode = mode;

@@ -53,6 +53,42 @@ int pfb_drop_masked_done(PfbContext* h, const uint8_t* mask, cudaStream_t s) {
   return 0;
 }
 
+int pfb_quadx_tables(const PfbModel* models, int k, QuadXParams* tables) {
+  for (int j = 0; j < k; ++j) {
+    const PfbModel& m = models[j];
+    if (m.abi_version != PFB_ABI_VERSION) return fail("pfb_set_models: model %d has ABI %d != library ABI %d", j, m.abi_version, PFB_ABI_VERSION);
+    if (m.kind != PFB_KIND_QUADX) return fail("pfb_set_models: model %d is not a QuadX (kind %d)", j, m.kind);
+    // every kernel runs ONE substep ratio and one dt per handle
+    if (m.physics_hz != models[0].physics_hz || m.control_hz != models[0].control_hz)
+      return fail("pfb_set_models: model %d runs at physics_hz %g / control_hz %g, model 0 at %g / %g: every model of a handle needs the same rates", j,
+                  m.physics_hz, m.control_hz, models[0].physics_hz, models[0].control_hz);
+    memset(&tables[j], 0, sizeof(QuadXParams));
+    if (build_quadx_params(m, tables[j]) != 0) return -1;
+    if (tables[j].ratio != tables[0].ratio || tables[j].dt != tables[0].dt || tables[j].ctrl_dt != tables[0].ctrl_dt ||
+        tables[j].noise_loc != tables[0].noise_loc)
+      return fail("pfb_set_models: model %d has a different substep ratio, dt or motor count than model 0", j);
+  }
+  return 0;
+}
+
+int pfb_install_quadx_set(PfbContext* h, const QuadXParams* tables, int k, const uint8_t* index_host, int64_t n) {
+  if (!h->qxset) {
+    h->qxset = new (std::nothrow) QuadXModelSet();
+    if (!h->qxset) return fail("out of host memory");
+  }
+  memset(h->qxset, 0, sizeof(QuadXModelSet));
+  for (int j = 0; j < k; ++j) {
+    h->qxset->m[j] = tables[j];
+    h->qxset->m[j].wind = h->qx.wind;
+  }
+  const size_t padded = (size_t)grid_for(n) * kBlock;  // whole tiles: the tile kernels read the index of every lane
+  if (!h->d_model_index) CUDA_OK(cudaMalloc(&h->d_model_index, padded));
+  CUDA_OK(cudaMemset(h->d_model_index, 0, padded));
+  CUDA_OK(cudaMemcpy(h->d_model_index, index_host, (size_t)n, cudaMemcpyHostToDevice));
+  h->qxset->index = h->d_model_index;
+  return 0;
+}
+
 // ---------------------------------------------------------------------------------------------------
 // host side
 // ---------------------------------------------------------------------------------------------------
@@ -64,45 +100,22 @@ int pfb_sizeof_model(void) { return (int)sizeof(PfbModel); }
 int pfb_sizeof_env_config(void) { return (int)sizeof(PfbEnvConfig); }
 int pfb_sizeof_buffers(void) { return (int)sizeof(PfbBuffers); }
 
-int pfb_create(const PfbModel* model, const PfbEnvConfig* env, int64_t n_envs, int device, uint64_t seed, PfbHandle* out) {
-  if (!model || !out) return fail("pfb_create: null argument");
-  if (model->abi_version != PFB_ABI_VERSION) return fail("PfbModel ABI %d != library ABI %d", model->abi_version, PFB_ABI_VERSION);
-  if (n_envs <= 0) return fail("n_envs must be positive");
-  if (env && env->inline_reset != 0 && env->inline_reset != 1) return fail("inline_reset must be 0 or 1, got %d", env->inline_reset);
-  if (model->kind != PFB_KIND_QUADX && model->kind != PFB_KIND_FIXEDWING && model->kind != PFB_KIND_ROCKET)
-    return fail("unknown vehicle kind %d", model->kind);
-  // An Aviary handle (env kind NONE) takes ONE field from its config, contact_response; every other handle parameter is
-  // what env == NULL gives
-  int aviary_contact = 0;
-  if (env && env->env_kind == PFB_ENV_NONE) {
-    aviary_contact = env->contact_response ? 1 : 0;
-    env = nullptr;
-  }
-  int count = 0;
-  cudaError_t e = cudaGetDeviceCount(&count);
-  if (e != cudaSuccess || count == 0)
-    return fail("no CUDA device: libpyflyt_b200 has no CPU fallback (%s)", e != cudaSuccess ? cudaGetErrorString(e) : "0 devices");
-  if (device < 0 || device >= count) return fail("device %d out of range (have %d)", device, count);
-  CUDA_OK(cudaSetDevice(device));
-  PfbContext* c = new (std::nothrow) PfbContext();
-  if (!c) return fail("out of host memory");
-  memset(c, 0, sizeof(*c));
+// The vehicle tables, env parameters and buffers of a single-kind handle on a fresh context (pfb_new_context frees everything if
+// this fails).  `env` = nullptr for an Aviary handle, whose one config field is `aviary_contact`.
+static int single_setup(PfbContext* c, const PfbModel* model, const PfbEnvConfig* env, int aviary_contact) {
+  const int64_t n_envs = c->n;
   c->model = *model;
   if (env) c->env = *env;
   else c->env.contact_response = aviary_contact;
-  c->n = n_envs;
-  c->device = device;
   if (model->kind == PFB_KIND_QUADX) {
-    if (build_quadx_params(*model, c->qx) != 0) { delete c; return -1; }
+    if (build_quadx_params(*model, c->qx) != 0) return -1;
   } else if (model->kind == PFB_KIND_FIXEDWING) {
-    if (fw_build_params(*model, env, c->fw, c->wp) != 0) { delete c; return -1; }
-    if (df_build_params(env, c->df) != 0) { delete c; return -1; }
-    if (env && env->env_kind == PFB_ENV_DOGFIGHT && (n_envs % (2 * env->team_size)) != 0) {
-      delete c;
+    if (fw_build_params(*model, env, c->fw, c->wp) != 0) return -1;
+    if (df_build_params(env, c->df) != 0) return -1;
+    if (env && env->env_kind == PFB_ENV_DOGFIGHT && (n_envs % (2 * env->team_size)) != 0)
       return fail("n_envs (%lld) must be a multiple of the arena size 2*team_size = %d", (long long)n_envs, 2 * env->team_size);
-    }
   } else {
-    if (rk_build_params(*model, env, c->rk, c->land) != 0) { delete c; return -1; }
+    if (rk_build_params(*model, env, c->rk, c->land) != 0) return -1;
     if (aviary_contact) c->rk.contact_response = 1;
   }
   c->hover.env_step_ratio = env ? env->env_step_ratio : 1;
@@ -116,10 +129,8 @@ int pfb_create(const PfbModel* model, const PfbEnvConfig* env, int64_t n_envs, i
     c->hover.dome2 = (float)(dome * dome);
   }
   c->hover.ma = (env && env->env_kind == PFB_ENV_MA_QUADX_HOVER) ? 1 : 0;
-  if (c->hover.ma && env->autoreset) {
-    delete c;
+  if (c->hover.ma && env->autoreset)
     return fail("MAQuadXHover is a per-agent epilogue: arenas are reset by the caller (pfb_env_reset with a mask), autoreset must be 0");
-  }
   if (env && env->env_kind != PFB_ENV_NONE) {
     const bool ok = (model->kind == PFB_KIND_QUADX && env->env_kind == PFB_ENV_QUADX_HOVER) ||
                     (model->kind == PFB_KIND_QUADX && env->env_kind == PFB_ENV_QUADX_WAYPOINTS) ||
@@ -127,16 +138,10 @@ int pfb_create(const PfbModel* model, const PfbEnvConfig* env, int64_t n_envs, i
                     (model->kind == PFB_KIND_FIXEDWING && env->env_kind == PFB_ENV_FIXEDWING_WAYPOINTS) ||
                     (model->kind == PFB_KIND_FIXEDWING && env->env_kind == PFB_ENV_DOGFIGHT) ||
                     (model->kind == PFB_KIND_ROCKET && env->env_kind == PFB_ENV_ROCKET_LANDING);
-    if (!ok) {
-      delete c;
-      return fail("env kind %d is not available for vehicle kind %d in this library", env->env_kind, model->kind);
-    }
+    if (!ok) return fail("env kind %d is not available for vehicle kind %d in this library", env->env_kind, model->kind);
   }
   if (env && env->env_kind == PFB_ENV_QUADX_WAYPOINTS) {
-    if (env->num_targets < 1 || env->num_targets > kMaxTargets) {
-      delete c;
-      return fail("num_targets must be in 1..%d, got %d", kMaxTargets, env->num_targets);
-    }
+    if (env->num_targets < 1 || env->num_targets > kMaxTargets) return fail("num_targets must be in 1..%d, got %d", kMaxTargets, env->num_targets);
     c->qwp.env_step_ratio = env->env_step_ratio;
     c->qwp.max_steps = env->max_steps;
     c->qwp.sparse_reward = env->sparse_reward;
@@ -149,14 +154,6 @@ int pfb_create(const PfbModel* model, const PfbEnvConfig* env, int64_t n_envs, i
     c->qwp.goal_reach_angle = (float)env->goal_reach_angle;
     c->qwp.min_height = 0.1f;  // quadx_waypoints_env.py:88
   }
-  c->rng.k0 = (uint32_t)seed;
-  c->rng.k1 = (uint32_t)(seed >> 32);
-  c->mode = 0;
-  cudaDeviceProp prop;
-  CUDA_OK(cudaGetDeviceProperties(&prop, device));
-  c->sm_count = prop.multiProcessorCount;
-  CUDA_OK(cudaMalloc(&c->d_counters, 8 * sizeof(int32_t)));  // [0..3] rotating autoreset counters, [4] ticket of the split dogfight
-  CUDA_OK(cudaMemset(c->d_counters, 0, 8 * sizeof(int32_t)));
   CUDA_OK(cudaMalloc(&c->d_done_list, 4 * (size_t)n_envs * sizeof(int32_t)));
   if (env && env->autoreset && (env->env_kind == PFB_ENV_QUADX_HOVER || env->env_kind == PFB_ENV_FIXEDWING_WAYPOINTS ||
                                  env->env_kind == PFB_ENV_QUADX_WAYPOINTS || env->env_kind == PFB_ENV_ROCKET_LANDING ||
@@ -186,8 +183,24 @@ int pfb_create(const PfbModel* model, const PfbEnvConfig* env, int64_t n_envs, i
       for (int k = 0; k < 4; ++k) CUDA_OK(cudaEventCreateWithFlags(&c->ev_spare[k], cudaEventDisableTiming));
     }
   }
-  *out = c;
   return 0;
+}
+
+int pfb_create(const PfbModel* model, const PfbEnvConfig* env, int64_t n_envs, int device, uint64_t seed, PfbHandle* out) {
+  if (!model || !out) return fail("pfb_create: null argument");
+  if (model->abi_version != PFB_ABI_VERSION) return fail("PfbModel ABI %d != library ABI %d", model->abi_version, PFB_ABI_VERSION);
+  if (n_envs <= 0) return fail("n_envs must be positive");
+  if (env && env->inline_reset != 0 && env->inline_reset != 1) return fail("inline_reset must be 0 or 1, got %d", env->inline_reset);
+  if (model->kind != PFB_KIND_QUADX && model->kind != PFB_KIND_FIXEDWING && model->kind != PFB_KIND_ROCKET)
+    return fail("unknown vehicle kind %d", model->kind);
+  // An Aviary handle (env kind NONE) takes ONE field from its config, contact_response; every other handle parameter is
+  // what env == NULL gives
+  int aviary_contact = 0;
+  if (env && env->env_kind == PFB_ENV_NONE) {
+    aviary_contact = env->contact_response ? 1 : 0;
+    env = nullptr;
+  }
+  return pfb_new_context(n_envs, device, seed, out, [&](PfbContext* c) { return single_setup(c, model, env, aviary_contact); });
 }
 
 int pfb_destroy(PfbHandle h) {
@@ -198,8 +211,9 @@ int pfb_destroy(PfbHandle h) {
     if (h->side) {
       cudaStreamSynchronize(h->side);
       cudaStreamDestroy(h->side);
-      cudaEventDestroy(h->ev_step);
-      for (int k = 0; k < 4; ++k) cudaEventDestroy(h->ev_spare[k]);
+      if (h->ev_step) cudaEventDestroy(h->ev_step);  // a handle whose creation failed may lack them
+      for (int k = 0; k < 4; ++k)
+        if (h->ev_spare[k]) cudaEventDestroy(h->ev_spare[k]);
     }
     cudaFree(h->d_spare);
     if (h->d_episode) cudaFree(h->d_episode);
@@ -251,7 +265,6 @@ int pfb_bind(PfbHandle h, const PfbBuffers* b) {
   if (!b->state || !b->istate || !b->setpoint || !b->start_pos || !b->start_orn)
     return fail("pfb_bind: state, istate, setpoint, start_pos and start_orn are mandatory");
   if (((uintptr_t)b->setpoint & 15) || ((uintptr_t)b->state & 15)) return fail("pfb_bind: buffers must be 16-byte aligned");
-  if (h->mixed && mx_bind(h, b)) return -1;
   h->buf = *b;
   h->bound = true;
   return 0;
@@ -277,8 +290,18 @@ int pfb_set_mode(PfbHandle h, int mode, void* stream) {
   REQUIRE_BOUND(h);
   cudaStream_t s = (cudaStream_t)stream;
   if (h->mixed) return mx_set_mode(h, mode, s);
+  const int lo = kModeLo[h->model.kind], hi = kModeHi[h->model.kind];
+  if (mode < lo || mode > hi) {  // the messages of quadx.py:259-262, fixedwing.py:216-219, base_drone.py:252-255
+    if (is_rk(h)) return fail("`mode` must be either 0 or be registered in self.registered_controllers.keys()=dict_keys([]), got %d.", mode);
+    if (is_fw(h))
+      return fail("`mode` must be between %d and %d or be registered in self.registered_controllers.keys()=dict_keys([]), got %d.", lo, hi, mode);
+    return fail("`mode` must be between %d and %d, got %d", lo, hi, mode);
+  }
   if (is_fw(h)) return fw_set_mode(h, mode, s);
-  if (is_rk(h)) return rk_set_mode(h, mode, s);
+  if (is_rk(h)) {  // the rocket's one mode: nothing to preset
+    h->mode = 0;
+    return 0;
+  }
   return qx_set_mode(h, mode, s);
 }
 
@@ -288,7 +311,7 @@ int pfb_set_modes(PfbHandle h, const int8_t* modes, void* stream) {
     return fail("pfb_set_modes: only Aviary handles fly one flight mode per drone; a handle with an env epilogue flies its env's flight_mode");
   REQUIRE_BOUND(h);
   if (h->mixed) return mx_set_modes(h, modes, (cudaStream_t)stream);
-  const int lo = is_rk(h) ? 0 : -1, hi = is_rk(h) || is_fw(h) ? 0 : 7;  // quadx.py:259-262, fixedwing.py:216-219, rocket: mode 0 only
+  const int lo = kModeLo[h->model.kind], hi = kModeHi[h->model.kind];
   bool uniform = true;
   for (int64_t i = 0; i < h->n; ++i) {
     if (modes[i] < lo || modes[i] > hi)
@@ -372,7 +395,6 @@ int pfb_set_wind(PfbHandle h, const PfbWind* wind) {
     if (wind->kind == PFB_WIND_LOG && !(wind->z0 > 0.0 && wind->z0 < wind->z_ref)) return fail("log wind profile needs 0 < z0 < z_ref");
     if (wind->kind == PFB_WIND_POWER && !(wind->alpha >= 0.0)) return fail("power-law wind profile needs alpha >= 0, got %g", wind->alpha);
   }
-  if (h->mixed) return mx_set_wind(h, wind);
   WindParams w;
   pfb_narrow_wind(wind, w);
   if (h->d_spare && memcmp(&w, &h->qx.wind, sizeof(w)) != 0) {
@@ -406,20 +428,7 @@ int pfb_set_models(PfbHandle h, const PfbModel* models, int k, const uint8_t* in
   if (is_ma(h)) return fail("pfb_set_models: MAQuadXHover handles fly one vehicle model");
   if (k < 1 || k > PFB_MAX_QUADX_MODELS) return fail("pfb_set_models: k = %d, must be in 1..%d", k, PFB_MAX_QUADX_MODELS);
   QuadXParams tables[PFB_MAX_QUADX_MODELS];
-  for (int j = 0; j < k; ++j) {
-    const PfbModel& m = models[j];
-    if (m.abi_version != PFB_ABI_VERSION) return fail("pfb_set_models: model %d has ABI %d != library ABI %d", j, m.abi_version, PFB_ABI_VERSION);
-    if (m.kind != PFB_KIND_QUADX) return fail("pfb_set_models: model %d is not a QuadX (kind %d)", j, m.kind);
-    // every kernel runs ONE substep ratio and one dt per handle
-    if (m.physics_hz != models[0].physics_hz || m.control_hz != models[0].control_hz)
-      return fail("pfb_set_models: model %d runs at physics_hz %g / control_hz %g, model 0 at %g / %g: every model of a handle needs the same rates", j,
-                  m.physics_hz, m.control_hz, models[0].physics_hz, models[0].control_hz);
-    memset(&tables[j], 0, sizeof(QuadXParams));
-    if (build_quadx_params(m, tables[j]) != 0) return -1;
-    if (tables[j].ratio != tables[0].ratio || tables[j].dt != tables[0].dt || tables[j].ctrl_dt != tables[0].ctrl_dt ||
-        tables[j].noise_loc != tables[0].noise_loc)
-      return fail("pfb_set_models: model %d has a different substep ratio, dt or motor count than model 0", j);
-  }
+  if (pfb_quadx_tables(models, k, tables)) return -1;
   for (int64_t i = 0; i < h->n; ++i)
     if (index_host[i] >= k) return fail("pfb_set_models: index[%lld] = %d, must be < k = %d", (long long)i, (int)index_host[i], k);
   CUDA_OK(cudaSetDevice(h->device));
@@ -442,28 +451,13 @@ int pfb_set_models(PfbHandle h, const PfbModel* models, int k, const uint8_t* in
     h->qxset = nullptr;
     return 0;
   }
-  if (!h->qxset) {
-    h->qxset = new (std::nothrow) QuadXModelSet();
-    if (!h->qxset) return fail("out of host memory");
-  }
-  memset(h->qxset, 0, sizeof(QuadXModelSet));
-  for (int j = 0; j < k; ++j) {
-    h->qxset->m[j] = tables[j];
-    h->qxset->m[j].wind = wind;
-  }
-  const size_t padded = (size_t)grid_for(h->n) * kBlock;  // whole tiles: the tile kernels read the index of every lane
-  if (!h->d_model_index) CUDA_OK(cudaMalloc(&h->d_model_index, padded));
-  CUDA_OK(cudaMemset(h->d_model_index, 0, padded));
-  CUDA_OK(cudaMemcpy(h->d_model_index, index_host, (size_t)h->n, cudaMemcpyHostToDevice));
-  h->qxset->index = h->d_model_index;
-  return 0;
+  return pfb_install_quadx_set(h, tables, k, index_host, h->n);
 }
 
 int pfb_reseed(PfbHandle h, uint64_t seed, void* stream) {
   if (!h) return fail("null handle");
   CUDA_OK(cudaSetDevice(h->device));
   cudaStream_t s = (cudaStream_t)stream;
-  if (h->mixed) return mx_reseed(h, seed, s);
   if (h->side) CUDA_OK(cudaStreamSynchronize(h->side));  // no spare rebuild of the old streams may still be in flight
   h->rng.k0 = (uint32_t)seed;
   h->rng.k1 = (uint32_t)(seed >> 32);
@@ -617,7 +611,7 @@ int pfb_dogfight_split_step(PfbHandle h, const float* actions, const uint64_t* p
   return 0;
 }
 
-int64_t pfb_launch_count(PfbHandle h) { return h ? h->launches + (h->mixed ? mx_launches(h) : 0) : 0; }
+int64_t pfb_launch_count(PfbHandle h) { return h ? h->launches : 0; }
 
 int pfb_profile_begin(PfbHandle h, int capacity) {
   if (!h) return fail("null handle");

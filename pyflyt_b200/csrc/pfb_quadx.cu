@@ -5,37 +5,13 @@
 // The Hover step moves a warp's 32-env state tile and observation tile with one TMA bulk copy each.
 #include <cuda_runtime.h>
 
-#include "pfb_context.h"
-#include "pfb_noise.cuh"
+#include "pfb_aviary.cuh"
 
 using namespace pfb;
 
 // ---------------------------------------------------------------------------------------------------
 // kernels — Aviary surface
 // ---------------------------------------------------------------------------------------------------
-// QuadX handles keep their state WARP-TILED (pfb_quadx.cuh) except QuadX-Waypoints, whose kernels (pfb_quadx_wp.cu) still use
-// the field-major [F][N] rows + istate; TILED selects the addressing of the kernels both layouts share.
-template <int MODE, bool TILED>
-__device__ __forceinline__ void qx_load_any(const float* __restrict__ st, const int32_t* __restrict__ ist, int rows, int64_t N, int64_t i,
-                                            QuadXRegs& s, int& step_count) {
-  if (TILED) {
-    quadx_load_tile<MODE, kTileGroupStride>(st + qx_tile_base(i, rows), s, step_count);
-  } else {
-    quadx_load<MODE>(st, ist, N, i, s);
-    step_count = ist[(int64_t)QI_STEP * N + i];
-  }
-}
-template <int MODE, bool TILED>
-__device__ __forceinline__ void qx_store_any(float* __restrict__ st, int32_t* __restrict__ ist, int rows, int64_t N, int64_t i,
-                                             const QuadXRegs& s, int step_count) {
-  if (TILED) {
-    quadx_store_tile<MODE, kTileGroupStride>(st + qx_tile_base(i, rows), s, step_count);
-  } else {
-    quadx_store<MODE>(st, ist, N, i, s);
-    ist[(int64_t)QI_STEP * N + i] = step_count;
-  }
-}
-
 // Aviary.reset + QuadX.reset + update_state (aviary.py:218-312, quadx.py:222-231)
 template <bool TILED>
 __global__ void __launch_bounds__(kBlock) k_quadx_reset(float* __restrict__ st, int32_t* __restrict__ ist, int rows,
@@ -45,10 +21,7 @@ __global__ void __launch_bounds__(kBlock) k_quadx_reset(float* __restrict__ st, 
   int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= N) return;
   if (mask && !mask[i]) return;
-  QuadXRegs s;
-  quadx_reset(s, start_pos[3 * i + 0], start_pos[3 * i + 1], start_pos[3 * i + 2], start_orn[3 * i + 0],
-              start_orn[3 * i + 1], start_orn[3 * i + 2]);
-  qx_store_any<7, TILED>(st, ist, rows, N, i, s, 0);  // mode 7 touches every PID row
+  qx_reset_drone<TILED>(st, ist, rows, N, i, start_pos, start_orn, i);
   if (setpoint) reinterpret_cast<float4*>(setpoint)[i] = make_float4(0.f, 0.f, 0.f, 0.f);
 }
 
@@ -93,14 +66,7 @@ __global__ void __launch_bounds__(kBlock) k_quadx_set_modes(float* __restrict__ 
                                                             const int8_t* __restrict__ modes, int64_t N) {
   int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= N) return;
-  QuadXRegs s;
-  int step_count;
-  quadx_load_tile<7, kTileGroupStride>(st + qx_tile_base(i, rows), s, step_count);
-  float4 sp = reinterpret_cast<const float4*>(setpoint)[i];
-  s.sp[0] = sp.x; s.sp[1] = sp.y; s.sp[2] = sp.z; s.sp[3] = sp.w;
-  quadx_set_mode_any(s, modes[i]);
-  quadx_store_tile<7, kTileGroupStride>(st + qx_tile_base(i, rows), s, step_count);
-  reinterpret_cast<float4*>(setpoint)[i] = make_float4(s.sp[0], s.sp[1], s.sp[2], s.sp[3]);
+  qx_set_mode_drone<4>(st, rows, i, modes, setpoint, i);
 }
 
 // n_steps x Aviary.step() with drone i in flight mode modes[i].  Every PID row is moved (the mode-7 set); quadx_mask_pid
@@ -112,17 +78,7 @@ __global__ void __launch_bounds__(kBlock, kMinBlocks)
                               int n_steps, uint32_t seq, int64_t N) {
   int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= N) return;
-  const QuadXParams& p = qx_model(ps, i);
-  const int mode = modes[i];
-  QuadXRegs s;
-  int step_count;
-  quadx_load_tile<7, kTileGroupStride>(st + qx_tile_base(i, rows), s, step_count);
-  quadx_mask_pid(s, mode);
-  float4 sp = __ldg(reinterpret_cast<const float4*>(setpoint) + i);
-  s.sp[0] = sp.x; s.sp[1] = sp.y; s.sp[2] = sp.z; s.sp[3] = sp.w;
-  auto nz = make_noise<INJECT>(noise, N, i, rng, seq, TAG_AVIARY, qx_model0(ps).noise_loc, qx_model0(ps).ratio);
-  for (int k = 0; k < n_steps; ++k) quadx_aviary_step_any<CONTACT>(p, s, mode, nz);
-  quadx_store_tile<7, kTileGroupStride>(st + qx_tile_base(i, rows), s, step_count);
+  qx_aviary_step_drone<INJECT, CONTACT, 4>(ps, rng, st, rows, i, modes, setpoint, noise, N, i, n_steps, seq);
 }
 
 // Aviary.state(i) / aux_state(i) / contact_array  -> row-major API buffers
@@ -132,11 +88,8 @@ __global__ void __launch_bounds__(kBlock) k_quadx_observe(const float* __restric
                                                           uint8_t* __restrict__ contact, int64_t N) {
   int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= N) return;
-  QuadXRegs s;
-  int step_count;
-  qx_load_any<-1, TILED>(st, ist, rows, N, i, s, step_count);
-  float o[12], a[4];
-  quadx_drone_state(s, o, a);
+  float o[12], a[4], hi[3], lo[3];
+  const bool c = qx_query_drone<TILED>(st, ist, rows, N, i, o, a, hi, lo);
   if (drone_state) {
     float4* d = reinterpret_cast<float4*>(drone_state + 12 * i);
     d[0] = make_float4(o[0], o[1], o[2], o[3]);
@@ -144,7 +97,7 @@ __global__ void __launch_bounds__(kBlock) k_quadx_observe(const float* __restric
     d[2] = make_float4(o[8], o[9], o[10], o[11]);
   }
   if (aux) reinterpret_cast<float4*>(aux)[i] = make_float4(a[0], a[1], a[2], a[3]);
-  if (contact) contact[i] = (s.flags & FLAG_CONTACT_ARRAY) ? 1 : 0;
+  if (contact) contact[i] = c ? 1 : 0;
 }
 
 // ---------------------------------------------------------------------------------------------------

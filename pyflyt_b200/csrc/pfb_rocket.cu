@@ -2,8 +2,7 @@
 #include <cmath>
 #include <cstring>
 
-#include "pfb_context.h"
-#include "pfb_noise.cuh"
+#include "pfb_aviary.cuh"
 #include "pfb_rocket_host.h"
 #include "pfb_tail_step.cuh"
 
@@ -24,10 +23,7 @@ __global__ void __launch_bounds__(kBlock) k_rk_reset(const __grid_constant__ Roc
   int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= N) return;
   if (mask && !mask[i]) return;
-  RocketRegs s;
-  rocket_reset(p, s, start_pos[3 * i], start_pos[3 * i + 1], start_pos[3 * i + 2], start_orn[3 * i], start_orn[3 * i + 1], start_orn[3 * i + 2]);
-  rocket_store(st, ist, N, i, s);
-  ist[(int64_t)RI_STEP * N + i] = 0;
+  rk_reset_drone(p, st, ist, N, i, start_pos, start_orn, i);
   if (setpoint)
     for (int k = 0; k < 7; ++k) setpoint[7 * i + k] = 0.0f;
 }
@@ -56,13 +52,7 @@ __global__ void __launch_bounds__(kBlock, kMinBlocks)
                      uint32_t seq, int64_t N) {
   int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= N) return;
-  RocketRegs s;
-  rocket_load(st, ist, N, i, s);
-#pragma unroll
-  for (int k = 0; k < 7; ++k) s.sp[k] = __ldg(setpoint + 7 * i + k);
-  auto nz = make_noise<INJECT>(noise, N, i, rng, seq, TAG_AVIARY, p.noise_loc, p.ratio);
-  for (int k = 0; k < n_steps; ++k) rocket_aviary_step(p, s, nz, false);
-  rocket_store(st, ist, N, i, s);
+  rk_aviary_step_drone<INJECT>(p, rng, st, ist, N, i, setpoint, noise, N, i, n_steps, seq);
 }
 
 __global__ void __launch_bounds__(kBlock) k_rk_observe(const float* __restrict__ st, const int32_t* __restrict__ ist,
@@ -70,15 +60,13 @@ __global__ void __launch_bounds__(kBlock) k_rk_observe(const float* __restrict__
                                                        uint8_t* __restrict__ contact, int64_t N) {
   int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= N) return;
-  RocketRegs s;
-  rocket_load(st, ist, N, i, s);
-  float o[12], a[9];
-  rocket_drone_state(s, o, a);
+  float o[12], a[9], hi[3], lo[3];
+  const bool c = rk_query_drone(st, ist, N, i, o, a, hi, lo);
   if (drone_state)
     for (int k = 0; k < 12; ++k) drone_state[12 * i + k] = o[k];
   if (aux)
     for (int k = 0; k < 9; ++k) aux[9 * i + k] = a[k];
-  if (contact) contact[i] = (s.flags & FLAG_CONTACT_ARRAY) ? 1 : 0;
+  if (contact) contact[i] = c ? 1 : 0;
 }
 
 // ---------------------------------------------------------------------------------------------------
@@ -325,14 +313,6 @@ int rk_reset(PfbContext* h, const uint8_t* mask, cudaStream_t s) {
   k_rk_reset<<<grid_for(h->n), kBlock, 0, s>>>(h->rk, h->buf.state, h->buf.istate, h->buf.setpoint, h->buf.start_pos, h->buf.start_orn, mask, h->n);
   LAUNCH_CHECK(h);
   if (!mask) h->mode = 0;
-  return 0;
-}
-
-int rk_set_mode(PfbContext* h, int mode, cudaStream_t s) {
-  (void)s;
-  if (mode != 0)  // base_drone.py:252-255
-    return fail("`mode` must be either 0 or be registered in self.registered_controllers.keys()=dict_keys([]), got %d.", mode);
-  h->mode = 0;
   return 0;
 }
 

@@ -358,6 +358,82 @@ def test_mixed_handle_bit_equal_to_single_kind_handles(variant):
 
 
 @pytest.mark.gpu
+def test_mixed_reset_and_set_mode_against_single_kind_handles():
+    """Masked and full resets, set_mode(int) and set_mode(list) on a mixed handle against single-kind handles over the same
+    drones: the state bit for bit, each setpoint row at its kind's width, and the columns past that width zero, also where they
+    held values before.  Steps in between show that the modes are kept or replaced as on the single-kind handles."""
+    import torch
+
+    from pyflyt_b200 import _lib
+    from pyflyt_b200.core.aviary import BatchedAviary
+
+    n = 256 + 13
+    kinds, opts, start, orn, modes, sp = _mixed_setup(n, 5)
+    mixed = BatchedAviary(start, orn, drone_type=kinds, drone_options=opts, seed=3)
+    uniform = {}
+    for k in ("quadx", "fixedwing", "rocket"):
+        kopts = [o if kk == k else CF2X for o, kk in zip(opts, kinds)] if k == "quadx" else None
+        uniform[k] = BatchedAviary(start, orn, drone_type=k, drone_options=kopts, seed=3)
+    avs = [mixed] + list(uniform.values())
+    ks = np.array(kinds)
+    fill = torch.as_tensor(sp, device="cuda")
+    for k, u in uniform.items():  # non-zero columns past each drone's own setpoint length
+        fill[torch.as_tensor(ks == k, device="cuda"), u.setpoint_dim :] = 9.0
+    mask = torch.as_tensor(np.random.default_rng(6).random(n) < 0.5, dtype=torch.uint8, device="cuda")
+
+    def load_setpoints():
+        mixed.setpoints.copy_(fill)
+        for u in uniform.values():
+            u.setpoints.copy_(fill[:, : u.setpoint_dim])
+
+    def set_modes(ms):
+        mixed.set_mode(ms)
+        for k, u in uniform.items():
+            u.set_mode(ms if isinstance(ms, int) else [m if kk == k else 0 for m, kk in zip(ms, kinds)])
+
+    def same(x, y):  # bit for bit
+        return torch.equal(x.contiguous().view(torch.int32), y.contiguous().view(torch.int32))
+
+    def check(what, rows_rewritten=True):
+        torch.cuda.synchronize()
+        s = mixed.all_states
+        for k, u in uniform.items():
+            m = torch.as_tensor(ks == k, device="cuda")
+            assert same(s[m], u.all_states[m]), (what, k)
+            assert same(mixed.setpoints[m][:, : u.setpoint_dim], u.setpoints[m]), (what, k)
+            if rows_rewritten:
+                assert bool((mixed.setpoints[m][:, u.setpoint_dim :] == 0).all()), (what, k)
+
+    def step_and_check(what):  # a step leaves the setpoint rows as they are
+        load_setpoints()
+        for a in avs:
+            a.step(3)
+        check(what, rows_rewritten=False)
+
+    set_modes(modes)
+    step_and_check("per-drone modes")
+    load_setpoints()
+    for a in avs:
+        _lib.check(_lib.lib().pfb_reset(a._h, C.c_void_p(mask.data_ptr()), a._s()))
+    check("masked reset")
+    step_and_check("modes kept by a masked reset")
+    load_setpoints()
+    set_modes(0)
+    check("set_mode(0)")
+    step_and_check("mode 0")
+    load_setpoints()
+    set_modes(modes)
+    check("set_mode(list)")
+    step_and_check("per-drone modes again")
+    load_setpoints()
+    for a in avs:
+        a.reset()
+    check("reset")
+    assert float(mixed.setpoints.abs().max()) == 0.0
+    step_and_check("mode 0 after a reset")
+
+
+@pytest.mark.gpu
 def test_one_launch_per_step_and_accessors():
     import torch
 
