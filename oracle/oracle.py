@@ -45,6 +45,8 @@ def lib() -> C.CDLL:
         L.orc_set_wind.argtypes = [vp, vp]
         L.orc_wind_field.argtypes = [vp, i64, dp, dp]
         L.orc_surface_wrench.argtypes = [vp, C.c_int, i64, dp, dp, dp, dp, dp]
+        L.orc_solve_contacts.argtypes = [vp, i64, dp, dp, dp, dp, dp, dp, dp, dp, C.c_double, dp, dp, u8p]
+        L.orc_contact_flag.argtypes = [vp, i64, dp, dp, dp, u8p]
         L.orc_reset.argtypes = [vp, u8p]
         L.orc_set_mode.argtypes = [vp, C.c_int]
         L.orc_set_setpoints.argtypes = [vp, dp, C.c_int]
@@ -87,6 +89,38 @@ def surface_wrench(model, si: int, actuation, vb, w):
     F, T = np.zeros((len(act), 3)), np.zeros((len(act), 3))
     L.orc_surface_wrench(C.byref(model), int(si), len(act), _dp(act), _dp(vb), _dp(w), _dp(F), _dp(T))
     return F, T
+
+
+def _rows(a, n, width):
+    """`a` as n contiguous fp64 rows of `width` values (n values for width 1), a scalar or a single row broadcast"""
+    a = np.asarray(a, dtype=np.float64)
+    if width == 1:
+        return np.ascontiguousarray(np.broadcast_to(a, (n,)))
+    return np.ascontiguousarray(np.broadcast_to(a.reshape(-1, width), (n, width)))
+
+
+def solve_contacts(model, pz, R, v, w, M, c, I_O, top, dt):
+    """The floor contact solver of ``model`` on its own, in fp64, for n cases: base altitude pz[n], rotation R[n][3][3] (body
+    to world), world velocity v[n][3] and world rate w[n][3], composite mass M[n], COM offset c[n][3] and inertia about the base
+    origin I_O[n][3][3] (base frame), surface height top[n], time step dt -> (v, w, touched) after the solve.  Scalars and
+    single rows broadcast over the n cases."""
+    L = lib()
+    pz = np.ascontiguousarray(np.atleast_1d(np.asarray(pz, dtype=np.float64)))
+    n = len(pz)
+    R, v, w, c, I_O = (_rows(a, n, k) for a, k in ((R, 9), (v, 3), (w, 3), (c, 3), (I_O, 9)))
+    M, top = _rows(M, n, 1), _rows(top, n, 1)
+    vo, wo, touched = np.zeros((n, 3)), np.zeros((n, 3)), np.zeros(n, dtype=np.uint8)
+    L.orc_solve_contacts(C.byref(model), n, _dp(pz), _dp(R), _dp(v), _dp(w), _dp(M), _dp(c), _dp(I_O), _dp(top), float(dt), _dp(vo), _dp(wo), _u8(touched))
+    return vo, wo, touched.astype(bool)
+
+
+def contact_flag(model, pz, R, top):
+    """detect_contact_at of ``model`` for n poses: base altitude pz[n], rotation R[n][3][3], surface height top[n] -> bool[n]"""
+    pz = np.ascontiguousarray(np.atleast_1d(np.asarray(pz, dtype=np.float64)))
+    n = len(pz)
+    out = np.zeros(n, dtype=np.uint8)
+    lib().orc_contact_flag(C.byref(model), n, _dp(pz), _dp(_rows(R, n, 9)), _dp(_rows(top, n, 1)), _u8(out))
+    return out.astype(bool)
 
 
 class Oracle:

@@ -1,6 +1,6 @@
 // TEST HARNESS — runs the shared PFB_HD math helpers of pyflyt_b200/csrc one element at a time, so that each can be held
-// against an fp64 reference on its own (tests/test_device_math.py).  Built twice from this one file by the `probe` target
-// of pyflyt_b200/csrc/Makefile:
+// against an fp64 reference on its own (tests/test_device_math.py; the floor contact solver and flag: tests/test_contact_solver.py).
+// Built twice from this one file by the `probe` target of pyflyt_b200/csrc/Makefile:
 //   * nvcc with the product's flags (sm_90a): a grid-stride kernel per helper, arrays are DEVICE pointers;
 //   * g++: the same evaluators in a host loop, arrays are HOST pointers (IEEE division / sqrt and libm in the helpers).
 // Each evaluator calls the helper and nothing else.  Never linked into libpyflyt_b200.so; the kernels only write results.
@@ -139,6 +139,47 @@ struct Fast {  // 0: fast_rcp, 1: fast_rsqrt, 2: fast_sqrt
   PFB_HD void operator()(int64_t i) const { out[i] = which == 0 ? fast_rcp(x[i]) : which == 1 ? fast_rsqrt(x[i]) : fast_sqrt(x[i]); }
 };
 
+// apply_contact_impulses over a primitive list (ContactParams, or the QuadX table read in place), with the vehicle's own state
+// registers: pz[n], R[n][9] (body to world, row-major), world velocity v[n][3], body rate w[n][3], mass M[n], COM offset c[n][3],
+// central inertia Ic[n][6] (xx, xy, xz, yy, yz, zz; base frame), surface height top[n] -> world velocity vo[n][3], body rate wo[n][3]
+template <class Shapes, class Regs>
+struct ContactImpulses {
+  Shapes cp;
+  float dt;
+  const float *pz, *R, *v, *w, *M, *c, *Ic, *top;
+  float *vo, *wo;
+  PFB_HD void operator()(int64_t i) const {
+    Regs s;
+    memset(&s, 0, sizeof(s));
+    const float* r = R + 9 * i;
+    s.R.m00 = r[0]; s.R.m01 = r[1]; s.R.m02 = r[2]; s.R.m10 = r[3]; s.R.m11 = r[4]; s.R.m12 = r[5]; s.R.m20 = r[6]; s.R.m21 = r[7]; s.R.m22 = r[8];
+    s.vx = v[3 * i]; s.vy = v[3 * i + 1]; s.vz = v[3 * i + 2];
+    s.wx = w[3 * i]; s.wy = w[3 * i + 1]; s.wz = w[3 * i + 2];
+    const float* I = Ic + 6 * i;
+    apply_contact_impulses(&cp, s, pz[i], top[i], M[i], Vec3{c[3 * i], c[3 * i + 1], c[3 * i + 2]}, I[0], I[1], I[2], I[3], I[4], I[5], dt);
+    vo[3 * i] = (float)s.vx; vo[3 * i + 1] = (float)s.vy; vo[3 * i + 2] = (float)s.vz;
+    wo[3 * i] = s.wx; wo[3 * i + 1] = s.wy; wo[3 * i + 2] = s.wz;
+  }
+};
+struct GroundContact {  // pz[n], R[n][9], top[n] -> ground_contact flag [n]
+  ContactParams cp;
+  const float *pz, *R, *top;
+  int32_t* out;
+  PFB_HD void operator()(int64_t i) const { out[i] = ground_contact(cp, pz[i], R[9 * i + 6], R[9 * i + 7], R[9 * i + 8], top[i]) ? 1 : 0; }
+};
+struct QuadXGroundContact {  // pz[n], R[n][9] -> quadx_ground_contact flag [n] (the floor only)
+  QuadXParams p;
+  const float *pz, *R;
+  int32_t* out;
+  PFB_HD void operator()(int64_t i) const {
+    QuadXRegs s;
+    memset(&s, 0, sizeof(s));
+    s.pz = pz[i];
+    s.R.m20 = R[9 * i + 6]; s.R.m21 = R[9 * i + 7]; s.R.m22 = R[9 * i + 8];
+    out[i] = quadx_ground_contact(p, s) ? 1 : 0;
+  }
+};
+
 #define PROBE_API extern "C" __attribute__((visibility("default")))
 
 PROBE_API const char* probe_last_error(void) { return g_err; }
@@ -171,4 +212,42 @@ PROBE_API int probe_solve_sym3(int64_t n, const float* J, const float* r, float*
 PROBE_API int probe_fast(int which, int64_t n, const float* x, float* out) {
   if (which < 0 || which > 2) return fail("fast helper %d out of range", which);
   return run(Fast{which, x, out}, n);
+}
+// the contact solver of a HOST PfbModel, narrowed as pfb_create narrows it: the QuadX table for QuadX models, a ContactParams
+// with the fixed-wing or rocket registers otherwise
+template <class Shapes, class Regs>
+static int run_contact(const Shapes& cp, float dt, int64_t n, const float* pz, const float* R, const float* v, const float* w, const float* M,
+                       const float* c, const float* Ic, const float* top, float* vo, float* wo) {
+  ContactImpulses<Shapes, Regs> e;
+  e.cp = cp; e.dt = dt;
+  e.pz = pz; e.R = R; e.v = v; e.w = w; e.M = M; e.c = c; e.Ic = Ic; e.top = top; e.vo = vo; e.wo = wo;
+  return run(e, n);
+}
+PROBE_API int probe_contact_impulses(const PfbModel* m, int64_t n, const float* pz, const float* R, const float* v, const float* w, const float* M,
+                                     const float* c, const float* Ic, const float* top, float* vo, float* wo) {
+  const float dt = (float)(1.0 / m->physics_hz);
+  if (m->kind == PFB_KIND_QUADX) {
+    QuadXParams p;
+    if (build_quadx_params(*m, p)) return -1;
+    return run_contact<QuadXParams, QuadXRegs>(p, dt, n, pz, R, v, w, M, c, Ic, top, vo, wo);
+  }
+  ContactParams cp;
+  memset(&cp, 0, sizeof(cp));
+  if (pfb_build_contact(*m, cp)) return -1;
+  if (m->kind == PFB_KIND_ROCKET) return run_contact<ContactParams, RocketRegs>(cp, dt, n, pz, R, v, w, M, c, Ic, top, vo, wo);
+  return run_contact<ContactParams, FixedwingRegs>(cp, dt, n, pz, R, v, w, M, c, Ic, top, vo, wo);
+}
+// the contact flag: quadx_ground_contact over the QuadX table (top must be 0: QuadX drones meet the floor only), ground_contact otherwise
+PROBE_API int probe_contact_flag(const PfbModel* m, int64_t n, const float* pz, const float* R, const float* top, int32_t* out) {
+  if (m->kind == PFB_KIND_QUADX) {
+    QuadXGroundContact e;
+    if (build_quadx_params(*m, e.p)) return -1;
+    e.pz = pz; e.R = R; e.out = out;
+    return run(e, n);
+  }
+  GroundContact e;
+  memset(&e.cp, 0, sizeof(e.cp));
+  if (pfb_build_contact(*m, e.cp)) return -1;
+  e.pz = pz; e.R = R; e.top = top; e.out = out;
+  return run(e, n);
 }

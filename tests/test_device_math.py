@@ -51,6 +51,8 @@ def _lib(device: bool):
     L.probe_wind_profile.argtypes = [vp, i64, vp, vp]
     L.probe_solve_sym3.argtypes = [i64, vp, vp, vp]
     L.probe_fast.argtypes = [i32, i64, vp, vp]
+    L.probe_contact_impulses.argtypes = [vp, i64] + [vp] * 10
+    L.probe_contact_flag.argtypes = [vp, i64, vp, vp, vp, vp]
     assert L.probe_is_device() == int(device), path
     _LIBS[name] = L
     return L
@@ -114,6 +116,14 @@ class Probe:
 
     def fast(self, which, x):
         return self("probe_fast", (int(which),), [F32(x)], [(1, F32)])[0]
+
+    def contact_impulses(self, model, pz, R, v, w, M, c, Ic, top):
+        """apply_contact_impulses: world velocity v and body rate w after the solve (tests/test_contact_solver.py)"""
+        ins = [F32(pz), F32(R).reshape(-1, 9), F32(v), F32(w), F32(M), F32(c), F32(Ic), F32(top)]
+        return self("probe_contact_impulses", (C.byref(model),), ins, [(3, F32), (3, F32)])
+
+    def contact_flag(self, model, pz, R, top):
+        return self("probe_contact_flag", (C.byref(model),), [F32(pz), F32(R).reshape(-1, 9), F32(top)], [(1, np.int32)])[0].astype(bool)
 
 
 def _f64(a):

@@ -315,7 +315,11 @@ def test_mixed_handle_bit_equal_to_single_kind_handles(variant):
     contact = variant == "contact"
     if contact:  # dropped onto the floor from low heights
         start[:, 2] = np.random.default_rng(1).uniform(0.3, 2.0, n).astype(np.float32)
-        orn[np.array(kinds) == "rocket", 0] = 0.0
+        rk = np.array(kinds) == "rocket"
+        # upright rockets: the origin 0.05-2 m above the resting height, where the legs' lowest corners (z = -2.425 in the body)
+        # touch the floor; lower, the Baumgarte bias would throw a rocket whose legs start inside the floor out of it
+        start[rk, 2] = (2.425 + np.random.default_rng(2).uniform(0.05, 2.0, int(rk.sum()))).astype(np.float32)
+        orn[rk, :2] = 0.0
         sp[np.array(kinds) == "rocket"] = 0.0  # not ignited: the rockets drop and rest on the floor
     wind = AnalyticWind("power", base=(3.0, -1.5, 0.2), z_ref=10.0, alpha=1.0 / 7.0) if variant == "wind" else None
     mixed = BatchedAviary(start, orn, drone_type=kinds, drone_options=opts, seed=11, contact_response=contact)
@@ -352,9 +356,11 @@ def test_mixed_handle_bit_equal_to_single_kind_handles(variant):
         assert torch.equal(con[m], u.contact_array[m]), k
         assert torch.equal(mixed.precise_positions[m], u.precise_positions[m]), k
     assert bool(torch.isfinite(s).all())
-    if contact:  # the QuadX and fixed-wing drones did reach the floor (their contact flags, as every kind's, match bit for bit above)
-        for k in ("quadx", "fixedwing"):
+    if contact:  # every kind did reach the floor (the contact flags match bit for bit above); the rockets came to rest on their legs
+        for k in ("quadx", "fixedwing", "rocket"):
             assert bool(touched[torch.as_tensor(ks == k, device="cuda")].any()), k
+        rz = mixed.precise_positions[torch.as_tensor(ks == "rocket", device="cuda"), 2]
+        assert bool(con[torch.as_tensor(ks == "rocket", device="cuda")].all()) and float(rz.min()) > 2.3 and float(rz.max()) < 2.5, (rz.min(), rz.max())
 
 
 @pytest.mark.gpu
