@@ -176,7 +176,8 @@ typedef struct PfbEnvConfig {
                               * rocket_landing_env.py:231-263) and by Aviary handles (env_kind PFB_ENV_NONE: QuadX, fixed-wing and
                               * rocket drones land on, slide along and rest on the floor).  pfb_create reads no other field of a
                               * PFB_ENV_NONE config.  The other env kinds ignore it (they terminate on the first contact).         */
-  int32_t _pad_cr;
+  int32_t mixed_control_hz;  /* 1 = the tables passed to pfb_create_mixed may differ in control_hz (see there).  Read only by
+                              * pfb_create_mixed from its PFB_ENV_NONE aviary_cfg; pfb_create and the env kinds ignore it.         */
 } PfbEnvConfig;
 
 /* Analytic, time-invariant wind field evaluated IN-KERNEL at every drag body / lifting surface (SURVEY.md 8f item 4).
@@ -251,7 +252,16 @@ int pfb_create(const PfbModel* model, const PfbEnvConfig* env, int64_t n_envs, i
 int pfb_destroy(PfbHandle h);
 /* Aviary(drone_type=[...]) with drones of several kinds (aviary.py:139-190): drone i flies models[model_index[i]] (host array
  * of n entries, each < k).  Every table has the same physics_hz and control_hz; at most PFB_MAX_QUADX_MODELS QuadX tables,
- * one fixed-wing and one rocket table.  aviary_cfg: NULL, or a PFB_ENV_NONE config of which only contact_response is read.
+ * one fixed-wing and one rocket table.  aviary_cfg: NULL, or a PFB_ENV_NONE config of which only contact_response and
+ * mixed_control_hz are read.
+ * With aviary_cfg->mixed_control_hz = 1 the tables may differ in control_hz (the reference's Aviary with per-drone
+ * drone_options control_hz, aviary.py:287-298, 506-529): every table has the same physics_hz, which each control_hz divides;
+ * sorted, each distinct rate is a multiple of the one before; U = physics_hz / min(control_hz) is in 1..4.  A QuadX table is
+ * one (model, rate) pair (its PIDs use the control period); several fixed-wing, or rocket, tables must be byte-equal apart
+ * from control_hz (one model at several rates), and two identical tables are refused.  One pfb_aviary_step step is then U
+ * physics substeps u = 0..U-1 for every drone; drone i, with r_i = physics_hz / control_hz_i, runs its control tick before
+ * substep u when u % r_i == 0.  Injected noise is [n_steps * U][N] (one draw per drone per substep, whatever its rate);
+ * Philox draws are keyed by (seed, i, Aviary step, substep).  If every table has the same control_hz, the flag changes nothing.
  * The handle is an Aviary handle (the env entry points, pfb_set_models and pfb_set_base_velocity refuse it) with:
  *   state     pfb_state_floats() floats, carved by the library into one region per kind (PFB_LAYOUT_BY_KIND): QuadX
  *             warp-tiled, then fixed-wing and rocket field-major, each on a 128-byte boundary; istate [pfb_istate_rows][N];

@@ -9,9 +9,9 @@ difference in meaning: drone ``i`` lives in its OWN world (the reference puts th
 so ``contact_array[i]`` is "drone i touched the floor during the last step".
 
 ``drone_options`` may be a sequence with one dict per drone, as in the reference (aviary.py:75): a QuadX batch then flies up
-to ``MAX_QUADX_MODELS`` different vehicle tables (``models``), drone ``i`` the table ``model_index[i]``.  All of them must run
-at the same ``control_hz``.  Drones ``32 k .. 32 k + 31`` share one warp: a batch runs fastest when each such tile flies one
-model (DESIGN.md §4a).
+to ``MAX_QUADX_MODELS`` different vehicle tables (``models``), drone ``i`` the table ``model_index[i]``.  All of them run at
+the same ``control_hz`` unless ``mixed_control_hz=True`` (below).  Drones ``32 k .. 32 k + 31`` share one warp: a batch runs
+fastest when each such tile flies one model (DESIGN.md §4a).
 
 The floor: the reference's Aviary is a PyBullet world, so a drone that reaches the floor stands on it.  Here, by default, the
 floor only raises ``contact_array`` and a drone keeps falling through ``z = 0`` (the envs end an episode on the first
@@ -24,9 +24,17 @@ a batch then flies QuadX, fixed-wing and rocket drones together, all stepped by 
 keeps its own kind's surface: ``set_setpoint(i, sp)`` takes drone ``i``'s own setpoint length (QuadX 4, fixed-wing 4 or 6,
 rocket 7) and ``state(i)`` / ``aux_state(i)`` return its own aux length (4, 6 or 9); ``setpoints`` is ``[N, 7]`` and
 ``all_aux_states`` a list of ``N`` tensors.  Each kind's drones take their tables from their own ``drone_options`` entries (up
-to ``MAX_QUADX_MODELS`` QuadX models, one fixed-wing and one rocket model), and every drone runs at one ``control_hz``.  Such
-a batch is an Aviary only: no ``env_config``, no ``set_base_velocity``, no ``state_row``.  Drone ``i`` draws the random stream
-drone ``i`` of a single-kind batch with the same seed draws, so it flies exactly as it would there.
+to ``MAX_QUADX_MODELS`` QuadX models, one fixed-wing and one rocket model), and every drone runs at one ``control_hz`` unless
+``mixed_control_hz=True`` (below).  Such a batch is an Aviary only: no ``env_config``, no ``set_base_velocity``, no
+``state_row``.  Drone ``i`` draws the random stream drone ``i`` of a single-kind batch with the same seed draws, so it flies
+exactly as it would there.
+
+``mixed_control_hz=True`` lets the drones' ``drone_options`` differ in ``control_hz``, as in the reference's
+examples/core/02_multi_drone.py (three QuadX at 60, 120 and 240 Hz): the rates must form common multiples (the reference's
+``AssertionError`` otherwise), ``updates_per_step`` and ``step_period`` follow the slowest rate (at most 4 physics steps per
+Aviary step), and drone ``i`` runs its controller on the physics steps that are multiples of ``physics_hz / control_hz[i]``.
+Such a batch is a mixed handle whatever its kinds, with the surface described above (``setpoints`` ``[N, 7]``); a batch whose
+rates turn out equal is the batch built without the option (DESIGN.md §4e).
 
 All state is held in caller-visible ``torch`` tensors; the CUDA library (libpyflyt_b200.so) only sees
 raw device pointers.  There is no CPU path.
@@ -84,11 +92,17 @@ class BatchedAviary:
         env_config: PfbEnvConfig | None = None,
         env_offset: int = 0,
         contact_response: bool = False,
+        mixed_control_hz: bool = False,
     ):
         """``contact_response``: the floor pushes back (contact impulses + Coulomb friction) instead of only raising
         ``contact_array``.  The reference always responds, since every ``Aviary`` is a PyBullet world; here it is opt-in so
         that a handle built without it steps exactly as before, and so that flight far above the floor never pays for the
-        solver.  Aviary handles only: an env handle (``env_config``) has its own contact policy."""
+        solver.  Aviary handles only: an env handle (``env_config``) has its own contact policy.
+
+        ``mixed_control_hz``: the drones' ``drone_options`` may differ in ``control_hz``, as in the reference's
+        tests/test_core.py::test_multi_spawn (DESIGN.md §4e).  An Aviary step is then ``physics_hz / min(control_hz)`` physics
+        steps, and each drone runs its controller every ``physics_hz / control_hz`` of them.  Opt-in so that a batch built
+        without it keeps refusing different rates.  Aviary handles only: an env flies one drone at one rate."""
         start_pos = np.asarray(start_pos, dtype=np.float32)
         start_orn = np.asarray(start_orn, dtype=np.float32)
         # shape checks with the reference's messages (aviary.py:120-131)
@@ -96,6 +110,8 @@ class BatchedAviary:
             raise AviaryInitException(f"start_pos must be shape (n, 3), currently {start_pos.shape}.")
         if start_orn.shape != start_pos.shape:
             raise AviaryInitException(f"start_orn must be same shape as start_pos, currently {start_orn.shape}.")
+        if mixed_control_hz and env_config is not None:
+            raise AviaryInitException("mixed_control_hz is an Aviary-handle option; an env handle (env_config) flies one drone at one control_hz.")
         kinds = None  # one vehicle kind per drone (a list that holds more than one kind), else None
         if isinstance(drone_type, (tuple, list)):
             if len(set(drone_type)) != 1:
@@ -117,14 +133,18 @@ class BatchedAviary:
         models, index = None, None
         if kinds is not None:
             try:
-                models, index = build_mixed_model_set(kinds, drone_options, physics_hz, int(start_pos.shape[0]))
+                models, index = build_mixed_model_set(kinds, drone_options, physics_hz, int(start_pos.shape[0]), mixed_control_hz)
             except ModelSetError as e:
                 raise AviaryInitException(str(e)) from None
         elif drone_options is not None and not isinstance(drone_options, dict):
             try:
-                models, index = build_model_set(drone_type, drone_options, physics_hz, int(start_pos.shape[0]))
+                models, index = build_model_set(drone_type, drone_options, physics_hz, int(start_pos.shape[0]), mixed_control_hz)
             except ModelSetError as e:
                 raise AviaryInitException(str(e)) from None
+        # different control rates: a mixed handle, whether the batch flies one kind or several
+        multi_rate = models is not None and len({float(m.control_hz) for m in models}) > 1
+        if multi_rate and kinds is None:
+            kinds = [str(drone_type)] * int(start_pos.shape[0])
         if not torch.cuda.is_available():
             raise _lib.PfbError("pyflyt_b200 needs a CUDA device (H100, sm_90a); there is no CPU fallback.")
         self.device = torch.device(device)
@@ -139,17 +159,24 @@ class BatchedAviary:
             self.model = build_model(drone_type, opts.pop("drone_model", None), opts.pop("model_dir", None), physics_hz, control_hz, **opts)
             self.models = [self.model]
         else:
-            control_hz = int(models[0].control_hz)
+            control_hz = int(min(m.control_hz for m in models))  # the slowest drone sets the Aviary step (aviary.py:288-289)
             self.model = models[0]
             self.models = models
+        # [N] control rate of every drone
+        self.control_hz = np.full(self.num_drones, control_hz, dtype=np.int64) if index is None else np.array([int(models[k].control_hz) for k in index], dtype=np.int64)
         if contact_response:
             if env_config is not None:
                 raise AviaryInitException("contact_response is an Aviary-handle option; an env handle (env_config) keeps its own contact policy.")
             env_config = PfbEnvConfig()  # env kind NONE: pfb_create reads only contact_response from it
             env_config.contact_response = 1
+        if multi_rate:
+            if env_config is None:
+                env_config = PfbEnvConfig()  # env kind NONE: pfb_create_mixed reads contact_response and mixed_control_hz
+            env_config.mixed_control_hz = 1
         self.contact_response = bool(contact_response)
+        self.mixed_control_hz = bool(mixed_control_hz)
         self.env_config = env_config
-        self.updates_per_step = int(physics_hz / control_hz)  # aviary.py:288-289 (single control rate)
+        self.updates_per_step = int(physics_hz / control_hz)  # aviary.py:288-289
         self.step_period = 1.0 / control_hz
         self.seed = 0 if seed is None else int(seed)
 

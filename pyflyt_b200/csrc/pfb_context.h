@@ -131,9 +131,10 @@ int pfb_new_context(int64_t n, int device, uint64_t seed, PfbContext** out, Setu
   return 0;
 }
 
-// pfb_lib.cu: the coefficient tables of k QuadX models that one handle flies (one substep ratio, dt and motor count), and
-// their installation as the handle's model set with its current wind and the per-drone index (n entries, padded to whole tiles)
-int pfb_quadx_tables(const PfbModel* models, int k, pfb::QuadXParams* tables);
+// pfb_lib.cu: the coefficient tables of k QuadX models that one handle flies (one substep ratio, dt and motor count; with
+// one_rate = false the control rates may differ: a mixed handle at several rates), and their installation as the handle's
+// model set with its current wind and the per-drone index (n entries, padded to whole tiles)
+int pfb_quadx_tables(const PfbModel* models, int k, pfb::QuadXParams* tables, bool one_rate = true);
 int pfb_install_quadx_set(PfbContext* h, const pfb::QuadXParams* tables, int k, const uint8_t* index_host, int64_t n);
 
 // PfbContext::mode of an Aviary handle whose drones fly the modes in d_modes; pfb_set_mode and a full pfb_reset replace it

@@ -483,6 +483,22 @@ PFB_HD void fixedwing_aviary_step_any(const FixedwingParams& p, FixedwingRegs& s
 #pragma unroll 1
   for (int u = 0; u < p.ratio; ++u) fixedwing_substep<FULL, CONTACT>(p, s, cmd, noise.get(u));
 }
+// fixedwing_aviary_step_any inside an Aviary step of U substeps at several control rates: the command mapping runs before
+// substep u when u % r == 0 (r = physics_hz / control_hz of this drone, a divisor of U); draw u of the step.  r == U: the above.
+template <bool FULL, bool CONTACT, typename NoiseFn>
+PFB_HD void fixedwing_aviary_step_rates(const FixedwingParams& p, FixedwingRegs& s, int mode, int r, int U, NoiseFn& noise) {
+  s.flags &= ~(uint32_t)FLAG_CONTACT_ARRAY;
+  noise.begin_step();
+  float cmd[6];
+#pragma unroll 1
+  for (int u = 0; u < U; ++u) {
+    if (u % r == 0) {
+      if (mode == -1) fixedwing_command<-1>(s, cmd);
+      else fixedwing_command<0>(s, cmd);
+    }
+    fixedwing_substep<FULL, CONTACT>(p, s, cmd, noise.get(u));
+  }
+}
 // launch-uniform test for the FULL instantiation
 PFB_HD bool fixedwing_full_model(const FixedwingParams& p) { return p.n_surfaces == kMaxSurfaces && p.wind.kind == 0; }
 

@@ -53,18 +53,18 @@ int pfb_drop_masked_done(PfbContext* h, const uint8_t* mask, cudaStream_t s) {
   return 0;
 }
 
-int pfb_quadx_tables(const PfbModel* models, int k, QuadXParams* tables) {
+int pfb_quadx_tables(const PfbModel* models, int k, QuadXParams* tables, bool one_rate) {
   for (int j = 0; j < k; ++j) {
     const PfbModel& m = models[j];
     if (m.abi_version != PFB_ABI_VERSION) return fail("pfb_set_models: model %d has ABI %d != library ABI %d", j, m.abi_version, PFB_ABI_VERSION);
     if (m.kind != PFB_KIND_QUADX) return fail("pfb_set_models: model %d is not a QuadX (kind %d)", j, m.kind);
     // every kernel runs ONE substep ratio and one dt per handle
-    if (m.physics_hz != models[0].physics_hz || m.control_hz != models[0].control_hz)
+    if (m.physics_hz != models[0].physics_hz || (one_rate && m.control_hz != models[0].control_hz))
       return fail("pfb_set_models: model %d runs at physics_hz %g / control_hz %g, model 0 at %g / %g: every model of a handle needs the same rates", j,
                   m.physics_hz, m.control_hz, models[0].physics_hz, models[0].control_hz);
     memset(&tables[j], 0, sizeof(QuadXParams));
     if (build_quadx_params(m, tables[j]) != 0) return -1;
-    if (tables[j].ratio != tables[0].ratio || tables[j].dt != tables[0].dt || tables[j].ctrl_dt != tables[0].ctrl_dt ||
+    if ((one_rate && (tables[j].ratio != tables[0].ratio || tables[j].ctrl_dt != tables[0].ctrl_dt)) || tables[j].dt != tables[0].dt ||
         tables[j].noise_loc != tables[0].noise_loc)
       return fail("pfb_set_models: model %d has a different substep ratio, dt or motor count than model 0", j);
   }

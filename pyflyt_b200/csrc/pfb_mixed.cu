@@ -10,6 +10,8 @@
 // (pfb_aviary.cuh) with the user index of its slot.
 #include <cuda_runtime.h>
 
+#include <algorithm>
+#include <cmath>
 #include <cstring>
 #include <memory>
 #include <new>
@@ -35,6 +37,10 @@ struct MixedKinds {
   int8_t* d_slot_mode;       // [n] flight mode of each slot
   int8_t* h_slot_mode;       // [n] pfb_set_modes' modes in slot order, on their way to d_slot_mode
   uint8_t* h_kind;           // [n] kind of each user drone
+  // several control rates (PfbEnvConfig::mixed_control_hz): physics substeps per Aviary step, and the control ratio
+  // physics_hz / control_hz of each slot (a divisor of U); d_slot_ratio = nullptr when every drone runs at one rate
+  int U;
+  uint8_t* d_slot_ratio;
 };
 
 // ---------------------------------------------------------------------------------------------------
@@ -84,6 +90,8 @@ struct MixedStep {
   int64_t n;
   int n_steps;
   uint32_t seq;
+  const uint8_t* slot_ratio;    // RATES: [n] control ratio of each slot
+  int U;                        // RATES: physics substeps per Aviary step
 };
 // the whole argument travels in the kernel-parameter bank, which holds 32 764 bytes on sm_90
 static_assert(sizeof(MixedStep<QuadXModelSet>) <= 32764, "the mixed step's __grid_constant__ argument exceeds the kernel-parameter limit");
@@ -91,10 +99,12 @@ static_assert(sizeof(MixedStep<QuadXModelSet>) <= 32764, "the mixed step's __gri
 // n_steps x Aviary.step() for every drone of a mixed handle.  Drone u draws the noise of drone u of a uniform handle of its
 // kind (Philox counter keyed by the USER index, injected column u), and runs the per-drone-mode step of its kind, so each
 // drone's trajectory is bit-equal to the one it flies in a uniform handle with the same seed.  CONTACT: the floor pushes back.
+// RATES (a handle whose drones run at several control rates): every drone runs the handle's U substeps per Aviary step and
+// its control tick on the substeps that are multiples of its slot's ratio; its noise is keyed with U, whatever its own ratio.
 // The branches spell out the step bodies of pfb_aviary.cuh rather than call them: called, their pointers and counts are held
 // in registers across the step loop instead of being read from the parameter bank where they are used, and the kernel needs
 // more stack.
-template <bool INJECT, bool CONTACT, class PS>
+template <bool INJECT, bool CONTACT, bool RATES, class PS>
 __global__ void __launch_bounds__(kBlock, kMinBlocks) k_mixed_aviary_step(const __grid_constant__ MixedStep<PS> a) {
   const MixedRows& r = a.r;
   const int b = blockIdx.x;
@@ -110,8 +120,14 @@ __global__ void __launch_bounds__(kBlock, kMinBlocks) k_mixed_aviary_step(const 
     quadx_mask_pid(s, mode);
 #pragma unroll
     for (int c = 0; c < 4; ++c) s.sp[c] = __ldg(a.setpoint + kMixedSetpointDim * u + c);
-    auto nz = make_noise<INJECT>(a.noise, a.n, u, a.rng, a.seq, TAG_AVIARY, qx_model0(a.qx).noise_loc, qx_model0(a.qx).ratio);
-    for (int k = 0; k < a.n_steps; ++k) quadx_aviary_step_any<CONTACT>(p, s, mode, nz);
+    if constexpr (RATES) {
+      const int ratio = a.slot_ratio[j];
+      auto nz = make_noise<INJECT>(a.noise, a.n, u, a.rng, a.seq, TAG_AVIARY, qx_model0(a.qx).noise_loc, a.U);
+      for (int k = 0; k < a.n_steps; ++k) quadx_aviary_step_rates<CONTACT>(p, s, mode, ratio, a.U, nz);
+    } else {
+      auto nz = make_noise<INJECT>(a.noise, a.n, u, a.rng, a.seq, TAG_AVIARY, qx_model0(a.qx).noise_loc, qx_model0(a.qx).ratio);
+      for (int k = 0; k < a.n_steps; ++k) quadx_aviary_step_any<CONTACT>(p, s, mode, nz);
+    }
     quadx_store_tile<7, kTileGroupStride>(r.qx_st + qx_tile_base(j, QX_ROWS), s, step_count);
   } else if (b < r.cta_qx + r.cta_fw) {
     const int64_t j = (int64_t)(b - r.cta_qx) * kBlock + threadIdx.x;
@@ -123,11 +139,21 @@ __global__ void __launch_bounds__(kBlock, kMinBlocks) k_mixed_aviary_step(const 
     fixedwing_load(r.fw_st, r.fw_ist, r.n_fw, j, s);
 #pragma unroll
     for (int c = 0; c < 6; ++c) s.sp[c] = __ldg(a.setpoint + kMixedSetpointDim * u + c);
-    auto nz = make_noise<INJECT>(a.noise, a.n, u, a.rng, a.seq, TAG_AVIARY, p.noise_loc, p.ratio);
-    if (fixedwing_full_model(p)) {
-      for (int k = 0; k < a.n_steps; ++k) fixedwing_aviary_step_any<true, CONTACT>(p, s, mode, nz);
+    if constexpr (RATES) {
+      const int ratio = a.slot_ratio[r.n_qx + j];
+      auto nz = make_noise<INJECT>(a.noise, a.n, u, a.rng, a.seq, TAG_AVIARY, p.noise_loc, a.U);
+      if (fixedwing_full_model(p)) {
+        for (int k = 0; k < a.n_steps; ++k) fixedwing_aviary_step_rates<true, CONTACT>(p, s, mode, ratio, a.U, nz);
+      } else {
+        for (int k = 0; k < a.n_steps; ++k) fixedwing_aviary_step_rates<false, CONTACT>(p, s, mode, ratio, a.U, nz);
+      }
     } else {
-      for (int k = 0; k < a.n_steps; ++k) fixedwing_aviary_step_any<false, CONTACT>(p, s, mode, nz);
+      auto nz = make_noise<INJECT>(a.noise, a.n, u, a.rng, a.seq, TAG_AVIARY, p.noise_loc, p.ratio);
+      if (fixedwing_full_model(p)) {
+        for (int k = 0; k < a.n_steps; ++k) fixedwing_aviary_step_any<true, CONTACT>(p, s, mode, nz);
+      } else {
+        for (int k = 0; k < a.n_steps; ++k) fixedwing_aviary_step_any<false, CONTACT>(p, s, mode, nz);
+      }
     }
     fixedwing_store(r.fw_st, r.fw_ist, r.n_fw, j, s);
   } else {
@@ -139,8 +165,14 @@ __global__ void __launch_bounds__(kBlock, kMinBlocks) k_mixed_aviary_step(const 
     rocket_load(r.rk_st, r.rk_ist, r.n_rk, j, s);
 #pragma unroll
     for (int c = 0; c < 7; ++c) s.sp[c] = __ldg(a.setpoint + kMixedSetpointDim * u + c);
-    auto nz = make_noise<INJECT>(a.noise, a.n, u, a.rng, a.seq, TAG_AVIARY, p.noise_loc, p.ratio);
-    for (int k = 0; k < a.n_steps; ++k) rocket_aviary_step(p, s, nz, false);
+    if constexpr (RATES) {
+      const int ratio = a.slot_ratio[r.n_qx + r.n_fw + j];
+      auto nz = make_noise<INJECT>(a.noise, a.n, u, a.rng, a.seq, TAG_AVIARY, p.noise_loc, a.U);
+      for (int k = 0; k < a.n_steps; ++k) rocket_aviary_step_rates(p, s, ratio, a.U, nz);
+    } else {
+      auto nz = make_noise<INJECT>(a.noise, a.n, u, a.rng, a.seq, TAG_AVIARY, p.noise_loc, p.ratio);
+      for (int k = 0; k < a.n_steps; ++k) rocket_aviary_step(p, s, nz, false);
+    }
     rocket_store(r.rk_st, r.rk_ist, r.n_rk, j, s);
   }
 }
@@ -318,7 +350,7 @@ int mx_set_modes(PfbContext* h, const int8_t* modes, cudaStream_t s) {
   return set_slot_modes(h, s);
 }
 
-template <bool INJECT, bool CONTACT, class PS>
+template <bool INJECT, bool CONTACT, bool RATES, class PS>
 static void launch_step(const PfbContext* h, const PS& ps, const float* noise, int n_steps, uint32_t seq, cudaStream_t s) {
   const MixedKinds* m = h->mixed;
   MixedStep<PS> a;
@@ -334,14 +366,23 @@ static void launch_step(const PfbContext* h, const PS& ps, const float* noise, i
   a.n = h->n;
   a.n_steps = n_steps;
   a.seq = seq;
-  k_mixed_aviary_step<INJECT, CONTACT, PS><<<grid_all(m), kBlock, 0, s>>>(a);
+  a.slot_ratio = m->d_slot_ratio;
+  a.U = m->U;
+  k_mixed_aviary_step<INJECT, CONTACT, RATES, PS><<<grid_all(m), kBlock, 0, s>>>(a);
+}
+
+// RATES: several control rates (d_slot_ratio set), chosen by the handle and uniform over the launch
+template <bool RATES>
+static void launch_steps(const PfbContext* h, const float* noise, int n_steps, uint32_t seq, cudaStream_t s) {
+  const bool contact = h->env.contact_response != 0;
+  QX_PARAMS_SWITCH(h, (contact ? (noise ? launch_step<true, true, RATES>(h, ps, noise, n_steps, seq, s) : launch_step<false, true, RATES>(h, ps, noise, n_steps, seq, s))
+                                : (noise ? launch_step<true, false, RATES>(h, ps, noise, n_steps, seq, s) : launch_step<false, false, RATES>(h, ps, noise, n_steps, seq, s))));
 }
 
 int mx_aviary_step(PfbContext* h, int n_steps, const float* noise, cudaStream_t s) {
   const uint32_t seq = (uint32_t)h->aviary_seq++;
-  const bool contact = h->env.contact_response != 0;
-  QX_PARAMS_SWITCH(h, (contact ? (noise ? launch_step<true, true>(h, ps, noise, n_steps, seq, s) : launch_step<false, true>(h, ps, noise, n_steps, seq, s))
-                                : (noise ? launch_step<true, false>(h, ps, noise, n_steps, seq, s) : launch_step<false, false>(h, ps, noise, n_steps, seq, s))));
+  if (h->mixed->d_slot_ratio) launch_steps<true>(h, noise, n_steps, seq, s);
+  else launch_steps<false>(h, noise, n_steps, seq, s);
   LAUNCH_CHECK(h);
   return 0;
 }
@@ -363,6 +404,7 @@ void mx_destroy(PfbContext* h) {
   if (!m) return;
   if (m->d_slot_user) cudaFree(m->d_slot_user);
   if (m->d_slot_mode) cudaFree(m->d_slot_mode);
+  if (m->d_slot_ratio) cudaFree(m->d_slot_ratio);
   delete[] m->h_slot_mode;
   delete[] m->h_kind;
   delete m;
@@ -411,9 +453,28 @@ static int mixed_setup(PfbContext* c, const PfbModel* models, int k, const uint8
   CUDA_OK(cudaMalloc(&m->d_slot_mode, (size_t)n));
   CUDA_OK(cudaMemcpy(m->d_slot_user, slot_user.get(), (size_t)n * sizeof(int32_t), cudaMemcpyHostToDevice));
   CUDA_OK(cudaMemset(m->d_slot_mode, 0, (size_t)n));
+  const bool rates = aviary_cfg && aviary_cfg->mixed_control_hz;
+  QuadXParams tables[PFB_MAX_QUADX_MODELS];
+  if (m->count[PFB_KIND_QUADX] && pfb_quadx_tables(qx_models, kq, tables, !rates)) return -1;
+  // several control rates: the ratio of every slot, one source for every kind (pfb_create_mixed has checked the rates)
+  double slowest = models[0].control_hz;
+  for (int j = 1; j < k; ++j) slowest = std::min(slowest, models[j].control_hz);
+  m->U = (int)std::lround(models[0].physics_hz / slowest);
+  bool several = false;
+  for (int j = 0; j < k; ++j) several |= models[j].control_hz != slowest;
+  if (rates && several) {
+    std::unique_ptr<uint8_t[]> slot_ratio(new (std::nothrow) uint8_t[n]);
+    if (!slot_ratio) return fail("out of host memory");
+    for (int64_t t = 0; t < n; ++t) {
+      const PfbModel& mt = models[model_index[slot_user[t]]];
+      slot_ratio[t] = (uint8_t)std::lround(mt.physics_hz / mt.control_hz);
+      if (t < m->count[PFB_KIND_QUADX] && slot_ratio[t] != tables[qx_index[t]].ratio)
+        return fail("pfb_create_mixed: slot %lld has control ratio %d, its QuadX table %d", (long long)t, (int)slot_ratio[t], tables[qx_index[t]].ratio);
+    }
+    CUDA_OK(cudaMalloc(&m->d_slot_ratio, (size_t)n));
+    CUDA_OK(cudaMemcpy(m->d_slot_ratio, slot_ratio.get(), (size_t)n, cudaMemcpyHostToDevice));
+  }
   if (m->count[PFB_KIND_QUADX]) {
-    QuadXParams tables[PFB_MAX_QUADX_MODELS];
-    if (pfb_quadx_tables(qx_models, kq, tables)) return -1;
     c->qx = tables[0];
     if (kq > 1 && pfb_install_quadx_set(c, tables, kq, qx_index.get(), m->count[PFB_KIND_QUADX])) return -1;
   }
@@ -433,22 +494,53 @@ extern "C" int pfb_create_mixed(const PfbModel* models, int k, const uint8_t* mo
   if (k < 1 || k > PFB_MAX_QUADX_MODELS + 2) return fail("pfb_create_mixed: k = %d, must be in 1..%d", k, PFB_MAX_QUADX_MODELS + 2);
   if (aviary_cfg && aviary_cfg->env_kind != PFB_ENV_NONE)
     return fail("pfb_create_mixed: a mixed-kind handle is an Aviary handle; env kind %d flies one vehicle kind", aviary_cfg->env_kind);
+  const bool rates = aviary_cfg && aviary_cfg->mixed_control_hz;
   int tables[kKinds] = {0, 0, 0};
   for (int j = 0; j < k; ++j) {
     const PfbModel& mj = models[j];
     if (mj.abi_version != PFB_ABI_VERSION) return fail("pfb_create_mixed: model %d has ABI %d != library ABI %d", j, mj.abi_version, PFB_ABI_VERSION);
     if (mj.kind < PFB_KIND_QUADX || mj.kind > PFB_KIND_ROCKET) return fail("pfb_create_mixed: model %d has unknown vehicle kind %d", j, mj.kind);
-    // one launch steps every drone with one substep count and one dt
-    if (mj.physics_hz != models[0].physics_hz || mj.control_hz != models[0].control_hz)
+    if (rates) {  // one launch steps every drone with one dt; each drone's control tick falls on whole substeps
+      if (mj.physics_hz != models[0].physics_hz)
+        return fail("pfb_create_mixed: model %d runs at physics_hz %g, model 0 at %g: every drone of a handle needs the same physics_hz", j, mj.physics_hz,
+                    models[0].physics_hz);
+      if (!(mj.control_hz > 0.0) || std::fmod(mj.physics_hz, mj.control_hz) != 0.0)
+        return fail("pfb_create_mixed: model %d: `physics_hz` (%g) must be multiple of `control_hz` (%g).", j, mj.physics_hz, mj.control_hz);
+    } else if (mj.physics_hz != models[0].physics_hz || mj.control_hz != models[0].control_hz)  // one substep count and one dt
       return fail("pfb_create_mixed: model %d runs at physics_hz %g / control_hz %g, model 0 at %g / %g: every drone of a handle needs the same "
                   "physics_hz and control_hz", j, mj.physics_hz, mj.control_hz, models[0].physics_hz, models[0].control_hz);
     tables[mj.kind] += 1;
   }
   if (tables[PFB_KIND_QUADX] > PFB_MAX_QUADX_MODELS)
     return fail("pfb_create_mixed: %d QuadX tables, at most %d", tables[PFB_KIND_QUADX], PFB_MAX_QUADX_MODELS);
-  if (tables[PFB_KIND_FIXEDWING] > 1 || tables[PFB_KIND_ROCKET] > 1)
+  if (rates) {
+    // the reference's rule (aviary.py:287-298): sorted, each rate a multiple of the one before; U = physics_hz / slowest in 1..4
+    double hz[PFB_MAX_QUADX_MODELS + 2];
+    for (int j = 0; j < k; ++j) hz[j] = models[j].control_hz;
+    std::sort(hz, hz + k);
+    for (int j = 1; j < k; ++j)
+      if (std::fmod(hz[j], hz[j - 1]) != 0.0)
+        return fail("pfb_create_mixed: control_hz %g and %g: Looprates must form common multiples of each other.", hz[j - 1], hz[j]);
+    const double U = models[0].physics_hz / hz[0];
+    if (U > 4.0)
+      return fail("pfb_create_mixed: physics_hz %g / slowest control_hz %g = %g physics substeps per Aviary step; a handle runs at most 4 (the limit on "
+                  "one table's physics_hz / control_hz, applied to the handle)", models[0].physics_hz, hz[0], U);
+    // several fixed-wing (rocket) tables are one model at several rates: byte-equal apart from control_hz, and not identical
+    for (int j = 0; j < k; ++j)
+      for (int l = j + 1; l < k; ++l) {
+        if (models[j].kind != models[l].kind || models[j].kind == PFB_KIND_QUADX) continue;
+        PfbModel a = models[j], b = models[l];
+        a.control_hz = b.control_hz = 0.0;
+        if (memcmp(&a, &b, sizeof(PfbModel)) != 0)
+          return fail("pfb_create_mixed: %s tables %d and %d differ beyond control_hz; a handle flies one fixed-wing and one rocket model",
+                      models[j].kind == PFB_KIND_FIXEDWING ? "fixed-wing" : "rocket", j, l);
+        if (models[j].control_hz == models[l].control_hz)
+          return fail("pfb_create_mixed: %s tables %d and %d are identical", models[j].kind == PFB_KIND_FIXEDWING ? "fixed-wing" : "rocket", j, l);
+      }
+  } else if (tables[PFB_KIND_FIXEDWING] > 1 || tables[PFB_KIND_ROCKET] > 1) {
     return fail("pfb_create_mixed: %d fixed-wing and %d rocket tables; a handle flies one fixed-wing and one rocket model", tables[PFB_KIND_FIXEDWING],
                 tables[PFB_KIND_ROCKET]);
+  }
   for (int64_t i = 0; i < n; ++i)
     if (model_index[i] >= k) return fail("pfb_create_mixed: model_index[%lld] = %d, must be < k = %d", (long long)i, (int)model_index[i], k);
   return pfb_new_context(n, device, seed, out, [&](PfbContext* c) { return mixed_setup(c, models, k, model_index, aviary_cfg); });

@@ -552,6 +552,20 @@ PFB_HD void quadx_aviary_step_any(const QuadXParams& p, QuadXRegs& s, int mode, 
   for (int u = 0; u < p.ratio; ++u) quadx_substep<CONTACT>(p, s, noise.get(u));
 }
 
+// quadx_aviary_step_any inside an Aviary step of U substeps whose drones run at several control rates (aviary.py:506-529):
+// this drone, physics_hz / control_hz = r (a divisor of U, the table's own ratio), runs its control tick before substep u when
+// u % r == 0 and takes draw u of the step.  With r == U it is quadx_aviary_step_any.
+template <bool CONTACT = false, typename NoiseFn>
+PFB_HD void quadx_aviary_step_rates(const QuadXParams& p, QuadXRegs& s, int mode, int r, int U, NoiseFn& noise) {
+  s.flags &= ~(uint32_t)FLAG_CONTACT_ARRAY;
+  noise.begin_step();
+#pragma unroll 1
+  for (int u = 0; u < U; ++u) {
+    if (u % r == 0) quadx_update_control_any(p, s, mode);
+    quadx_substep<CONTACT>(p, s, noise.get(u));
+  }
+}
+
 PFB_HD void quadx_set_mode_any(QuadXRegs& s, int mode) { PFB_QX_MODE_CASES(mode, quadx_set_mode<M>(s)); }
 
 // quadx.py:222-231 + aviary.py:310-311: a freshly constructed drone at its start pose

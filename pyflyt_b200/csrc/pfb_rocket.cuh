@@ -226,6 +226,19 @@ PFB_HD void rocket_aviary_step(const RocketParams& p, RocketRegs& s, NoiseFn& no
 #pragma unroll 1
   for (int u = 0; u < p.ratio; ++u) rocket_substep(p, s, cmd, noise.get(u), with_pad);
 }
+// rocket_aviary_step (no pad) inside an Aviary step of U substeps at several control rates: rocket_command runs before
+// substep u when u % r == 0 (r = physics_hz / control_hz of this drone, a divisor of U); draw u of the step.  r == U: the above.
+template <typename NoiseFn>
+PFB_HD void rocket_aviary_step_rates(const RocketParams& p, RocketRegs& s, int r, int U, NoiseFn& noise) {
+  s.flags &= ~(uint32_t)(FLAG_CONTACT_ARRAY | FLAG_CONTACT_PAD | FLAG_CONTACT_GROUND);
+  noise.begin_step();
+  float cmd[8];
+#pragma unroll 1
+  for (int u = 0; u < U; ++u) {
+    if (u % r == 0) rocket_command(s, cmd);
+    rocket_substep(p, s, cmd, noise.get(u), false);
+  }
+}
 
 // rocket.py:226-239 + aviary.py:310-311
 PFB_HD void rocket_reset(const RocketParams& p, RocketRegs& s, float sx, float sy, float sz, float roll, float pitch, float yaw) {

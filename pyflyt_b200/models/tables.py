@@ -144,7 +144,7 @@ class PfbEnvConfig(C.Structure):
         ("spawn_min_height", C.c_double),
         ("spawn_max_height", C.c_double),
         ("contact_response", C.c_int32),
-        ("_pad_cr", C.c_int32),
+        ("mixed_control_hz", C.c_int32),
     ]
 
 
@@ -366,7 +366,36 @@ def _options_key(opts: dict) -> str:
     return repr(sorted((str(k), repr(v)) for k, v in opts.items()))
 
 
-def build_model_set(kind: str, drone_options, physics_hz: int, n: int) -> tuple[list[PfbModel], np.ndarray]:
+MAX_UPDATES_PER_STEP = 4  # physics steps per Aviary step a handle runs (the library's limit on physics_hz / control_hz)
+
+
+def check_control_rates(rates, physics_hz: int, mixed_control_hz: bool) -> None:
+    """The control rates of one batch.  Without ``mixed_control_hz`` they must all be equal.  With it, they follow the
+    reference's rule (aviary.py:287-298): sorted, each rate is an integer multiple of the one before, and an Aviary step is
+    ``physics_hz / min(control_hz)`` physics steps, here at most ``MAX_UPDATES_PER_STEP``."""
+    rates = sorted({int(r) for r in rates})
+    if len(rates) <= 1:
+        return
+    if not mixed_control_hz:
+        raise ModelSetError(f"every drone of a batch needs the same control_hz (one substep ratio per batch; mixed_control_hz=True lets them differ); got {rates}.")
+    if any(b % a for a, b in zip(rates, rates[1:])):
+        raise AssertionError("Looprates must form common multiples of each other.")  # aviary.py:293-298
+    updates = physics_hz // rates[0]
+    if updates > MAX_UPDATES_PER_STEP:
+        raise ModelSetError(
+            f"control_hz {rates} at physics_hz {physics_hz}: an Aviary step of the slowest drone is {updates} physics steps; a batch runs at "
+            f"most {MAX_UPDATES_PER_STEP} (the limit on one drone's physics_hz / control_hz)."
+        )
+
+
+def _bytes_but_rate(m: PfbModel) -> bytes:
+    """the table's bytes with control_hz zeroed: fixed-wing and rocket tables depend on the rate through nothing else"""
+    c = PfbModel.from_buffer_copy(m)
+    c.control_hz = 0.0
+    return C.string_at(C.addressof(c), C.sizeof(c))
+
+
+def build_model_set(kind: str, drone_options, physics_hz: int, n: int, mixed_control_hz: bool = False) -> tuple[list[PfbModel], np.ndarray]:
     """Per-drone vehicle tables for ``n`` drones of one ``kind``.
 
     ``drone_options`` is what the reference's ``Aviary`` takes (aviary.py:75, 196-199): ``None`` or one dict for every drone,
@@ -376,7 +405,11 @@ def build_model_set(kind: str, drone_options, physics_hz: int, n: int) -> tuple[
 
     Raises ``ModelSetError`` for a sequence of the wrong length (the reference's message), for entries with different
     ``control_hz`` (each handle runs one substep ratio), for more than ``MAX_QUADX_MODELS`` distinct QuadX tables and for more
-    than one distinct fixed-wing or rocket table."""
+    than one distinct fixed-wing or rocket table.
+
+    ``mixed_control_hz=True`` lets the entries differ in ``control_hz`` under ``check_control_rates`` (an ``AssertionError``
+    with the reference's message for rates that do not form common multiples).  A QuadX table is then one (model, rate) pair;
+    fixed-wing and rocket tables may differ in ``control_hz`` only, one table per rate."""
     if drone_options is None or isinstance(drone_options, dict):
         entries = [dict(drone_options or {})]
         index = np.zeros(n, dtype=np.int64)
@@ -395,9 +428,8 @@ def build_model_set(kind: str, drone_options, physics_hz: int, n: int) -> tuple[
                 keys[key] = len(entries)
                 entries.append(d)
             index[i] = keys[key]
-    rates = sorted({int(e.get("control_hz", 120)) for e in entries})
-    if len(rates) > 1:
-        raise ModelSetError(f"every drone of a batch needs the same control_hz (one substep ratio per batch); got {rates}.")
+    if not mixed_control_hz:
+        check_control_rates([e.get("control_hz", 120) for e in entries], physics_hz, False)
     tables: list[PfbModel] = []
     by_bytes: dict[bytes, int] = {}
     remap = np.zeros(len(entries), dtype=np.int64)
@@ -410,8 +442,11 @@ def build_model_set(kind: str, drone_options, physics_hz: int, n: int) -> tuple[
             by_bytes[b] = len(tables)
             tables.append(m)
         remap[j] = by_bytes[b]
-    if kind != "quadx" and len(tables) > 1:
-        raise ModelSetError(f"a {kind} batch flies one vehicle model; the drone_options build {len(tables)} different ones.")
+    if mixed_control_hz:  # after build_model: a control_hz that does not divide physics_hz raises its ValueError first, as in the reference
+        check_control_rates([m.control_hz for m in tables], physics_hz, True)
+    models = len({_bytes_but_rate(m) for m in tables}) if mixed_control_hz else len(tables)
+    if kind != "quadx" and models > 1:
+        raise ModelSetError(f"a {kind} batch flies one vehicle model; the drone_options build {models} different ones.")
     if len(tables) > MAX_QUADX_MODELS:
         raise ModelSetError(f"a batch flies at most {MAX_QUADX_MODELS} different vehicle models; the drone_options build {len(tables)}.")
     return tables, remap[index].astype(np.uint8)
@@ -420,14 +455,16 @@ def build_model_set(kind: str, drone_options, physics_hz: int, n: int) -> tuple[
 KINDS = ("quadx", "fixedwing", "rocket")  # PFB_KIND_QUADX, PFB_KIND_FIXEDWING, PFB_KIND_ROCKET
 
 
-def build_mixed_model_set(kinds, drone_options, physics_hz: int, n: int) -> tuple[list[PfbModel], np.ndarray]:
+def build_mixed_model_set(kinds, drone_options, physics_hz: int, n: int, mixed_control_hz: bool = False) -> tuple[list[PfbModel], np.ndarray]:
     """Per-drone vehicle tables for ``n`` drones of several kinds: ``kinds[i]`` is drone ``i``'s ``drone_type``.
 
     ``drone_options`` is what the reference's ``Aviary`` takes: ``None`` or one dict for every drone, or a sequence of ``n``
     dicts, one per drone.  The sub-sequence of each kind goes through ``build_model_set`` (so each kind keeps its limits: up to
     ``MAX_QUADX_MODELS`` QuadX tables, one fixed-wing and one rocket table).  Returns ``(tables, index)``: the QuadX tables,
     then the fixed-wing table, then the rocket table (those present), and a uint8 array ``[n]``, drone ``i`` flies
-    ``tables[index[i]]``.  Every drone must run at the same ``control_hz`` (one launch steps them all with one substep count)."""
+    ``tables[index[i]]``.  Every drone must run at the same ``control_hz`` (one launch steps them all with one substep count),
+    unless ``mixed_control_hz=True``: then the rates of all kinds together follow ``check_control_rates``, and the fixed-wing
+    and rocket tables of each kind follow the QuadX ones in ``build_model_set``'s order, one per rate."""
     kinds = list(kinds)
     if len(kinds) != n:
         raise ModelSetError(f"If multiple `drone_types` are used, must have same number of `drone_types` ({len(kinds)}) as number of drones ({n}).")
@@ -445,12 +482,10 @@ def build_mixed_model_set(kinds, drone_options, physics_hz: int, n: int) -> tupl
         if not ids:
             continue
         opts = [seq[i] for i in ids] if per_drone else drone_options
-        t, idx = build_model_set(kind, opts, physics_hz, len(ids))
+        t, idx = build_model_set(kind, opts, physics_hz, len(ids), mixed_control_hz)
         index[ids] = idx.astype(np.int64) + len(tables)
         tables.extend(t)
-    rates = sorted({float(m.control_hz) for m in tables})
-    if len(rates) > 1:
-        raise ModelSetError(f"every drone of a batch needs the same control_hz (one substep ratio per batch); got {[int(r) for r in rates]}.")
+    check_control_rates([m.control_hz for m in tables], physics_hz, mixed_control_hz)
     return tables, index.astype(np.uint8)
 
 

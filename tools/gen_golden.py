@@ -269,13 +269,14 @@ def _padded_rows(rows, w):
     return np.array([np.concatenate([r, np.zeros(w - len(r))]) for r in rows])
 
 
-def fly_mixed_kinds(name, drone_type, drone_options, start_pos, start_orn, mode_calls, setpoint_fn, n_steps, seed):
+def fly_mixed_kinds(name, drone_type, drone_options, start_pos, start_orn, mode_calls, setpoint_fn, n_steps, seed, kind="mixed_kinds"):
     """Aviary-level flight of QuadX, fixed-wing and rocket drones in ONE reference Aviary (``drone_type`` a list,
     aviary.py:139-190, as examples/core/08_mixed_drones.py does): ``mode_calls`` = {step_index: [n] modes}, each applied with
     ``Aviary.set_mode(list)`` before that step; ``setpoint_fn(step, modes)`` returns None or a list of ``n`` per-drone
     setpoints of each drone's own length, applied with ``set_all_setpoints`` (aviary.py:470-478 indexes ``setpoints[i]``).
     Every drone draws one normal per physics step (its motors or its booster), in drone order, so the recorded draws are
-    [step][substep][drone].  Setpoints are stored padded to 7 columns, aux states to 9."""
+    [step][substep][drone], with ``updates_per_step`` substeps (the slowest drone's ratio when the drones' ``control_hz`` differ,
+    aviary.py:287-298).  Setpoints are stored padded to 7 columns, aux states to 9."""
     n = len(drone_type)
     rng = ril.ScriptedNoise(seed)
     env = Aviary(
@@ -309,7 +310,7 @@ def fly_mixed_kinds(name, drone_type, drone_options, start_pos, start_orn, mode_
     assert noise.size == T * int(env.updates_per_step) * n, (noise.size, T, n)
     np.savez_compressed(
         os.path.join(OUT, f"{name}.npz"),
-        kind="mixed_kinds",
+        kind=kind,
         drone_type=json.dumps(list(drone_type)),
         n_drones=n,
         drone_options=json.dumps(drone_options),
@@ -378,6 +379,104 @@ def mixed_kind_fixtures():
 
     scenario("mixed_kinds_grouped", ["rocket"] * 2 + ["quadx"] * 4 + ["fixedwing"] * 2, 101)
     scenario("mixed_kinds_interleaved", ["rocket", "quadx", "fixedwing", "quadx", "rocket", "fixedwing", "quadx", "fixedwing", "rocket", "quadx"], 102)
+
+
+def rate_fixtures():
+    """Drones at different control rates in one reference Aviary (per-drone ``drone_options`` ``control_hz``; the reference's
+    tests/test_core.py::test_multi_spawn and examples/core/02_multi_drone.py).  An Aviary step is physics_hz / min(control_hz)
+    physics steps and each drone runs its controller on every physics_hz / control_hz-th of them (aviary.py:287-298, 506-529).
+    No drone touches the floor."""
+    # test_multi_spawn: three cf2x at 60 / 120 / 240 Hz in mode 7, a new height at step 150.  cf2x's gains are tuned for faster
+    # control: at 60 or 80 Hz its attitude loop rings after a lateral command and amplifies the round-off difference of two fp64
+    # codes to millimetres within a hundred steps, so here (and below) the slow cf2x drones fly the inner-loop modes or climb
+    pos = np.array([[-1.0, 0.0, 1.0], [0.0, 0.0, 1.0], [1.0, 0.0, 1.0]])
+
+    def spawn_sp(i, modes):
+        if i != 150:
+            return None
+        return [np.array([p[0], p[1], 0.0, 1.2]) for p in pos]
+
+    fly_mixed_kinds("rates_multi_spawn", ["quadx"] * 3, [dict(control_hz=60), dict(control_hz=120), dict(control_hz=240)], pos.tolist(),
+                    np.zeros((3, 3)).tolist(), {0: [7, 7, 7]}, spawn_sp, 300, seed=111, kind="rates")
+
+    # both QuadX models at every rate, in modes -1, 0, 2, 6, 7, re-assigned by one set_mode(list) at step 100
+    table = {-1: [0.3, 0.31, 0.32, 0.3], 0: [0.1, -0.05, 0.05, 0.45], 2: [0.1, -0.1, 0.2, 1.0], 6: [0.5, 0.3, 0.3, 0.2], 7: [0.5, -0.5, 0.4, 1.0]}
+    combos = [(m, hz) for m in ("cf2x", "primitive_drone") for hz in (60, 120, 240)] + [("primitive_drone", 60), ("cf2x", 120), ("cf2x", 240),
+                                                                                      ("primitive_drone", 60)]
+    n = 10
+    opts = [dict(drone_model=combos[d][0], control_hz=combos[d][1]) for d in range(n)]
+    cycle = [-1, 0, 2, 6, 7]
+    first = [cycle[d % 5] for d in range(n)]
+    second = [cycle[(d + 2) % 5] for d in range(n)]
+    pos = np.array([[8.0 * d, 0.0, 60.0 + 0.5 * d] for d in range(n)])
+    orn = [[0.05 * (d % 3), -0.04 * (d % 2), 0.3 * (d % 5)] for d in range(n)]
+
+    def modes_sp(i, modes):
+        if i % 100 != 0 and i % 100 != 40:
+            return None
+        out = []
+        for d, m in enumerate(modes):
+            sp = np.array(table[m]) * (1.0 if i % 100 == 0 else -0.5)
+            if m in (2, 7):
+                sp[3] = pos[d, 2] + (1.0 if i % 100 == 0 else -0.5)
+            if m == 7:
+                sp[:2] += pos[d, :2]
+            if m == -1:
+                sp = np.array(table[-1])
+            out.append(sp)
+        return out
+
+    fly_mixed_kinds("rates_models_modes", ["quadx"] * n, opts, pos.tolist(), orn, {0: first, 100: second}, modes_sp, 200, seed=112, kind="rates")
+
+    # rockets, QuadX and fixed-wing drones interleaved: QuadX at 60 / 120 / 240 Hz, fixed-wing at 60 / 120 Hz, rockets at 120 / 240 Hz
+    kinds = ["rocket", "quadx", "fixedwing", "quadx", "rocket", "fixedwing", "quadx", "fixedwing", "rocket", "quadx"]
+    hz = {"quadx": [60, 120, 240], "fixedwing": [60, 120], "rocket": [120, 240]}
+    seen = {"quadx": 0, "fixedwing": 0, "rocket": 0}
+    opts, first = [], []
+    for k in kinds:
+        c = hz[k][seen[k] % len(hz[k])]
+        opts.append(dict(drone_model={"quadx": "cf2x", "fixedwing": "fixedwing", "rocket": "rocket"}[k], control_hz=c))
+        first.append({"quadx": [0, 7, 7, 0][seen[k] % 4], "fixedwing": [0, -1][seen[k] % 2], "rocket": 0}[k])
+        seen[k] += 1
+    pos = np.array([[12.0 * d, 0.0, {"quadx": 150.0, "fixedwing": 200.0, "rocket": 150.0}[k] + 0.5 * d] for d, k in enumerate(kinds)])
+    orn = [[np.pi / 2, 0.0, 0.2 * (d % 3)] if k == "rocket" else [0.05 * (d % 3), -0.04 * (d % 2), 0.3 * (d % 5)] for d, k in enumerate(kinds)]
+    r = np.random.default_rng(113)
+
+    def kinds_sp(i, modes):
+        if i % 50 != 10:
+            return None
+        out = []
+        for d, (k, m) in enumerate(zip(kinds, modes)):
+            if k == "rocket":
+                out.append(np.concatenate([r.uniform(-0.5, 0.5, 3), [1.0, r.uniform(0.3, 0.8)], r.uniform(-0.3, 0.3, 2)]))
+            elif k == "fixedwing":
+                out.append(np.concatenate([r.uniform(-0.6, 0.6, 5), r.uniform(0.3, 1.0, 1)]) if m == -1 else
+                           np.concatenate([r.uniform(-0.5, 0.5, 3), r.uniform(0.3, 1.0, 1)]))
+            elif m == 7:
+                out.append(np.array([pos[d, 0] + r.uniform(-1, 1), pos[d, 1] + r.uniform(-1, 1), r.uniform(-0.8, 0.8), pos[d, 2] + r.uniform(-1, 1)]))
+            else:
+                out.append(np.concatenate([r.uniform(-0.3, 0.3, 3), r.uniform(0.3, 0.45, 1)]))
+        return out
+
+    fly_mixed_kinds("rates_kinds_interleaved", kinds, opts, pos.tolist(), orn, {0: first}, kinds_sp, 300, seed=113, kind="rates")
+
+    # 80 and 240 Hz: three physics steps per Aviary step
+    kinds = ["quadx", "quadx", "fixedwing", "rocket", "quadx"]
+    opts = [dict(control_hz=80), dict(control_hz=240), dict(control_hz=80), dict(control_hz=240), dict(drone_model="primitive_drone", control_hz=80)]
+    pos = np.array([[0.0, 0.0, 30.0], [10.0, 0.0, 30.0], [20.0, 0.0, 80.0], [30.0, 0.0, 60.0], [40.0, 0.0, 30.0]])
+    orn = [[0.05, -0.04, 0.3], [0.0, 0.05, -0.2], [0.05, 0.1, 0.4], [np.pi / 2, 0.0, 0.2], [-0.05, 0.0, 0.1]]
+    r = np.random.default_rng(114)
+
+    def thirds_sp(i, modes):
+        if i % 60 != 0:
+            return None
+        return [np.concatenate([r.uniform(-0.1, 0.1, 3), r.uniform(0.35, 0.45, 1)]),
+                np.concatenate([r.uniform(-0.3, 0.3, 3), r.uniform(0.3, 0.45, 1)]),
+                np.concatenate([r.uniform(-0.5, 0.5, 3), r.uniform(0.3, 1.0, 1)]),
+                np.concatenate([r.uniform(-0.5, 0.5, 3), [1.0, r.uniform(0.3, 0.8)], r.uniform(-0.3, 0.3, 2)]),
+                np.array([pos[4, 0] + r.uniform(-1, 1), pos[4, 1] + r.uniform(-1, 1), r.uniform(-0.5, 0.5), pos[4, 2] + r.uniform(-1, 1)])]
+
+    fly_mixed_kinds("rates_thirds", kinds, opts, pos.tolist(), orn, {0: [0, 0, 0, 0, 7]}, thirds_sp, 240, seed=114, kind="rates")
 
 
 def wind_fields(wind):
@@ -1036,3 +1135,5 @@ if __name__ == "__main__":
         ground_fixtures()
     if which in ("all", "mixedkinds"):
         mixed_kind_fixtures()
+    if which in ("all", "rates"):
+        rate_fixtures()
