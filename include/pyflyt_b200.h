@@ -147,6 +147,20 @@ typedef struct PfbModel {
   double starting_velocity[3]; /* fixedwing.py:35,201                                                */
 } PfbModel;
 
+/* PfbEnvConfig.autoreset: what pfb_env_step does with an env that terminates or truncates on call k.
+ *   NONE       nothing: the caller resets it (pfb_env_reset with a mask)
+ *   NEXT_STEP  call k + 1 is its reset: the action is ignored, obs is the first observation of the new episode, reward 0,
+ *              both flags 0 (gymnasium's AutoresetMode.NEXT_STEP)
+ *   SAME_STEP  call k resets it too: reward, term, trunc and info are the terminal step's, the terminal observation goes to
+ *              row i of PfbBuffers.final_obs and obs holds the first observation of the new episode; call k + 1 steps it with
+ *              the caller's action (gymnasium's AutoresetMode.SAME_STEP).  QuadX-Hover, QuadX-Waypoints,
+ *              Fixedwing-Waypoints and Rocket-Landing only; pfb_env_step_host / pfb_env_step_mapped refuse such a handle.
+ * Autoreset episode e of env i starts from the same state in both modes: its warm-up is keyed by (seed, global env id, e).
+ * pfb_create refuses any other value. */
+#define PFB_AUTORESET_NONE 0
+#define PFB_AUTORESET_NEXT_STEP 1
+#define PFB_AUTORESET_SAME_STEP 2
+
 /* Env-epilogue constants (gym_envs/quadx_envs/quadx_hover_env.py:29-38 and friends). */
 typedef struct PfbEnvConfig {
   int32_t env_kind;          /* PFB_ENV_*                                                            */
@@ -155,7 +169,7 @@ typedef struct PfbEnvConfig {
   int32_t max_steps;         /* agent_hz * max_duration_seconds                                      */
   int32_t angle_representation; /* 0 euler, 1 quaternion                                             */
   int32_t sparse_reward;
-  int32_t autoreset;         /* 1: NEXT_STEP autoreset inside pfb_env_step (gymnasium's default)     */
+  int32_t autoreset;         /* PFB_AUTORESET_*: 0 none, 1 NEXT_STEP (gymnasium's default), 2 SAME_STEP */
   int32_t warmup_steps;      /* 10 Aviary steps after reset (quadx_base_env.py:209-210)              */
   double flight_dome_size;
   double goal_reach_distance, goal_reach_angle;  /* waypoint envs                                    */
@@ -223,7 +237,9 @@ typedef struct PfbBuffers {
   uint8_t* term;             /* [N]                                                                  */
   uint8_t* trunc;            /* [N]                                                                  */
   uint8_t* info;             /* [N] bit0 out_of_bounds, bit1 collision, bit2 env_complete            */
-  float* final_obs;          /* reserved (NEXT_STEP autoreset returns the terminal obs itself)       */
+  float* final_obs;          /* [N][O] SAME_STEP autoreset: row i = terminal observation of env i when it
+                              * finished on the last pfb_env_step (other rows untouched); mandatory there,
+                              * unused otherwise (NEXT_STEP returns the terminal obs in obs itself)       */
   /* outputs of pfb_observe_state (Aviary.state / aux_state) */
   float* drone_state;        /* [N][12] = state(i) (4,3) flattened: ang_vel_b, euler, lin_vel_b, pos */
   float* aux_state;          /* [N][A]                                                               */

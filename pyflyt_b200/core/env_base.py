@@ -9,7 +9,11 @@ from __future__ import annotations
 import torch
 
 from ..models import PfbEnvConfig
+from ..models.tables import AUTORESET_NEXT_STEP, AUTORESET_SAME_STEP
 from .aviary import BatchedAviary
+
+# env_config's autoreset_mode -> PfbEnvConfig.autoreset when autoreset is on
+AUTORESET_MODES = {"next_step": AUTORESET_NEXT_STEP, "same_step": AUTORESET_SAME_STEP}
 
 
 def check_env_args(agent_hz: int, render_mode: None | str, angle_representation: str = "quaternion", hz_error: type = ValueError) -> None:
@@ -26,21 +30,28 @@ def check_env_args(agent_hz: int, render_mode: None | str, angle_representation:
 
 
 def env_config(env_kind: int, *, agent_hz: int, max_duration_seconds: float, angle_representation: str, sparse_reward: bool,
-               autoreset: bool, flight_dome_size: float, inline_reset: bool = False, **fields) -> PfbEnvConfig:
+               autoreset: bool, flight_dome_size: float, inline_reset: bool = False, autoreset_mode: str = "next_step",
+               **fields) -> PfbEnvConfig:
     """The ``PfbEnvConfig`` of an env of kind ``env_kind``: the fields every kind derives from its constructor arguments, then
     the kind-specific ``fields`` as given.
 
     ``inline_reset`` (autoreset kinds): integrate every post-reset warm-up inside the step launch instead of copying the env's
-    spare post-reset state.  The results are the same bit for bit; the tests compare the two paths."""
+    spare post-reset state.  The results are the same bit for bit; the tests compare the two paths.
+
+    ``autoreset_mode`` (with ``autoreset``): ``"next_step"``, gymnasium's NEXT_STEP (a finished env is reset on the next
+    call, which ignores its action), or ``"same_step"``, gymnasium's SAME_STEP (it is reset inside the call that finishes it,
+    which returns the terminal observation in ``final_obs``)."""
     if inline_reset not in (0, 1):
         raise ValueError(f"inline_reset must be a bool, got {inline_reset!r}")
+    if autoreset_mode not in AUTORESET_MODES:
+        raise ValueError(f"autoreset_mode must be one of {sorted(AUTORESET_MODES)}, got {autoreset_mode!r}")
     cfg = PfbEnvConfig()
     cfg.env_kind = env_kind
     cfg.env_step_ratio = int(120 / agent_hz)
     cfg.max_steps = int(agent_hz * max_duration_seconds)
     cfg.angle_representation = 0 if angle_representation == "euler" else 1
     cfg.sparse_reward = int(bool(sparse_reward))
-    cfg.autoreset = int(bool(autoreset))
+    cfg.autoreset = AUTORESET_MODES[autoreset_mode] if autoreset else 0
     cfg.warmup_steps = 10  # Aviary steps after a reset: quadx_base_env.py:209-210, fixedwing_base_env.py:187-188
     cfg.flight_dome_size = float(flight_dome_size)
     cfg.inline_reset = int(inline_reset)
@@ -87,16 +98,31 @@ class VecEnv(AviaryEnv):
         whole batch (``BatchedAviary.reseed``): the same seed then replays the same episodes."""
         return self._reset(mask=mask, noise=noise, seed=seed)
 
+    @property
+    def same_step(self) -> bool:
+        """Whether a finished env is reset inside the step that finishes it (``autoreset_mode="same_step"``)."""
+        return self.config.autoreset == AUTORESET_SAME_STEP
+
     def step(self, actions: torch.Tensor, noise=None):
         """env.step(action) for every env.  With ``autoreset`` (gymnasium's default NEXT_STEP mode) an env that terminated or
         truncated on the previous call is reset on this one: its action is ignored and it returns the first observation of the
-        new episode with reward 0 and both flags False, all inside the same kernel launch."""
+        new episode with reward 0 and both flags False, all inside the same kernel launch.
+
+        With ``autoreset_mode="same_step"`` (gymnasium's SAME_STEP) an env that terminates or truncates on this call is reset
+        on it too: the returned observation is the first one of its new episode, while reward, terminated, truncated and the
+        other info keys are those of the step that finished it (so ``info`` holds its terminal flags; there is no
+        ``final_info``).  ``info["final_obs"]`` is a zero-copy [N, O] view of its terminal observations, valid where
+        ``info["_final_obs"]`` (= terminated | truncated) is set."""
         a = self.aviary
         if not (torch.is_tensor(actions) and actions.is_cuda and actions.dtype == torch.float32 and actions.is_contiguous()):
             a.setpoints.copy_(torch.as_tensor(actions, dtype=torch.float32, device=self.device).reshape(a.setpoints.shape))
             actions = None
         a.env_step(actions=actions, noise=noise)
-        return a.obs, a.reward, a.term.bool(), a.trunc.bool(), self._info()
+        term, trunc, info = a.term.bool(), a.trunc.bool(), self._info()
+        if self.same_step:
+            info["final_obs"] = a.final_obs
+            info["_final_obs"] = term | trunc
+        return a.obs, a.reward, term, trunc, info
 
     def rollout(self, n_steps: int) -> None:
         """n_steps env steps with on-device uniform random actions (the benchmark's workload); the buffers then hold the last

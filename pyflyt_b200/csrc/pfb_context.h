@@ -79,6 +79,7 @@ struct PfbContext {
   float* d_spare;          // spare post-reset states (env-major records), zero-initialised; nullptr = warm-ups run inline
   int2* d_consumed;        // QuadX-Hover fused rollout: (env, episode to rebuild) for every spare a launch consumed
   int fused_ready;         // every env has its spares kRolloutAhead ahead and the step pipeline is drained (cleared by single steps / resets)
+  uint32_t same_launches;  // QuadX-Hover SAME_STEP launches so far: launch n appends its top-up list to d_counters[5 + n % 2]
   uint32_t* d_elist;       // QuadX-Hover: [4][N] episode number being built for each done-list entry (builder phase 0 -> phase 1)
   uint32_t* d_episode;     // QuadX-Hover: [N] episode number of each env's current valid spare (its buffer = episode & kSpareMask)
   cudaStream_t side;       // tail-CTA kinds: the spare rebuild runs here, concurrently with the following step launches
@@ -202,7 +203,7 @@ static inline StepPlan plan_step(PfbContext* h) {
   // tail CTAs (front of the grid) reset the envs that finished on the previous call; one per SM is
   // plenty for the ~1-3 % of envs that finish per step, and the loop is grid-strided anyway
   p.tail = 0;
-  if (h->env.autoreset != 0) {
+  if (h->env.autoreset == PFB_AUTORESET_NEXT_STEP) {  // SAME_STEP resets in the regular lanes: no tail CTAs
     p.tail = h->sm_count;
     int need = grid_for(h->n);
     if (p.tail > need) p.tail = need;
@@ -236,11 +237,12 @@ constexpr int kModeHi[3] = {7, 0, 0};
   }
 
 // ---- host side of the tail-CTA env kinds (pfb_tail_step.cuh): QuadX-Waypoints, Fixedwing-Waypoints, Rocket-Landing, Dogfight ----
-// Each kind passes one generic lambda `launch(StepVariant<INJECT, RANDACT, AUTORESET>{}, const TailLaunch&)` that launches its step
-// kernel and returns 0 or the result of fail(); it serves the step, the side-stream spare rebuild and the build after a reset.
-template <bool INJECT, bool RANDACT, bool AUTORESET>
+// Each kind passes one generic lambda `launch(StepVariant<INJECT, RANDACT, AUTORESET, SAME>{}, const TailLaunch&)` that launches its
+// step kernel and returns 0 or the result of fail(); it serves the step, the side-stream spare rebuild and the build after a reset.
+// SAME: the SAME_STEP step kernel (tail_step_same), which reads only the current lists, the spares and spare_copy of L.
+template <bool INJECT, bool RANDACT, bool AUTORESET, bool SAME = false>
 struct StepVariant {
-  static constexpr bool inject = INJECT, randact = RANDACT, autoreset = AUTORESET;
+  static constexpr bool inject = INJECT, randact = RANDACT, autoreset = AUTORESET, same = SAME;
 };
 struct TailLaunch {
   int grid, tail_blocks;
@@ -256,13 +258,20 @@ template <class Launch>
 int tail_env_step(PfbContext* h, const float* noise, bool randact, cudaStream_t s, Launch&& launch) {
   const StepPlan pl = plan_step(h);
   float* spare = h->env.autoreset ? h->d_spare : nullptr;
-  // the rebuild of the spares consumed by step k - 2 must be complete before step k (an env cannot finish again sooner)
-  if (spare && h->step_seq >= 2) CUDA_OK(cudaStreamWaitEvent(s, h->ev_spare[(h->step_seq - 2) % 4], 0));
+  const bool same = h->env.autoreset == PFB_AUTORESET_SAME_STEP;
+  // NEXT_STEP: the rebuild of the spares consumed by step k - 2 must be complete before step k (an env cannot finish again sooner).
+  // SAME_STEP: an env reset on step k - 1 may finish again on step k and take its next spare there, so step k waits for the
+  // rebuild behind step k - 1
+  if (spare && same && h->step_seq >= 1) CUDA_OK(cudaStreamWaitEvent(s, h->ev_spare[(h->step_seq - 1) % 4], 0));
+  if (spare && !same && h->step_seq >= 2) CUDA_OK(cudaStreamWaitEvent(s, h->ev_spare[(h->step_seq - 2) % 4], 0));
   if (pl.prof) CUDA_OK(cudaEventRecord(h->prof_ev[2 * h->prof_n], s));
   const TailLaunch L = {pl.grid, pl.tail, spare, (spare && !h->env.inline_reset) ? 1 : 0, 0,
                         pl.cnt_prev, pl.list_prev, pl.cnt_cur, pl.list_cur, pl.cnt_next, pl.seq, s};
   int rc;
-  if (h->env.autoreset) {
+  if (same) {
+    if (noise) return fail("injected noise (parity mode) is only supported with autoreset = 0");
+    rc = randact ? launch(StepVariant<false, true, true, true>{}, L) : launch(StepVariant<false, false, true, true>{}, L);
+  } else if (h->env.autoreset) {
     if (noise) return fail("injected noise (parity mode) is only supported with autoreset = 0");
     rc = randact ? launch(StepVariant<false, true, true>{}, L) : launch(StepVariant<false, false, true>{}, L);
   } else {
@@ -278,7 +287,10 @@ int tail_env_step(PfbContext* h, const float* noise, bool randact, cudaStream_t 
   if (spare) {  // rebuild the spares this launch consumed, on the side stream (ordered behind it), while the next launches run
     CUDA_OK(cudaEventRecord(h->ev_step, s));
     CUDA_OK(cudaStreamWaitEvent(h->side, h->ev_step, 0));
-    const TailLaunch B = {h->sm_count, h->sm_count, spare, 0, 1, pl.cnt_prev, pl.list_prev, pl.cnt_cur, pl.list_cur, pl.cnt_next, pl.seq, h->side};
+    // NEXT_STEP consumes the spares of the previous step's list in its tail CTAs, SAME_STEP those of its own list
+    const int32_t* rb_count = same ? pl.cnt_cur : pl.cnt_prev;
+    const int32_t* rb_list = same ? pl.list_cur : pl.list_prev;
+    const TailLaunch B = {h->sm_count, h->sm_count, spare, 0, 1, rb_count, rb_list, pl.cnt_cur, pl.list_cur, pl.cnt_next, pl.seq, h->side};
     if (launch(StepVariant<false, false, true>{}, B)) return -1;
     LAUNCH_CHECK(h);
     CUDA_OK(cudaEventRecord(h->ev_spare[h->step_seq % 4], h->side));

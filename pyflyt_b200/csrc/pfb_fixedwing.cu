@@ -317,6 +317,18 @@ __global__ void __launch_bounds__(kBlock, kAeroBlocks)
   tail_step<AUTORESET>(WpEnv<INJECT, RANDACT>{p, w, rng}, st, ist, actions, noise, obs, reward, term, trunc, info, start_pos, start_orn,
                        prev_count, prev_list, cur_count, cur_list, next_count, spare, spare_copy, build, tail_blocks, step_seq, N);
 }
+// SAME_STEP autoreset: a finishing env is reset in this launch (tail_step_same)
+template <bool RANDACT>
+__global__ void __launch_bounds__(kBlock, kAeroBlocks)
+    k_fwwp_step_same(const __grid_constant__ FixedwingParams p, const __grid_constant__ WaypointParams w, const __grid_constant__ RngParams rng,
+                     float* __restrict__ st, int32_t* __restrict__ ist, float* __restrict__ actions, float* __restrict__ obs,
+                     float* __restrict__ final_obs, float* __restrict__ reward, uint8_t* __restrict__ term, uint8_t* __restrict__ trunc,
+                     uint8_t* __restrict__ info, const float* __restrict__ start_pos, const float* __restrict__ start_orn,
+                     int32_t* __restrict__ cur_count, int32_t* __restrict__ cur_list, int32_t* __restrict__ next_count,
+                     const float* __restrict__ spare, int spare_copy, uint32_t step_seq, int64_t N) {
+  tail_step_same(WpEnv<false, RANDACT>{p, w, rng}, st, ist, actions, nullptr, obs, final_obs, reward, term, trunc, info, start_pos, start_orn,
+                 cur_count, cur_list, next_count, spare, spare_copy, step_seq, N);
+}
 
 template <bool INJECT>
 __global__ void __launch_bounds__(kBlock)
@@ -416,6 +428,13 @@ int fw_observe(PfbContext* h, cudaStream_t s) {
 static auto fwwp_launcher(PfbContext* h, float* actions, const float* noise) {
   return [=](auto v, const TailLaunch& L) -> int {
     using V = decltype(v);
+    if constexpr (V::same) {
+      k_fwwp_step_same<V::randact><<<L.grid, kBlock, 0, L.stream>>>(h->fw, h->wp, h->rng, h->buf.state, h->buf.istate, actions, h->buf.obs,
+                                                                    h->buf.final_obs, h->buf.reward, h->buf.term, h->buf.trunc, h->buf.info,
+                                                                    h->buf.start_pos, h->buf.start_orn, L.cur_count, L.cur_list, L.next_count,
+                                                                    L.spare, L.spare_copy, L.seq, h->n);
+      return 0;
+    }
     k_fwwp_step<V::inject, V::randact, V::autoreset><<<L.grid, kBlock, 0, L.stream>>>(
         h->fw, h->wp, h->rng, h->buf.state, h->buf.istate, actions, noise, h->buf.obs, h->buf.reward, h->buf.term, h->buf.trunc, h->buf.info,
         h->buf.start_pos, h->buf.start_orn, L.prev_count, L.prev_list, L.cur_count, L.cur_list, L.next_count, L.spare, L.spare_copy, L.build,

@@ -46,7 +46,8 @@ __global__ void __launch_bounds__(1024) k_drop_masked_done(int32_t* __restrict__
   if (threadIdx.x == 0) *count = kept;
 }
 int pfb_drop_masked_done(PfbContext* h, const uint8_t* mask, cudaStream_t s) {
-  if (!mask || !h->env.autoreset || !h->d_done_list) return 0;
+  // SAME_STEP: every finished env was reset by the step that finished it, nothing is pending
+  if (!mask || !h->env.autoreset || h->env.autoreset == PFB_AUTORESET_SAME_STEP || !h->d_done_list) return 0;
   const uint64_t k = h->step_seq;  // the next step: its tail CTAs read list [(k - 1) % 4]
   k_drop_masked_done<<<1, 1024, 0, s>>>(h->d_done_list + ((k + 3) % 4) * h->n, h->d_counters + ((k + 3) % 4), mask);
   LAUNCH_CHECK(h);
@@ -200,6 +201,11 @@ int pfb_create(const PfbModel* model, const PfbEnvConfig* env, int64_t n_envs, i
     aviary_contact = env->contact_response ? 1 : 0;
     env = nullptr;
   }
+  if (env && (env->autoreset < PFB_AUTORESET_NONE || env->autoreset > PFB_AUTORESET_SAME_STEP))
+    return fail("autoreset must be 0 (none), 1 (NEXT_STEP) or 2 (SAME_STEP), got %d", env->autoreset);
+  if (env && env->autoreset == PFB_AUTORESET_SAME_STEP && (env->env_kind == PFB_ENV_MA_QUADX_HOVER || env->env_kind == PFB_ENV_DOGFIGHT))
+    return fail("SAME_STEP autoreset (autoreset = 2) is for the single-agent env kinds; MAQuadXHover and MAFixedwingDogfight reset arenas "
+                "through pfb_env_reset (MAQuadXHover) or NEXT_STEP (MAFixedwingDogfight)");
   return pfb_new_context(n_envs, device, seed, out, [&](PfbContext* c) { return single_setup(c, model, env, aviary_contact); });
 }
 
@@ -265,6 +271,8 @@ int pfb_bind(PfbHandle h, const PfbBuffers* b) {
   if (!b->state || !b->istate || !b->setpoint || !b->start_pos || !b->start_orn)
     return fail("pfb_bind: state, istate, setpoint, start_pos and start_orn are mandatory");
   if (((uintptr_t)b->setpoint & 15) || ((uintptr_t)b->state & 15)) return fail("pfb_bind: buffers must be 16-byte aligned");
+  if (h->env.autoreset == PFB_AUTORESET_SAME_STEP && !b->final_obs)
+    return fail("pfb_bind: a SAME_STEP autoreset handle writes the terminal observations to final_obs, which is NULL");
   h->buf = *b;
   h->bound = true;
   return 0;
@@ -500,6 +508,9 @@ int pfb_env_step_host(PfbHandle h, const float* host_actions, float* host_obs, f
                       uint8_t* host_trunc, void* stream) {
   REQUIRE_BOUND(h);
   if (require_env(h)) return -1;
+  if (h->env.autoreset == PFB_AUTORESET_SAME_STEP)
+    return fail("pfb_env_step_host: its single obs | reward | term | trunc copy has no room for final_obs; a SAME_STEP autoreset handle "
+                "steps through pfb_env_step");
   cudaStream_t s = (cudaStream_t)stream;
   const int O = pfb_obs_dim(h);
   CUDA_OK(cudaMemcpyAsync(h->buf.setpoint, host_actions, (size_t)h->n * pfb_setpoint_dim(h) * sizeof(float), cudaMemcpyHostToDevice, s));
@@ -533,6 +544,8 @@ int pfb_env_step_mapped(PfbHandle h, const float* host_actions, float* host_obs,
                         uint8_t* host_trunc, void* stream) {
   REQUIRE_BOUND(h);
   if (require_env(h)) return -1;
+  if (h->env.autoreset == PFB_AUTORESET_SAME_STEP)
+    return fail("pfb_env_step_mapped: it writes no final_obs; a SAME_STEP autoreset handle steps through pfb_env_step");
   if (!host_actions || !host_obs || !host_reward || !host_term || !host_trunc) return fail("pfb_env_step_mapped: null argument");
   void *da = nullptr, *dob = nullptr, *dr = nullptr, *dte = nullptr, *dtr = nullptr;
   if (cudaHostGetDevicePointer(&da, (void*)host_actions, 0) != cudaSuccess || cudaHostGetDevicePointer(&dob, host_obs, 0) != cudaSuccess ||

@@ -731,6 +731,156 @@ __global__ void __launch_bounds__(kBlock, 14)
   if (bulk && lane == 0) bulk_store_wait_read();  // the CTA's shared memory must outlive the engine's reads
 }
 
+// SAME_STEP autoreset (PFB_AUTORESET_SAME_STEP): T env steps of every env in one launch — T = 1 for pfb_env_step (the caller's
+// actions, or RANDACT), up to kRolloutMaxSteps for pfb_env_rollout — on the look-ahead spares of the fused rollout.  Every lane
+// integrates every step; a lane whose env finishes writes the step's reward / flags / info from the terminal state and its
+// terminal observation row to final_obs, then swaps in the spare of episode e_local (or integrates it cold under the same
+// number) and observes the reset state into obs.  At launch, the spares e_local .. e_local + kRolloutAhead - 1 are valid (the
+// look-ahead invariant); a fourth reset of one env in a launch finds a stale record and takes the cold path.  After the steps,
+// the spares each env needs to be kRolloutAhead ahead again go on the top-up list, which k_hover_spare_topup builds on the
+// same stream before the next launch.  The list counter alternates between launches: this launch zeroes the one the next
+// appends to (the previous top-up, which read it, has finished).
+template <int MODE, bool RANDACT, class PS>
+__global__ void __launch_bounds__(kBlock, 14)
+    k_hover_same(const __grid_constant__ PS ps, const __grid_constant__ HoverParams h, const __grid_constant__ RngParams rng,
+                 float* __restrict__ st, int rows, float* __restrict__ actions, float* __restrict__ obs, float* __restrict__ final_obs,
+                 float* __restrict__ reward, uint8_t* __restrict__ term, uint8_t* __restrict__ trunc, uint8_t* __restrict__ info,
+                 const float* __restrict__ start_pos, const float* __restrict__ start_orn, const float* __restrict__ spare,
+                 uint32_t* __restrict__ episode, int32_t* __restrict__ consumed_count, int2* __restrict__ consumed_list,
+                 int32_t* __restrict__ next_consumed_count, int spare_copy, uint32_t step_seq0, int T, int64_t N) {
+  const int tile = (int)blockIdx.x;
+  __shared__ __align__(128) float smem2[2][kBlock * kObsMax];  // the observation tile of step t leaves by TMA while step t + 1 fills the other one
+  constexpr int kInGroups = qx_groups_moved<MODE>();
+  __shared__ __align__(128) float stile[kInGroups * kTileGroupStride];
+  __shared__ __align__(8) uint64_t mbar;
+  const int O = h.angle_representation == 0 ? 20 : 21;
+  const int lane = threadIdx.x;
+  const int64_t tile_first = (int64_t)tile * kBlock;
+  const int64_t i = tile_first + lane;
+  const bool active = i < N;
+  const QuadXParams& p = qx_model(ps, i);  // the model index is padded to whole tiles: every lane may read it
+  float* rec = st + qx_tile_base(i, rows);
+  if (tile == 0 && lane == 0) *next_consumed_count = 0;
+  if (lane == 0) {
+    mbar_init(&mbar, 1);
+    bulk_load_g2s(stile, st + qx_tile_base(tile_first, rows), (uint32_t)(kInGroups * kTileGroupStride * sizeof(float)), &mbar);
+  }
+  __syncwarp();
+  const uint32_t e0 = active ? episode[i] : 0u;  // the next spare this env consumes
+  uint32_t e_local = e0;
+  float sx = 0.f, sy = 0.f, sz = 0.f, ox = 0.f, oy = 0.f, oz = 0.f;
+  if (active) {
+    sx = start_pos[3 * i + 0]; sy = start_pos[3 * i + 1]; sz = start_pos[3 * i + 2];
+    ox = start_orn[3 * i + 0]; oy = start_orn[3 * i + 1]; oz = start_orn[3 * i + 2];
+  }
+  QuadXRegs s;
+  int step_count;
+  mbar_wait(&mbar, 0);
+  quadx_load_tile<MODE, kTileGroupStride>(stile + lane * 4, s, step_count);
+  int64_t nrows = N - tile_first;
+  if (nrows > kBlock) nrows = kBlock;
+  const uint32_t obs_bytes = (uint32_t)nrows * (uint32_t)O * 4u;
+  const bool bulk = (obs_bytes & 15u) == 0u;
+  float* obs_dst = obs + tile_first * O;
+  const uint64_t g = ((uint64_t)rng.env_offset_hi << 32 | rng.env_offset_lo) + (uint64_t)i;
+#pragma unroll 1
+  for (int t = 0; t < T; ++t) {
+    const uint32_t step_seq = step_seq0 + (uint32_t)t;
+    // ---- the step's draws: motor noise and the action, same counters as every other step launch
+    auto nz = make_noise<false>(nullptr, N, active ? i : 0, rng, step_seq, TAG_ENV_STEP, qx_model0(ps).noise_loc, qx_model0(ps).ratio);
+    nz.prefetch4();
+    float act[4] = {0.f, 0.f, 0.f, 0.f};
+    if (RANDACT) {
+      U4 r = philox4x32_10(U4{(uint32_t)g, (uint32_t)(g >> 32), step_seq, (uint32_t)TAG_ACTION << 24}, rng.k0, rng.k1);
+      const float pi = 3.14159265358979323846f;
+      if (MODE == -1) {
+        act[0] = 0.8f * u32_to_unit_open(r.x); act[1] = 0.8f * u32_to_unit_open(r.y);
+        act[2] = 0.8f * u32_to_unit_open(r.z); act[3] = 0.8f * u32_to_unit_open(r.w);
+      } else {
+        act[0] = pi * (2.0f * u32_to_unit_open(r.x) - 1.0f); act[1] = pi * (2.0f * u32_to_unit_open(r.y) - 1.0f);
+        act[2] = pi * (2.0f * u32_to_unit_open(r.z) - 1.0f); act[3] = 0.8f * u32_to_unit_open(r.w);
+      }
+      if (active) reinterpret_cast<float4*>(actions)[i] = make_float4(act[0], act[1], act[2], act[3]);
+    } else if (active) {
+      const float4 a4 = __ldg(reinterpret_cast<const float4*>(actions) + i);
+      act[0] = a4.x; act[1] = a4.y; act[2] = a4.z; act[3] = a4.w;
+    }
+    const int n_aviary = active ? h.env_step_ratio : 0;
+    float rew = -0.1f;
+#pragma unroll
+    for (int k = 0; k < 4; ++k) s.sp[k] = act[k];
+#pragma unroll 1
+    for (int k = 0; k < n_aviary; ++k) {
+      if (s.flags & (FLAG_TERM | FLAG_TRUNC)) break;  // quadx_base_env.py:289-290
+      quadx_aviary_step<MODE>(p, s, nz);
+      hover_term_trunc_reward(h, s, step_count, rew);
+    }
+    step_count += 1;
+    if (active) hover_step_outputs(reward, term, trunc, info, i, rew, s.flags);
+    const bool done = active && (s.flags & (FLAG_TERM | FLAG_TRUNC)) != 0;
+    // ---- outputs of the step
+    float* smem = smem2[t & 1];
+    if (bulk && lane == 0) asm volatile("cp.async.bulk.wait_group.read 1;" ::: "memory");  // the copy that read THIS buffer two steps ago
+    __syncwarp();
+    float* row = smem + lane * O;
+    hover_observation(h, s, act, row);
+    if (done) {
+      for (int k = 0; k < O; ++k) final_obs[i * O + k] = row[k];
+      // env.reset(): begin_reset + end_reset (quadx_base_env.py:149-212), from the spare of episode e_local
+      const float* srec = spare_rec(spare, e_local, N, i);
+      const F4 m0 = ld_f4(srec + SP_POSE), m1 = ld_f4(srec + SP_POSE + 4), m2 = ld_f4(srec + SP_POSE + 8);
+      const bool hit = spare_copy && m1.z != 0.0f && bits_from_f(m2.x) == e_local && m0.x == sx && m0.y == sy && m0.z == sz && m0.w == ox &&
+                       m1.x == oy && m1.y == oz;
+      if (hit) {
+        int dummy;
+        quadx_load_tile<MODE, 4>(srec, s, dummy);
+        const F4 pw = ld_f4(srec + QX_PWM);
+        s.pwm[0] = pw.x; s.pwm[1] = pw.y; s.pwm[2] = pw.z; s.pwm[3] = pw.w;
+        s.flags = bits_from_f(m1.w);
+      } else {
+        HOVER_RESET_COLD(s, sx, sy, sz, ox, oy, oz, e_local);
+      }
+#pragma unroll
+      for (int k = 0; k < 4; ++k) { s.sp[k] = 0.0f; act[k] = 0.0f; }  // self.action = zeros (quadx_base_env.py:165)
+      step_count = 0;
+      e_local += 1u;
+      hover_observation(h, s, act, row);
+    }
+    fence_async_smem();
+    __syncwarp();
+    if (bulk) {
+      if (lane == 0) bulk_store_s2g(obs_dst, smem, obs_bytes);
+    } else {
+      for (int j = lane; j < (int)nrows * O; j += kBlock) obs_dst[j] = smem[j];
+    }
+    quadx_requantize(s);  // what storing the state and loading it again in the next launch does to the fp64-carried fields
+  }
+  if (active) {
+    quadx_store_tile<MODE, kTileGroupStride>(rec, s, step_count);
+    episode[i] = e_local;
+  }
+  // the top-up list: the spares e_local .. e_local + kRolloutAhead - 1 that are not valid any more (the ones from
+  // e0 + kRolloutAhead on), at most kRolloutAhead per env, in distinct buffers.  One atomic per warp.
+  if (spare_copy) {
+    const uint32_t first = e_local > e0 + (uint32_t)kRolloutAhead ? e_local : e0 + (uint32_t)kRolloutAhead;
+    const int need = active ? (int)(e_local + (uint32_t)kRolloutAhead - first) : 0;
+    int incl = need;
+#pragma unroll
+    for (int off = 1; off < kBlock; off <<= 1) {
+      const int v = __shfl_up_sync(0xffffffffu, incl, off);
+      if (lane >= off) incl += v;
+    }
+    const int total = __shfl_sync(0xffffffffu, incl, kBlock - 1);
+    if (total) {
+      int base = 0;
+      if (lane == kBlock - 1) base = atomicAdd(consumed_count, total);
+      base = __shfl_sync(0xffffffffu, base, kBlock - 1) + incl - need;
+      for (int j = 0; j < need; ++j) consumed_list[base + j] = make_int2((int)i, (int)(first + (uint32_t)j));
+    }
+  }
+  if (bulk && lane == 0) bulk_store_wait_read();  // the CTA's shared memory must outlive the engine's reads
+}
+
 // After a user reset of every env: each env gets a complete fresh spare (dense warps, all envs).
 template <int MODE, class PS>
 __global__ void __launch_bounds__(kBlock, kHoverBlocks)
@@ -875,8 +1025,52 @@ int hover_env_reset(PfbContext* h, const uint8_t* mask, const float* noise, cuda
   return 0;
 }
 
+// SAME_STEP: T env steps in one k_hover_same launch, then the top-up of the spares it consumed, on the same stream.  The first
+// launch after a reset or a change of the spares brings every env's spares kRolloutAhead ahead (k_hover_spare_ahead); with
+// inline_reset = 1 every reset is integrated cold and the spares are left alone.
+static int hover_same_launch(PfbContext* h, float* actions, bool randact, int T, cudaStream_t s) {
+  const int mode = h->hover.flight_mode;
+  const int tiles = grid_for(h->n);
+  const int spare_copy = h->env.inline_reset ? 0 : 1;
+  if (spare_copy && !h->fused_ready) {
+    QX_PARAMS_SWITCH(h, PFB_MODE_SWITCH(mode, (k_hover_spare_ahead<MODE, PS><<<tiles, kBlock, 0, s>>>(ps, h->hover, h->rng, h->buf.start_pos, h->buf.start_orn,
+                                                                                                      h->d_spare, h->d_episode, h->n))));
+    LAUNCH_CHECK(h);
+    h->fused_ready = 1;
+  }
+  const StepPlan pl = plan_step(h);
+  int32_t* cnt = h->d_counters + 5 + (h->same_launches & 1u);
+  int32_t* cnt_next = h->d_counters + 5 + ((h->same_launches + 1u) & 1u);
+  if (pl.prof) CUDA_OK(cudaEventRecord(h->prof_ev[2 * h->prof_n], s));
+#define SAME_ARGS ps, h->hover, h->rng, h->buf.state, qx_rows(h), actions, h->buf.obs, h->buf.final_obs, h->buf.reward, h->buf.term, h->buf.trunc, \
+                  h->buf.info, h->buf.start_pos, h->buf.start_orn, h->d_spare, h->d_episode, cnt, h->d_consumed, cnt_next, spare_copy, pl.seq, T, h->n
+  if (randact) { QX_PARAMS_SWITCH(h, PFB_MODE_SWITCH(mode, (k_hover_same<MODE, true, PS><<<tiles, kBlock, 0, s>>>(SAME_ARGS)))); }
+  else { QX_PARAMS_SWITCH(h, PFB_MODE_SWITCH(mode, (k_hover_same<MODE, false, PS><<<tiles, kBlock, 0, s>>>(SAME_ARGS)))); }
+#undef SAME_ARGS
+  LAUNCH_CHECK(h);
+  if (pl.prof) {
+    CUDA_OK(cudaEventRecord(h->prof_ev[2 * h->prof_n + 1], s));
+    h->prof_n += 1;
+  }
+  if (spare_copy) {
+    int topup_grid = 8 * h->sm_count;
+    if (topup_grid > tiles) topup_grid = tiles;
+    QX_PARAMS_SWITCH(h, PFB_MODE_SWITCH(mode, (k_hover_spare_topup<MODE, PS><<<topup_grid, kBlock, 0, s>>>(ps, h->hover, h->rng, h->buf.start_pos,
+                                                                                                           h->buf.start_orn, h->d_spare, cnt, h->d_consumed,
+                                                                                                           h->n))));
+    LAUNCH_CHECK(h);
+  }
+  h->same_launches += 1;
+  h->step_seq += (uint64_t)T;
+  return 0;
+}
+
 int hover_env_step(PfbContext* h, float* actions, const float* noise, bool randact, size_t dyn_smem, cudaStream_t s) {
   const int mode = h->hover.flight_mode;
+  if (h->env.autoreset == PFB_AUTORESET_SAME_STEP) {
+    if (noise) return fail("injected noise (parity mode) is only supported with autoreset = 0");
+    return hover_same_launch(h, actions, randact, 1, s);
+  }
   const bool autoreset = h->env.autoreset != 0;
   // step k appends the envs that finish to list k; its builder CTAs start the next spares of list k - 1 (the envs this launch
   // resets) and finish those of list k - 2, next to which phase 0 left the episode numbers it started (d_elist)
@@ -995,6 +1189,11 @@ int hover_invalidate_spares(PfbContext* h, cudaStream_t s) {
 }
 
 int hover_env_rollout(PfbContext* h, int n_steps, cudaStream_t s) {
+  if (h->env.autoreset == PFB_AUTORESET_SAME_STEP) {  // the same kernel as a single step, kRolloutMaxSteps steps per launch
+    for (int k = 0; k < n_steps; k += kRolloutMaxSteps)
+      if (hover_same_launch(h, h->buf.setpoint, true, n_steps - k < kRolloutMaxSteps ? n_steps - k : kRolloutMaxSteps, s)) return -1;
+    return 0;
+  }
   if (n_steps >= kFusedMinSteps && hover_fused_ok(h)) return hover_rollout_fused(h, n_steps, s);
   for (int k = 0; k < n_steps; ++k)
     if (hover_env_step(h, h->buf.setpoint, nullptr, true, 0, s)) return -1;

@@ -272,6 +272,18 @@ __global__ void __launch_bounds__(kBlock, kMinBlocks)
   tail_step<AUTORESET>(QwEnv<MODE, INJECT, RANDACT, PS>{ps, h, w, rng}, st, ist, actions, noise, obs, reward, term, trunc, info, start_pos,
                        start_orn, prev_count, prev_list, cur_count, cur_list, next_count, spare, spare_copy, build, tail_blocks, step_seq, N);
 }
+// SAME_STEP autoreset: a finishing env is reset in this launch (tail_step_same)
+template <int MODE, bool RANDACT, class PS>
+__global__ void __launch_bounds__(kBlock, kMinBlocks)
+    k_qxwp_step_same(const __grid_constant__ PS ps, const __grid_constant__ HoverParams h, const __grid_constant__ QxWaypointParams w,
+                     const __grid_constant__ RngParams rng, float* __restrict__ st, int32_t* __restrict__ ist, float* __restrict__ actions,
+                     float* __restrict__ obs, float* __restrict__ final_obs, float* __restrict__ reward, uint8_t* __restrict__ term,
+                     uint8_t* __restrict__ trunc, uint8_t* __restrict__ info, const float* __restrict__ start_pos,
+                     const float* __restrict__ start_orn, int32_t* __restrict__ cur_count, int32_t* __restrict__ cur_list,
+                     int32_t* __restrict__ next_count, const float* __restrict__ spare, int spare_copy, uint32_t step_seq, int64_t N) {
+  tail_step_same(QwEnv<MODE, false, RANDACT, PS>{ps, h, w, rng}, st, ist, actions, nullptr, obs, final_obs, reward, term, trunc, info, start_pos,
+                 start_orn, cur_count, cur_list, next_count, spare, spare_copy, step_seq, N);
+}
 
 template <int MODE, bool INJECT, class PS>
 __global__ void __launch_bounds__(kBlock)
@@ -309,6 +321,13 @@ static auto qwp_launcher(PfbContext* h, float* actions, const float* noise) {
   return [=](auto v, const TailLaunch& L) -> int {
     using V = decltype(v);
     const int mode = h->hover.flight_mode;
+    if constexpr (V::same) {
+      QX_PARAMS_SWITCH(h, PFB_MODE_SWITCH(mode, (k_qxwp_step_same<MODE, V::randact, PS><<<L.grid, kBlock, 0, L.stream>>>(
+                                                     ps, h->hover, h->qwp, h->rng, h->buf.state, h->buf.istate, actions, h->buf.obs, h->buf.final_obs,
+                                                     h->buf.reward, h->buf.term, h->buf.trunc, h->buf.info, h->buf.start_pos, h->buf.start_orn,
+                                                     L.cur_count, L.cur_list, L.next_count, L.spare, L.spare_copy, L.seq, h->n))));
+      return 0;
+    }
     QX_PARAMS_SWITCH(h, PFB_MODE_SWITCH(mode, (k_qxwp_step<MODE, V::inject, V::randact, V::autoreset, PS><<<L.grid, kBlock, 0, L.stream>>>(
                                                    ps, h->hover, h->qwp, h->rng, h->buf.state, h->buf.istate, actions, noise, h->buf.obs, h->buf.reward,
                                                    h->buf.term, h->buf.trunc, h->buf.info, h->buf.start_pos, h->buf.start_orn, L.prev_count, L.prev_list,

@@ -172,3 +172,72 @@ __device__ __forceinline__ void tail_step(const Env& env, float* __restrict__ st
   if (pl.tail) return;
   obs_write_block<Env::kObsStride>(obs, smem, row_skip, skip, pl.block_first, O, N);
 }
+
+// The step of one launch under SAME_STEP autoreset (PFB_AUTORESET_SAME_STEP): no tail CTAs, every lane owns env
+// block_first + threadIdx.x.  A lane whose env finishes writes the step's outputs from the terminal state as usual and its
+// terminal observation row to final_obs, stores the terminal state, then resets its env in this launch exactly as a tail
+// lane of tail_step would on the next one (the spare record, or the inline reset under the record's episode number, so both
+// modes give episode e of env i the same bits), observes the reset state into obs and appends the env to the done list of
+// this step.  The side-stream rebuild of the consumed spares reads that list; the next step launch waits for it.
+template <class Env>
+__device__ __forceinline__ void tail_step_same(const Env& env, float* __restrict__ st, int32_t* __restrict__ ist, float* __restrict__ actions,
+                                               const float* __restrict__ noise, float* __restrict__ obs, float* __restrict__ final_obs,
+                                               float* __restrict__ reward, uint8_t* __restrict__ term, uint8_t* __restrict__ trunc,
+                                               uint8_t* __restrict__ info, const float* __restrict__ start_pos, const float* __restrict__ start_orn,
+                                               int32_t* __restrict__ cur_count, int32_t* __restrict__ cur_list, int32_t* __restrict__ next_count,
+                                               const float* __restrict__ spare, int spare_copy, uint32_t step_seq, int64_t N) {
+  constexpr int R = Env::kStateRows;
+  static_assert(R + SPARE_TRAILER <= Env::kSpareRows, "spare record too small");
+  __shared__ float smem[kBlock * Env::kObsStride];
+  __shared__ uint8_t row_skip[kBlock];
+  const int O = env.obs_dim();
+  const int64_t block_first = (int64_t)blockIdx.x * kBlock;
+  const int64_t i = block_first + threadIdx.x;
+  if (blockIdx.x == 0 && threadIdx.x == 0) *next_count = 0;  // arm the counter the next launch appends to
+  float* row = smem + threadIdx.x * Env::kObsStride;
+  if (i < N) {
+    typename Env::Item x = env.item(i);
+    typename Env::Regs s;
+    float act[Env::kActions] = {};
+    int step_count = 0;
+    float rew = 0.0f;
+    env.load(st, ist, N, i, s);
+    s.flags &= ~(uint32_t)pfb::FLAG_FRESH_ANY;
+    env.action(actions, i, step_seq, act);
+    env.step(st, ist, noise, N, i, step_seq, act, s, x, step_count, rew);
+    env.observe(st, N, i, act, s, x, row);
+    env.store(st, ist, N, i, s, x, step_count);
+    reward[i] = rew;
+    term[i] = (s.flags & pfb::FLAG_TERM) ? 1 : 0;
+    trunc[i] = (s.flags & pfb::FLAG_TRUNC) ? 1 : 0;
+    if (info) info[i] = env.info(s, x);
+    const bool done = (s.flags & (pfb::FLAG_TERM | pfb::FLAG_TRUNC)) != 0;
+    if (done) {
+      obs_write_row(final_obs, i, O, row);
+      // env.reset(): what a tail lane of tail_step does with this env on the next launch
+      const float* rec = spare + i * Env::kSpareRows;
+      typename Env::Item y = env.item(i);
+      typename Env::Regs r;
+      float zero[Env::kActions] = {};
+      float pose[6];
+#pragma unroll
+      for (int k = 0; k < 3; ++k) { pose[k] = start_pos[3 * i + k]; pose[3 + k] = start_orn[3 * i + k]; }
+      const uint32_t nseq = __float_as_uint(rec[R + SPARE_EPISODE]);
+      bool hit = spare_copy && rec[R + SPARE_VALID] != 0.0f;
+      if (env.pose_keyed()) {
+#pragma unroll
+        for (int k = 0; k < 6; ++k) hit = hit && (rec[R + SPARE_POSE + k] == pose[k]);
+      }
+      if (hit) {
+        env.load_spare(rec, st, ist, N, i, r, y);
+        r.flags = __float_as_uint(rec[R + SPARE_FLAGS]);
+      } else {
+        env.reset(pose, nseq, nullptr, st, N, i, r, y);
+      }
+      env.observe(st, N, i, zero, r, y, row);
+      env.store(st, ist, N, i, r, y, 0);
+    }
+    done_list_append(__activemask(), done, i, cur_count, cur_list);
+  }
+  obs_write_block<Env::kObsStride>(obs, smem, row_skip, i >= N, block_first, O, N);
+}

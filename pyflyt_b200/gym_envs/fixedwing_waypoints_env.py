@@ -41,6 +41,7 @@ class FixedwingWaypointsVecEnv(WaypointsVecEnv):
         device: str | torch.device = "cuda:0",
         env_offset: int = 0,
         inline_reset: bool = False,
+        autoreset_mode: str = "next_step",
     ):
         check_env_args(agent_hz, render_mode, angle_representation)  # fixedwing_base_env.py:47-52
         if flight_mode != 0:
@@ -49,7 +50,7 @@ class FixedwingWaypointsVecEnv(WaypointsVecEnv):
         self.num_targets = int(num_targets)
         cfg = env_config(ENV_FIXEDWING_WAYPOINTS, agent_hz=agent_hz, max_duration_seconds=max_duration_seconds,
                          angle_representation=angle_representation, sparse_reward=sparse_reward, autoreset=autoreset,
-                         flight_dome_size=flight_dome_size, inline_reset=inline_reset, goal_reach_distance=float(goal_reach_distance),
+                         flight_dome_size=flight_dome_size, inline_reset=inline_reset, autoreset_mode=autoreset_mode, goal_reach_distance=float(goal_reach_distance),
                          goal_reach_angle=float("inf"), num_targets=self.num_targets, use_yaw_targets=0)
         sp = np.tile(np.array([[0.0, 0.0, 10.0]]), (self.num_envs, 1))  # fixedwing_waypoints_env.py:63
         so = np.zeros((self.num_envs, 3))

@@ -44,6 +44,7 @@ class QuadXHoverVecEnv(VecEnv):
         device: str | torch.device = "cuda:0",
         env_offset: int = 0,
         inline_reset: bool = False,
+        autoreset_mode: str = "next_step",
     ):
         check_env_args(agent_hz, render_mode, angle_representation)
         if flight_mode < -1 or flight_mode > 7:
@@ -53,7 +54,7 @@ class QuadXHoverVecEnv(VecEnv):
         self.sparse_reward = bool(sparse_reward)
         self.autoreset = bool(autoreset)
         cfg = env_config(ENV_QUADX_HOVER, agent_hz=agent_hz, max_duration_seconds=max_duration_seconds, angle_representation=angle_representation,
-                         sparse_reward=sparse_reward, autoreset=autoreset, flight_dome_size=flight_dome_size, inline_reset=inline_reset,
+                         sparse_reward=sparse_reward, autoreset=autoreset, flight_dome_size=flight_dome_size, inline_reset=inline_reset, autoreset_mode=autoreset_mode,
                          flight_mode=self.flight_mode)
         self.flight_dome_size = cfg.flight_dome_size
         self.max_steps = cfg.max_steps

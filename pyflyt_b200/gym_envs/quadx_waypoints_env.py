@@ -43,6 +43,7 @@ class QuadXWaypointsVecEnv(WaypointsVecEnv):
         device: str | torch.device = "cuda:0",
         env_offset: int = 0,
         inline_reset: bool = False,
+        autoreset_mode: str = "next_step",
     ):
         check_env_args(agent_hz, render_mode, angle_representation)
         if flight_mode < -1 or flight_mode > 7:
@@ -53,7 +54,7 @@ class QuadXWaypointsVecEnv(WaypointsVecEnv):
         self.flight_mode = int(flight_mode)
         cfg = env_config(ENV_QUADX_WAYPOINTS, agent_hz=agent_hz, max_duration_seconds=max_duration_seconds,
                          angle_representation=angle_representation, sparse_reward=sparse_reward, autoreset=autoreset,
-                         flight_dome_size=flight_dome_size, inline_reset=inline_reset, flight_mode=self.flight_mode,
+                         flight_dome_size=flight_dome_size, inline_reset=inline_reset, autoreset_mode=autoreset_mode, flight_mode=self.flight_mode,
                          goal_reach_distance=float(goal_reach_distance), goal_reach_angle=float(goal_reach_angle),
                          num_targets=self.num_targets, use_yaw_targets=int(self.use_yaw_targets))
         sp = np.tile(np.array([[0.0, 0.0, 1.0]]), (self.num_envs, 1))  # quadx_waypoints_env.py:71

@@ -44,6 +44,7 @@ class RocketLandingVecEnv(VecEnv):
         device: str | torch.device = "cuda:0",
         env_offset: int = 0,
         inline_reset: bool = False,
+        autoreset_mode: str = "next_step",
         contact_response: bool = True,
     ):
         """``randomize_drop`` / ``accelerate_drop`` are the reference's ``reset(options=...)`` switches
@@ -54,7 +55,7 @@ class RocketLandingVecEnv(VecEnv):
         self.num_envs = int(num_envs)
         cfg = env_config(ENV_ROCKET_LANDING, agent_hz=agent_hz, max_duration_seconds=max_duration_seconds,
                          angle_representation=angle_representation, sparse_reward=sparse_reward, autoreset=autoreset,
-                         flight_dome_size=float("inf"), inline_reset=inline_reset, ceiling=float(ceiling),
+                         flight_dome_size=float("inf"), inline_reset=inline_reset, autoreset_mode=autoreset_mode, ceiling=float(ceiling),
                          max_displacement=float(max_displacement), randomize_drop=int(bool(randomize_drop)),
                          accelerate_drop=int(bool(accelerate_drop)), contact_response=int(bool(contact_response)))
         sp = np.tile(np.array([[0.0, 0.0, ceiling * 0.9]]), (self.num_envs, 1))  # rocket_landing_env.py:60

@@ -1,7 +1,7 @@
 """gymnasium ``VectorEnv`` facade over the batched envs (SURVEY.md §8f item 2): N reference envs behind the API that
 SB3 / CleanRL-style trainers consume — ``num_envs``, ``single_observation_space`` / ``single_action_space`` and their
 batched versions, ``reset(seed=, options=) -> (obs, info)``, ``step(actions) -> (obs, reward, terminated, truncated, info)``
-with gymnasium's NEXT_STEP autoreset (``metadata["autoreset_mode"]``), ``close()``.
+with gymnasium's NEXT_STEP (default), SAME_STEP or DISABLED autoreset (``metadata["autoreset_mode"]``, per instance), ``close()``.
 
 Tensors are returned ZERO-COPY by default: ``obs``/``reward``/``terminated``/``truncated`` are views of the device buffers the
 CUDA step kernel writes (valid until the next ``step``; clone what you store).  ``output="numpy"`` copies them to the host
@@ -26,9 +26,21 @@ try:  # pragma: no cover - not installable in the build image
     from gymnasium.vector.vector_env import AutoresetMode
 
     _NEXT_STEP = AutoresetMode.NEXT_STEP
+    _MODES = {m.value: m for m in AutoresetMode}
 except Exception:
     _Base = object
     _NEXT_STEP = "NextStep"
+    _MODES = {m: m for m in ("NextStep", "SameStep", "Disabled")}
+# gymnasium's AutoresetMode values -> the batched envs' (autoreset, autoreset_mode) arguments
+_ENV_AUTORESET = {"NextStep": (True, "next_step"), "SameStep": (True, "same_step"), "Disabled": (False, "next_step")}
+
+
+def parse_autoreset_mode(mode) -> str:
+    """gymnasium's ``AutoresetMode`` member or its string value (``"NextStep"``, ``"SameStep"``, ``"Disabled"``) -> the value."""
+    value = getattr(mode, "value", mode)
+    if value not in _ENV_AUTORESET:
+        raise ValueError(f"autoreset_mode must be a gymnasium AutoresetMode or one of {list(_ENV_AUTORESET)}, got {mode!r}")
+    return value
 
 # id stem -> (module, VecEnv class, single-env adaptor module:class)
 ENV_TABLE = {
@@ -58,13 +70,20 @@ class PyFlytVectorEnv(_Base):
     metadata = {"render_modes": [], "autoreset_mode": _NEXT_STEP}
 
     def __init__(self, env_id: str, num_envs: int, output: str = "torch", device: str | torch.device = "cuda:0", seed: int | None = None,
-                 **env_kwargs: Any):
+                 autoreset_mode=_NEXT_STEP, **env_kwargs: Any):
+        """``autoreset_mode``: gymnasium's ``AutoresetMode`` or its string value.  NEXT_STEP (default) and SAME_STEP run the
+        reset inside the step launch; under SAME_STEP ``info["final_obs"]`` / ``info["_final_obs"]`` carry the terminal
+        observations.  DISABLED leaves finished envs alone until ``reset(options={"reset_mask": mask})`` resets the masked ones."""
         if output not in ("torch", "numpy"):
             raise ValueError("output must be 'torch' (zero-copy device tensors) or 'numpy'")
+        mode = parse_autoreset_mode(autoreset_mode)
         mod, cls, _ = ENV_TABLE[_stem(env_id)]
         self.spec_id = env_id
         self.output = output
-        self.env = getattr(__import__(mod, fromlist=[cls]), cls)(num_envs=int(num_envs), seed=seed, autoreset=True, device=device, **env_kwargs)
+        self.metadata = {**type(self).metadata, "autoreset_mode": _MODES[mode]}
+        autoreset, env_mode = _ENV_AUTORESET[mode]
+        self.env = getattr(__import__(mod, fromlist=[cls]), cls)(num_envs=int(num_envs), seed=seed, autoreset=autoreset, autoreset_mode=env_mode,
+                                                                 device=device, **env_kwargs)
         self.num_envs = int(num_envs)
         self.device = self.env.device
         dt = np.float32
@@ -86,7 +105,10 @@ class PyFlytVectorEnv(_Base):
         tests/test_gym_envs.py:92-112 of the reference).  The zero-copy tensors stay the same buffers across a seeded reset."""
         if isinstance(seed, (list, tuple)):
             seed = seed[0]
-        obs, info = self.env.reset(seed=seed)
+        mask = (options or {}).get("reset_mask")
+        if mask is not None:  # gymnasium's DISABLED contract: reset only the masked envs
+            mask = torch.as_tensor(np.asarray(mask) if not torch.is_tensor(mask) else mask, device=self.device).reshape(self.num_envs).bool()
+        obs, info = self.env.reset(seed=seed, mask=mask)
         return self._out(obs), self._info(info)
 
     def step(self, actions):

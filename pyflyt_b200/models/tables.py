@@ -19,6 +19,7 @@ from .urdf import Link, composite_rigid_body, load_urdf_links
 PFB_ABI_VERSION = 1
 KIND_QUADX, KIND_FIXEDWING, KIND_ROCKET = 0, 1, 2
 ENV_NONE, ENV_QUADX_HOVER, ENV_QUADX_WAYPOINTS, ENV_FIXEDWING_WAYPOINTS, ENV_ROCKET_LANDING, ENV_DOGFIGHT, ENV_MA_QUADX_HOVER = range(7)
+AUTORESET_NONE, AUTORESET_NEXT_STEP, AUTORESET_SAME_STEP = range(3)  # PfbEnvConfig.autoreset (PFB_AUTORESET_*)
 MAX_MOTORS, MAX_SURFACES, MAX_SHAPES = 4, 5, 16
 SHAPE_IDS = {"box": 0, "cylinder": 1, "sphere": 2}
 
