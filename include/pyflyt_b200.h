@@ -278,7 +278,7 @@ int pfb_destroy(PfbHandle h);
  * physics substeps u = 0..U-1 for every drone; drone i, with r_i = physics_hz / control_hz_i, runs its control tick before
  * substep u when u % r_i == 0.  Injected noise is [n_steps * U][N] (one draw per drone per substep, whatever its rate);
  * Philox draws are keyed by (seed, i, Aviary step, substep).  If every table has the same control_hz, the flag changes nothing.
- * The handle is an Aviary handle (the env entry points, pfb_set_models and pfb_set_base_velocity refuse it) with:
+ * The handle is an Aviary handle (the env entry points and pfb_set_models refuse it) with:
  *   state     pfb_state_floats() floats, carved by the library into one region per kind (PFB_LAYOUT_BY_KIND): QuadX
  *             warp-tiled, then fixed-wing and rocket field-major, each on a 128-byte boundary; istate [pfb_istate_rows][N];
  *   setpoint  [N][7] (pfb_setpoint_dim): drone i reads its own length (QuadX 4, fixed-wing 6, rocket 7), the rest is zero
@@ -350,9 +350,23 @@ int pfb_set_modes(PfbHandle h, const int8_t* modes, void* stream);
 /* n_steps × Aviary.step() (aviary.py:480-531).  noise: device [n_steps*updates_per_step][N] raw
  * draws of np_random.normal(*throttle.shape) (motors.py:134-138), or NULL → on-device Philox.        */
 int pfb_aviary_step(PfbHandle h, int n_steps, const float* noise, void* stream);
-/* p.resetBaseVelocity for every env (gym_envs/rocket_envs/rocket_base_env.py:228): device [N][3] world-
- * frame linear and angular velocities.                                                                */
+/* p.resetBaseVelocity for every drone (gym_envs/rocket_envs/rocket_base_env.py:228): device [N][3] world-frame linear and
+ * angular velocities, fp32.  Every Aviary handle (single-kind or mixed) and Rocket-Landing handles; the body rate the state
+ * carries is R^T w in fp32.  The other env handles refuse it.                                                              */
 int pfb_set_base_velocity(PfbHandle h, const float* lin_vel, const float* ang_vel, void* stream);
+/* p.resetBasePositionAndOrientation(pos, quat) and / or p.resetBaseVelocity(lin_vel, ang_vel), then drone.update_state(), for
+ * the drones of `mask` (device [N] uint8, NULL = every drone).  Device fp64 arrays in user drone order: pos [N][3], quat
+ * [N][4] (x, y, z, w), lin_vel / ang_vel [N][3], world frame; NULL = not given.  pos and quat come together or not at all.
+ * A pose zeroes both velocities, then the velocities given replace them; an input not given keeps its value.  Position,
+ * quaternion and velocity land in the hi / lo state words; the angular velocity is stored as the body rate R^T w of the
+ * drone's (new) attitude.  Everything else (flags incl. contact, controller memories, actuators, fuel, gimbal, setpoints,
+ * flight modes, model index, step count) is kept.  Aviary handles only (single-kind or mixed): env handles refuse it.      */
+int pfb_set_base_state(PfbHandle h, const uint8_t* mask, const double* pos, const double* quat, const double* lin_vel, const double* ang_vel,
+                       void* stream);
+/* getBasePositionAndOrientation / getBaseVelocity of every drone, in user order, into device fp64 arrays (NULL = not wanted):
+ * pos [N][3], quat [N][4] (x, y, z, w) and lin_vel [N][3] are the hi + lo sums of the state words, ang_vel [N][3] the world
+ * rate R w_body.  Aviary handles only.                                                                                      */
+int pfb_get_base_state(PfbHandle h, double* pos, double* quat, double* lin_vel, double* ang_vel, void* stream);
 /* Fills drone_state / aux_state / contact (Aviary.state(i), aux_state(i), contact_array).            */
 int pfb_observe_state(PfbHandle h, void* stream);
 

@@ -84,6 +84,8 @@ def lib() -> C.CDLL:
     L.pfb_aviary_step.argtypes = [vp, i32, vp, vp]
     L.pfb_observe_state.argtypes = [vp, vp]
     L.pfb_set_base_velocity.argtypes = [vp, vp, vp, vp]
+    L.pfb_set_base_state.argtypes = [vp, vp, vp, vp, vp, vp, vp]
+    L.pfb_get_base_state.argtypes = [vp, vp, vp, vp, vp, vp]
     L.pfb_env_reset.argtypes = [vp, vp, vp, vp]
     L.pfb_env_step.argtypes = [vp, vp, vp, vp]
     L.pfb_env_rollout.argtypes = [vp, i32, vp]
@@ -114,7 +116,7 @@ EXPORTS = [
     "pfb_model_from_files", "pfb_create", "pfb_create_mixed", "pfb_destroy", "pfb_set_env_offset", "pfb_state_rows", "pfb_state_layout", "pfb_state_floats", "pfb_set_noise_dump", "pfb_reseed", "pfb_set_wind", "pfb_sizeof_wind", "pfb_set_models",
     "pfb_istate_rows", "pfb_setpoint_dim",
     "pfb_obs_dim", "pfb_aux_dim", "pfb_bind", "pfb_reset", "pfb_set_mode", "pfb_set_modes", "pfb_aviary_step", "pfb_observe_state",
-    "pfb_set_base_velocity",
+    "pfb_set_base_velocity", "pfb_set_base_state", "pfb_get_base_state",
     "pfb_env_reset", "pfb_env_step", "pfb_env_rollout", "pfb_env_step_host", "pfb_env_step_mapped", "pfb_launch_count",
     "pfb_profile_begin", "pfb_profile_read", "pfb_dogfight_payload_dim", "pfb_dogfight_physics", "pfb_dogfight_physics_peer", "pfb_dogfight_combat", "pfb_dogfight_combat_wait", "pfb_dogfight_split_step",
 ]  # every symbol include/pyflyt_b200.h declares

@@ -4,9 +4,12 @@ Mirrors the surface of the reference's ``Aviary`` that its environments use
 (/root/reference/PyFlyt/core/aviary.py): ctor kwargs ``start_pos``/``start_orn``/``drone_type``/
 ``drone_options``/``seed``/``physics_hz`` (:69-83), ``reset`` (:218), ``step`` (:480), ``state(i)`` (:335),
 ``aux_state(i)`` (:353), ``all_states`` (:372), ``set_mode`` (:440), ``set_setpoint`` (:460),
-``set_all_setpoints`` (:470), ``contact_array`` (:322), counters (:227-229, :528-531) — with one
-difference in meaning: drone ``i`` lives in its OWN world (the reference puts them in one Bullet world),
-so ``contact_array[i]`` is "drone i touched the floor during the last step".
+``set_all_setpoints`` (:470), ``contact_array`` (:322), counters (:227-229, :528-531), and the Bullet client's base-state
+calls that scripts on top of the Aviary use: ``resetBasePositionAndOrientation`` / ``resetBaseVelocity`` followed by
+``drone.update_state()`` (``set_base_state``, ``set_base_velocity``) and ``getBasePositionAndOrientation`` /
+``getBaseVelocity`` (``base_state``), by drone index and mask rather than body id — with one difference in meaning: drone
+``i`` lives in its OWN world (the reference puts them in one Bullet world), so ``contact_array[i]`` is "drone i touched the
+floor during the last step".
 
 ``drone_options`` may be a sequence with one dict per drone, as in the reference (aviary.py:75): a QuadX batch then flies up
 to ``MAX_QUADX_MODELS`` different vehicle tables (``models``), drone ``i`` the table ``model_index[i]``.  All of them run at
@@ -25,8 +28,7 @@ keeps its own kind's surface: ``set_setpoint(i, sp)`` takes drone ``i``'s own se
 rocket 7) and ``state(i)`` / ``aux_state(i)`` return its own aux length (4, 6 or 9); ``setpoints`` is ``[N, 7]`` and
 ``all_aux_states`` a list of ``N`` tensors.  Each kind's drones take their tables from their own ``drone_options`` entries (up
 to ``MAX_QUADX_MODELS`` QuadX models, one fixed-wing and one rocket model), and every drone runs at one ``control_hz`` unless
-``mixed_control_hz=True`` (below).  Such a batch is an Aviary only: no ``env_config``, no ``set_base_velocity``, no
-``state_row``.  Drone ``i`` draws the random stream drone ``i`` of a single-kind batch with the same seed draws, so it flies
+``mixed_control_hz=True`` (below).  Such a batch is an Aviary only: no ``env_config``, no ``state_row``.  Drone ``i`` draws the random stream drone ``i`` of a single-kind batch with the same seed draws, so it flies
 exactly as it would there.
 
 ``mixed_control_hz=True`` lets the drones' ``drone_options`` differ in ``control_hz``, as in the reference's
@@ -332,12 +334,57 @@ class BatchedAviary:
         self._state_fresh = False
 
     def set_base_velocity(self, lin_vel: torch.Tensor, ang_vel: torch.Tensor) -> None:
-        """``p.resetBaseVelocity`` for every drone (used by rocket_base_env.py:228): [N, 3] world-frame tensors."""
-        self._single_kind("set_base_velocity")
+        """``p.resetBaseVelocity`` for every drone (used by rocket_base_env.py:228): [N, 3] world-frame velocities, taken in
+        fp32.  The state then carries the body rate R^T w, computed in fp32.  Like the env scripts that call it, it does not
+        zero anything else; ``set_base_state`` is the fp64, masked form."""
         lin = torch.as_tensor(lin_vel, dtype=torch.float32, device=self.device).reshape(self.num_drones, 3).contiguous()
         ang = torch.as_tensor(ang_vel, dtype=torch.float32, device=self.device).reshape(self.num_drones, 3).contiguous()
         _lib.check(_lib.lib().pfb_set_base_velocity(self._h, C.c_void_p(lin.data_ptr()), C.c_void_p(ang.data_ptr()), self._s()))
         self._state_fresh = False
+
+    def _rows64(self, x, width: int, name: str) -> torch.Tensor | None:
+        if x is None:
+            return None
+        t = torch.as_tensor(x, dtype=torch.float64, device=self.device)
+        if tuple(t.shape) != (self.num_drones, width):
+            raise ValueError(f"{name} must be shape ({self.num_drones}, {width}), got {tuple(t.shape)}.")
+        return t.contiguous()
+
+    def set_base_state(self, pos=None, quat=None, lin_vel=None, ang_vel=None, mask=None) -> None:
+        """``p.resetBasePositionAndOrientation(id, pos, quat)`` and / or ``p.resetBaseVelocity(id, lin_vel, ang_vel)``, then
+        ``drone.update_state()``, for the drones of ``mask`` ([N] bool; None = every drone).  ``pos`` [N, 3], ``quat`` [N, 4]
+        (x, y, z, w, PyBullet's order; unit norm to 1e-6), ``lin_vel`` / ``ang_vel`` [N, 3] in the world frame, numpy or
+        torch, taken in fp64; None = not given.  ``pos`` and ``quat`` come together.  A pose zeroes both velocities, as
+        Bullet's reset does, and the velocities given then replace them; what is not given keeps its value.  Flight modes,
+        setpoints, controller memories, motor throttles, surfaces, fuel, gimbal, model index, step count and the contact flags
+        are kept (DESIGN.md §4g).  Aviary handles only."""
+        if (pos is None) != (quat is None):
+            raise ValueError("pos and quat come together (resetBasePositionAndOrientation sets both) or not at all.")
+        p, q = self._rows64(pos, 3, "pos"), self._rows64(quat, 4, "quat")
+        lv, av = self._rows64(lin_vel, 3, "lin_vel"), self._rows64(ang_vel, 3, "ang_vel")
+        if q is not None:
+            err = float((torch.linalg.vector_norm(q, dim=1) - 1.0).abs().max())
+            if not err <= 1e-6:
+                raise ValueError(f"quat must be unit quaternions (x, y, z, w): a norm differs from 1 by {err:.3g} (> 1e-6).")
+        m = None
+        if mask is not None:
+            m = torch.as_tensor(mask, device=self.device)
+            if tuple(m.shape) != (self.num_drones,):
+                raise ValueError(f"mask must be shape ({self.num_drones},), got {tuple(m.shape)}.")
+            m = m.to(torch.uint8).contiguous()
+        ptr = lambda t: None if t is None else C.c_void_p(t.data_ptr())  # noqa: E731
+        _lib.check(_lib.lib().pfb_set_base_state(self._h, ptr(m), ptr(p), ptr(q), ptr(lv), ptr(av), self._s()))
+        self._state_fresh = False
+
+    def base_state(self) -> tuple[torch.Tensor, torch.Tensor, torch.Tensor, torch.Tensor]:
+        """``getBasePositionAndOrientation`` / ``getBaseVelocity`` of every drone: fp64 device tensors position [N, 3],
+        quaternion [N, 4] (x, y, z, w), world linear velocity [N, 3] (the hi + lo words the kernels carry) and world angular
+        velocity [N, 3] (R w_body).  ``set_base_state(*base_state())`` writes the same state back."""
+        n, f64 = self.num_drones, dict(dtype=torch.float64, device=self.device)
+        pos, quat, lin, ang = torch.empty((n, 3), **f64), torch.empty((n, 4), **f64), torch.empty((n, 3), **f64), torch.empty((n, 3), **f64)
+        _lib.check(_lib.lib().pfb_get_base_state(self._h, C.c_void_p(pos.data_ptr()), C.c_void_p(quat.data_ptr()), C.c_void_p(lin.data_ptr()),
+                                                 C.c_void_p(ang.data_ptr()), self._s()))
+        return pos, quat, lin, ang
 
     def _refresh(self):
         if not self._state_fresh:

@@ -1,7 +1,7 @@
 // pfb_aviary.cuh — the per-drone bodies of the Aviary operations, one per vehicle kind: the step in a per-drone flight mode,
-// the state query, the reset and the per-drone set_mode.  A body works on row j of its kind's state region (QuadX warp-tiled,
-// fixed-wing and rocket field-major [F][n] + istate [I][n]) and takes drone u's setpoint row (SP floats apart), start pose and
-// noise column.  The single-kind kernels call them with j = u = i; the mixed-kind kernels (pfb_mixed.cu) with u = slot_user[j].
+// the state query, the reset, the per-drone set_mode and the base state (set / get).  A body works on row j of its kind's state
+// region (QuadX warp-tiled, fixed-wing and rocket field-major [F][n] + istate [I][n]) and takes drone u's setpoint row (SP floats
+// apart), start pose, noise column or base-state rows.  The single-kind kernels call them with j = u = i; the mixed-kind kernels (pfb_mixed.cu) with u = slot_user[j].
 // Pointers are passed as parameters, not in structs (a __restrict__ member loses its __restrict__), and a table is bound by
 // reference to the kernel's own __grid_constant__ parameter (a copy of it is staged on the stack).
 #pragma once
@@ -152,6 +152,67 @@ __device__ __forceinline__ void rk_reset_drone(const RocketParams& p, float* st,
   rocket_reset(p, s, start_pos[3 * u], start_pos[3 * u + 1], start_pos[3 * u + 2], start_orn[3 * u], start_orn[3 * u + 1], start_orn[3 * u + 2]);
   rocket_store(st, ist, n, j, s);
   ist[(int64_t)RI_STEP * n + j] = 0;
+}
+
+// ---- base state of the drone in row j from / into drone u's rows of the caller's [N][3] / [N][4] arrays (base_state_set,
+// base_state_get: pfb_fixedwing.cuh); nullptr = not given / not wanted.  QuadX: Aviary handles only, so always warp-tiled.
+template <typename T>
+__device__ __forceinline__ void qx_set_base_drone(float* st, int rows, int64_t j, int64_t u, const double* pos, const double* quat, const T* lin,
+                                                  const T* ang) {
+  float* rec = st + qx_tile_base(j, rows);
+  QuadXRegs s;
+  int step_count;
+  quadx_load_tile<7, kTileGroupStride>(rec, s, step_count);  // mode 7 moves every PID row
+  const F4 pwm = ld_f4(rec + 9 * kTileGroupStride);  // the load leaves the last motor command zero: the store puts it back as it was
+  s.pwm[0] = pwm.x; s.pwm[1] = pwm.y; s.pwm[2] = pwm.z; s.pwm[3] = pwm.w;
+  base_state_set<T>(s, pos ? pos + 3 * u : nullptr, quat ? quat + 4 * u : nullptr, lin ? lin + 3 * u : nullptr, ang ? ang + 3 * u : nullptr);
+  quadx_store_tile<7, kTileGroupStride>(rec, s, step_count);
+}
+template <typename T>
+__device__ __forceinline__ void fw_set_base_drone(float* st, int32_t* ist, int64_t n, int64_t j, int64_t u, const double* pos, const double* quat,
+                                                  const T* lin, const T* ang) {
+  FixedwingRegs s;
+  fixedwing_load(st, ist, n, j, s);
+  base_state_set<T>(s, pos ? pos + 3 * u : nullptr, quat ? quat + 4 * u : nullptr, lin ? lin + 3 * u : nullptr, ang ? ang + 3 * u : nullptr);
+  fixedwing_store(st, ist, n, j, s);
+}
+template <typename T>
+__device__ __forceinline__ void rk_set_base_drone(float* st, int32_t* ist, int64_t n, int64_t j, int64_t u, const double* pos, const double* quat,
+                                                  const T* lin, const T* ang) {
+  RocketRegs s;
+  rocket_load(st, ist, n, j, s);
+  base_state_set<T>(s, pos ? pos + 3 * u : nullptr, quat ? quat + 4 * u : nullptr, lin ? lin + 3 * u : nullptr, ang ? ang + 3 * u : nullptr);
+  rocket_store(st, ist, n, j, s);
+}
+__device__ __forceinline__ void qx_get_base_drone(const float* st, int rows, int64_t j, int64_t u, const BaseStateOut& o) {
+  QuadXRegs s;
+  int step_count;
+  quadx_load_tile<-1, kTileGroupStride>(st + qx_tile_base(j, rows), s, step_count);
+  base_state_get(s, o.pos ? o.pos + 3 * u : nullptr, o.quat ? o.quat + 4 * u : nullptr, o.lin ? o.lin + 3 * u : nullptr, o.ang ? o.ang + 3 * u : nullptr);
+}
+__device__ __forceinline__ void fw_get_base_drone(const float* st, const int32_t* ist, int64_t n, int64_t j, int64_t u, const BaseStateOut& o) {
+  FixedwingRegs s;
+  fixedwing_load(st, ist, n, j, s);
+  base_state_get(s, o.pos ? o.pos + 3 * u : nullptr, o.quat ? o.quat + 4 * u : nullptr, o.lin ? o.lin + 3 * u : nullptr, o.ang ? o.ang + 3 * u : nullptr);
+}
+__device__ __forceinline__ void rk_get_base_drone(const float* st, const int32_t* ist, int64_t n, int64_t j, int64_t u, const BaseStateOut& o) {
+  RocketRegs s;
+  rocket_load(st, ist, n, j, s);
+  base_state_get(s, o.pos ? o.pos + 3 * u : nullptr, o.quat ? o.quat + 4 * u : nullptr, o.lin ? o.lin + 3 * u : nullptr, o.ang ? o.ang + 3 * u : nullptr);
+}
+// pfb_set_base_state (fp64) or pfb_set_base_velocity (F32) of the drone in row j of kind KIND's region, drone u's inputs
+template <bool F32>
+__device__ __forceinline__ void set_base_drone(int kind, const BaseStateIn& a, float* st, int32_t* ist, int rows, int64_t n, int64_t j, int64_t u) {
+  if (a.mask && !a.mask[u]) return;
+  if constexpr (F32) {
+    if (kind == 0) qx_set_base_drone<float>(st, rows, j, u, nullptr, nullptr, a.lin32, a.ang32);
+    else if (kind == 1) fw_set_base_drone<float>(st, ist, n, j, u, nullptr, nullptr, a.lin32, a.ang32);
+    else rk_set_base_drone<float>(st, ist, n, j, u, nullptr, nullptr, a.lin32, a.ang32);
+  } else {
+    if (kind == 0) qx_set_base_drone<double>(st, rows, j, u, a.pos, a.quat, a.lin, a.ang);
+    else if (kind == 1) fw_set_base_drone<double>(st, ist, n, j, u, a.pos, a.quat, a.lin, a.ang);
+    else rk_set_base_drone<double>(st, ist, n, j, u, a.pos, a.quat, a.lin, a.ang);
+  }
 }
 
 // ---- Aviary.set_mode(modes[j]) of the drone in row j (quadx.py:233-373): preset the setpoint, fresh attitude / position PIDs --

@@ -30,6 +30,17 @@ struct RngParams {
   uint32_t env_offset_hi;
 };
 
+// pfb_set_base_state / pfb_set_base_velocity / pfb_get_base_state: device arrays in user drone order, [N][3] (quaternions
+// [N][4]); nullptr = not given / not wanted.  lin32 / ang32 are the fp32 velocities of pfb_set_base_velocity (every drone).
+struct BaseStateIn {
+  const uint8_t* mask;  // [N]; nullptr = every drone
+  const double *pos, *quat, *lin, *ang;
+  const float *lin32, *ang32;
+};
+struct BaseStateOut {
+  double *pos, *quat, *lin, *ang;
+};
+
 // ---- mixed-model QuadX handles (pfb_set_models) ------------------------------------------------------------------------
 // The kernels that integrate a QuadX drone take their coefficient table as a template type PS, passed BY VALUE as the
 // __grid_constant__ kernel parameter:
@@ -326,6 +337,9 @@ int qx_set_mode(PfbContext* h, int mode, cudaStream_t s);
 int qx_set_modes(PfbContext* h, cudaStream_t s);  // after d_modes holds the modes
 int qx_aviary_step(PfbContext* h, int n_steps, const float* noise, cudaStream_t s);
 int qx_observe(PfbContext* h, cudaStream_t s);
+// base state (pfb_set_base_state / pfb_set_base_velocity: a.lin32 or a.ang32 set; pfb_get_base_state), Aviary handles: one launch
+int qx_set_base_state(PfbContext* h, const BaseStateIn& a, cudaStream_t s);
+int qx_get_base_state(PfbContext* h, const BaseStateOut& o, cudaStream_t s);
 int hover_spare_rows();     // floats of d_spare per env
 int hover_consumed_rows();  // entries of d_consumed per env
 int hover_env_reset(PfbContext* h, const uint8_t* mask, const float* noise, cudaStream_t s);
@@ -345,6 +359,8 @@ int fw_set_mode(PfbContext* h, int mode, cudaStream_t s);
 int fw_set_modes(PfbContext* h, cudaStream_t s);  // after d_modes holds the modes: zero the setpoints, flag the handle
 int fw_aviary_step(PfbContext* h, int n_steps, const float* noise, cudaStream_t s);
 int fw_observe(PfbContext* h, cudaStream_t s);
+int fw_set_base_state(PfbContext* h, const BaseStateIn& a, cudaStream_t s);
+int fw_get_base_state(PfbContext* h, const BaseStateOut& o, cudaStream_t s);
 int fw_env_reset(PfbContext* h, const uint8_t* mask, const float* noise, cudaStream_t s);
 int fw_env_step(PfbContext* h, float* actions, const float* noise, bool randact, cudaStream_t s);
 int fw_spare_rows();
@@ -356,9 +372,10 @@ int rk_state_rows();
 int rk_istate_rows();
 int rk_obs_dim(const PfbContext* h);
 int rk_reset(PfbContext* h, const uint8_t* mask, cudaStream_t s);
-int rk_set_velocity(PfbContext* h, const float* lin, const float* ang, cudaStream_t s);
 int rk_aviary_step(PfbContext* h, int n_steps, const float* noise, cudaStream_t s);
 int rk_observe(PfbContext* h, cudaStream_t s);
+int rk_set_base_state(PfbContext* h, const BaseStateIn& a, cudaStream_t s);
+int rk_get_base_state(PfbContext* h, const BaseStateOut& o, cudaStream_t s);
 int rk_env_reset(PfbContext* h, const uint8_t* mask, const float* noise, cudaStream_t s);
 int rk_env_step(PfbContext* h, float* actions, const float* noise, bool randact, cudaStream_t s);
 int rk_spare_rows();
@@ -385,6 +402,8 @@ int mx_set_mode(PfbContext* h, int mode, cudaStream_t s);
 int mx_set_modes(PfbContext* h, const int8_t* modes, cudaStream_t s);
 int mx_aviary_step(PfbContext* h, int n_steps, const float* noise, cudaStream_t s);
 int mx_observe(PfbContext* h, cudaStream_t s);
+int mx_set_base_state(PfbContext* h, const BaseStateIn& a, cudaStream_t s);
+int mx_get_base_state(PfbContext* h, const BaseStateOut& o, cudaStream_t s);
 void mx_destroy(PfbContext* h);
 
 // QuadX-Waypoints translation unit (pfb_quadx_wp.cu)

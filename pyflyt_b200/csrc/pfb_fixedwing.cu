@@ -35,6 +35,22 @@ __global__ void __launch_bounds__(kBlock) k_fw_reset(const __grid_constant__ Fix
     for (int k = 0; k < sp_dim; ++k) setpoint[(int64_t)sp_dim * i + k] = 0.0f;
 }
 
+// p.resetBasePositionAndOrientation / p.resetBaseVelocity + update_state (pfb_set_base_state; F32: pfb_set_base_velocity) and
+// getBasePositionAndOrientation / getBaseVelocity (pfb_get_base_state)
+template <bool F32>
+__global__ void __launch_bounds__(kBlock) k_fw_set_base_state(const __grid_constant__ BaseStateIn a, float* __restrict__ st,
+                                                              int32_t* __restrict__ ist, int64_t N) {
+  int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= N) return;
+  set_base_drone<F32>(PFB_KIND_FIXEDWING, a, st, ist, 0, N, i, i);
+}
+__global__ void __launch_bounds__(kBlock) k_fw_get_base_state(const __grid_constant__ BaseStateOut o, const float* __restrict__ st,
+                                                              const int32_t* __restrict__ ist, int64_t N) {
+  int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= N) return;
+  fw_get_base_drone(st, ist, N, i, i, o);
+}
+
 // CONTACT: the ground pushes back (Aviary handles with contact_response)
 template <int MODE, bool INJECT, bool CONTACT>
 __global__ void __launch_bounds__(kBlock, kMinBlocks)
@@ -414,6 +430,19 @@ int fw_aviary_step(PfbContext* h, int n_steps, const float* noise, cudaStream_t 
     else k_fw_aviary_step<-1, false, false><<<g, kBlock, 0, s>>>(FW_ARGS);
   }
 #undef FW_ARGS
+  LAUNCH_CHECK(h);
+  return 0;
+}
+
+int fw_set_base_state(PfbContext* h, const BaseStateIn& a, cudaStream_t s) {
+  if (a.lin32 || a.ang32) k_fw_set_base_state<true><<<grid_for(h->n), kBlock, 0, s>>>(a, h->buf.state, h->buf.istate, h->n);
+  else k_fw_set_base_state<false><<<grid_for(h->n), kBlock, 0, s>>>(a, h->buf.state, h->buf.istate, h->n);
+  LAUNCH_CHECK(h);
+  return 0;
+}
+
+int fw_get_base_state(PfbContext* h, const BaseStateOut& o, cudaStream_t s) {
+  k_fw_get_base_state<<<grid_for(h->n), kBlock, 0, s>>>(o, h->buf.state, h->buf.istate, h->n);
   LAUNCH_CHECK(h);
   return 0;
 }

@@ -413,6 +413,67 @@ PFB_HD void body_update_state(Regs& s) {
   s.vb.z = (float)(R.m02 * vx + R.m12 * vy + R.m22 * vz);
 }
 
+// ---- base state of one drone, any kind (QuadXRegs, FixedwingRegs, RocketRegs) -----------------------------------------------
+// p.resetBasePositionAndOrientation(pos, quat) / p.resetBaseVelocity(lin, ang) followed by drone.update_state().  The pointers are
+// the drone's own rows ([3], quaternion [4] x, y, z, w; world frame); nullptr = not given.  A pose zeroes both velocities (as
+// Bullet's reset does), the velocities given replace them.  The fp64 words are rounded to what the hi + lo state words hold, so
+// the registers equal what a reload of the stored state gives.  The state carries the BODY rate w_b = R^T w of the new attitude.
+// The flags (contact included), controller memories, actuators, fuel, gimbal and step count are kept; update_state's derived
+// values (R, body velocity) are re-derived by every load.
+PFB_HD double hi_lo_round(double d) {
+  float hi, lo;
+  split_hi_lo(d, hi, lo);
+  return join_hi_lo(hi, lo);
+}
+// fp64 world rate (pfb_set_base_state): R^T in fp64 from the drone's quaternion
+template <typename Regs>
+PFB_HD void set_body_rate(Regs& s, const double* w) {
+  Rot<double> R;
+  rot_from_quat<double>(s.qx, s.qy, s.qz, s.qw, R);
+  s.wx = (float)(R.m00 * w[0] + R.m10 * w[1] + R.m20 * w[2]);
+  s.wy = (float)(R.m01 * w[0] + R.m11 * w[1] + R.m21 * w[2]);
+  s.wz = (float)(R.m02 * w[0] + R.m12 * w[1] + R.m22 * w[2]);
+}
+// fp32 world rate (pfb_set_base_velocity): the drone's own R rounded to fp32, fp32 arithmetic
+template <typename Regs>
+PFB_HD void set_body_rate(Regs& s, const float* w) {
+  const float ox = w[0], oy = w[1], oz = w[2];
+  const auto& R = s.R;
+  s.wx = (float)R.m00 * ox + (float)R.m10 * oy + (float)R.m20 * oz;
+  s.wy = (float)R.m01 * ox + (float)R.m11 * oy + (float)R.m21 * oz;
+  s.wz = (float)R.m02 * ox + (float)R.m12 * oy + (float)R.m22 * oz;
+}
+// T = double (pfb_set_base_state) or float (pfb_set_base_velocity: no pose, fp32 velocities widened exactly)
+template <typename T, typename Regs>
+PFB_HD void base_state_set(Regs& s, const double* pos, const double* quat, const T* lin, const T* ang) {
+  if (pos) {
+    s.px = (xreal)hi_lo_round(pos[0]); s.py = (xreal)hi_lo_round(pos[1]); s.pz = (xreal)hi_lo_round(pos[2]);
+    s.qx = (qreal)hi_lo_round(quat[0]); s.qy = (qreal)hi_lo_round(quat[1]); s.qz = (qreal)hi_lo_round(quat[2]); s.qw = (qreal)hi_lo_round(quat[3]);
+    s.vx = s.vy = s.vz = (vreal)0;
+    s.wx = s.wy = s.wz = 0.0f;
+    body_update_state(s);
+  }
+  if (lin) {
+    s.vx = (vreal)hi_lo_round((double)lin[0]); s.vy = (vreal)hi_lo_round((double)lin[1]); s.vz = (vreal)hi_lo_round((double)lin[2]);
+  }
+  if (ang) set_body_rate(s, ang);
+}
+// getBasePositionAndOrientation / getBaseVelocity: the hi + lo sums, and the world rate R w_b in fp64
+template <typename Regs>
+PFB_HD void base_state_get(const Regs& s, double* pos, double* quat, double* lin, double* ang) {
+  if (pos) { pos[0] = (double)s.px; pos[1] = (double)s.py; pos[2] = (double)s.pz; }
+  if (quat) { quat[0] = (double)s.qx; quat[1] = (double)s.qy; quat[2] = (double)s.qz; quat[3] = (double)s.qw; }
+  if (lin) { lin[0] = (double)s.vx; lin[1] = (double)s.vy; lin[2] = (double)s.vz; }
+  if (ang) {
+    Rot<double> R;
+    rot_from_quat<double>(s.qx, s.qy, s.qz, s.qw, R);
+    const double wx = s.wx, wy = s.wy, wz = s.wz;
+    ang[0] = R.m00 * wx + R.m01 * wy + R.m02 * wz;
+    ang[1] = R.m10 * wx + R.m11 * wy + R.m12 * wz;
+    ang[2] = R.m20 * wx + R.m21 * wy + R.m22 * wz;
+  }
+}
+
 // fixedwing.py:229-259: mode 0 = RPYT mixing onto [left ail, right ail, h-tail, v-tail, main wing, motor]
 template <int MODE>
 PFB_HD void fixedwing_command(const FixedwingRegs& s, float* cmd) {

@@ -352,9 +352,47 @@ int pfb_aviary_step(PfbHandle h, int n_steps, const float* noise, void* stream) 
 int pfb_set_base_velocity(PfbHandle h, const float* lin_vel, const float* ang_vel, void* stream) {
   REQUIRE_BOUND(h);
   if (!lin_vel || !ang_vel) return fail("pfb_set_base_velocity: null argument");
-  if (h->mixed) return fail("pfb_set_base_velocity is not available on a mixed-kind handle");
-  if (is_rk(h)) return rk_set_velocity(h, lin_vel, ang_vel, (cudaStream_t)stream);
-  return fail("pfb_set_base_velocity is only built for the rocket (the one vehicle whose env calls resetBaseVelocity)");
+  if (h->env.env_kind != PFB_ENV_NONE && !is_rk(h))  // Rocket-Landing's reset calls it (rocket_base_env.py:228)
+    return fail("pfb_set_base_velocity: only Aviary handles and Rocket-Landing handles; this env builds its autoreset spares from the state");
+  const BaseStateIn a = {nullptr, nullptr, nullptr, nullptr, nullptr, lin_vel, ang_vel};
+  cudaStream_t s = (cudaStream_t)stream;
+  if (h->mixed) return mx_set_base_state(h, a, s);
+  if (is_fw(h)) return fw_set_base_state(h, a, s);
+  if (is_rk(h)) return rk_set_base_state(h, a, s);
+  return qx_set_base_state(h, a, s);
+}
+
+// env handles keep autoreset spares and episode bookkeeping built from the state: their base state is the env's business
+static int require_aviary(PfbHandle h, const char* what) {
+  if (h->env.env_kind != PFB_ENV_NONE)
+    return fail("%s: only Aviary handles; an env handle (env kind %d) builds its autoreset spares from the state", what, h->env.env_kind);
+  return 0;
+}
+
+int pfb_set_base_state(PfbHandle h, const uint8_t* mask, const double* pos, const double* quat, const double* lin_vel, const double* ang_vel,
+                       void* stream) {
+  REQUIRE_BOUND(h);
+  if (require_aviary(h, "pfb_set_base_state")) return -1;
+  if (!pos != !quat) return fail("pfb_set_base_state: pos and quat come together (a pose) or not at all");
+  if (!pos && !lin_vel && !ang_vel) return 0;
+  const BaseStateIn a = {mask, pos, quat, lin_vel, ang_vel, nullptr, nullptr};
+  cudaStream_t s = (cudaStream_t)stream;
+  if (h->mixed) return mx_set_base_state(h, a, s);
+  if (is_fw(h)) return fw_set_base_state(h, a, s);
+  if (is_rk(h)) return rk_set_base_state(h, a, s);
+  return qx_set_base_state(h, a, s);
+}
+
+int pfb_get_base_state(PfbHandle h, double* pos, double* quat, double* lin_vel, double* ang_vel, void* stream) {
+  REQUIRE_BOUND(h);
+  if (require_aviary(h, "pfb_get_base_state")) return -1;
+  if (!pos && !quat && !lin_vel && !ang_vel) return 0;
+  const BaseStateOut o = {pos, quat, lin_vel, ang_vel};
+  cudaStream_t s = (cudaStream_t)stream;
+  if (h->mixed) return mx_get_base_state(h, o, s);
+  if (is_fw(h)) return fw_get_base_state(h, o, s);
+  if (is_rk(h)) return rk_get_base_state(h, o, s);
+  return qx_get_base_state(h, o, s);
 }
 
 int pfb_observe_state(PfbHandle h, void* stream) {

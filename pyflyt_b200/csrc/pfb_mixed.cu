@@ -257,6 +257,28 @@ __global__ void __launch_bounds__(kBlock) k_mixed_set_modes(const __grid_constan
   for (int c = k == 0 ? 4 : (k == 1 ? 0 : 7); c < kMixedSetpointDim; ++c) setpoint[kMixedSetpointDim * u + c] = 0.0f;
 }
 
+// p.resetBasePositionAndOrientation / p.resetBaseVelocity + update_state of the drones of `a.mask` (user order; nullptr = every
+// drone), F32: pfb_set_base_velocity; and getBasePositionAndOrientation / getBaseVelocity of every drone, in user order
+template <bool F32>
+__global__ void __launch_bounds__(kBlock) k_mixed_set_base_state(const __grid_constant__ MixedRows r, const __grid_constant__ BaseStateIn a) {
+  int64_t j;
+  const int k = mixed_row(r, j);
+  if (k < 0) return;
+  const int64_t u = r.slot_user[(k > 0 ? r.n_qx : 0) + (k > 1 ? r.n_fw : 0) + j];
+  if (k == 0) set_base_drone<F32>(0, a, r.qx_st, nullptr, QX_ROWS, r.n_qx, j, u);
+  else if (k == 1) set_base_drone<F32>(1, a, r.fw_st, r.fw_ist, 0, r.n_fw, j, u);
+  else set_base_drone<F32>(2, a, r.rk_st, r.rk_ist, 0, r.n_rk, j, u);
+}
+__global__ void __launch_bounds__(kBlock) k_mixed_get_base_state(const __grid_constant__ MixedRows r, const __grid_constant__ BaseStateOut o) {
+  int64_t j;
+  const int k = mixed_row(r, j);
+  if (k < 0) return;
+  const int64_t u = r.slot_user[(k > 0 ? r.n_qx : 0) + (k > 1 ? r.n_fw : 0) + j];
+  if (k == 0) qx_get_base_drone(r.qx_st, QX_ROWS, j, u, o);
+  else if (k == 1) fw_get_base_drone(r.fw_st, r.fw_ist, r.n_fw, j, u, o);
+  else rk_get_base_drone(r.rk_st, r.rk_ist, r.n_rk, j, u, o);
+}
+
 // ---------------------------------------------------------------------------------------------------
 // host side
 // ---------------------------------------------------------------------------------------------------
@@ -395,6 +417,19 @@ int mx_observe(PfbContext* h, cudaStream_t s) {
   a.contact = h->buf.contact;
   a.pos = h->buf.obs;
   k_mixed_observe<<<grid_all(h->mixed), kBlock, 0, s>>>(a);
+  LAUNCH_CHECK(h);
+  return 0;
+}
+
+int mx_set_base_state(PfbContext* h, const BaseStateIn& a, cudaStream_t s) {
+  if (a.lin32 || a.ang32) k_mixed_set_base_state<true><<<grid_all(h->mixed), kBlock, 0, s>>>(rows_of(h), a);
+  else k_mixed_set_base_state<false><<<grid_all(h->mixed), kBlock, 0, s>>>(rows_of(h), a);
+  LAUNCH_CHECK(h);
+  return 0;
+}
+
+int mx_get_base_state(PfbContext* h, const BaseStateOut& o, cudaStream_t s) {
+  k_mixed_get_base_state<<<grid_all(h->mixed), kBlock, 0, s>>>(rows_of(h), o);
   LAUNCH_CHECK(h);
   return 0;
 }

@@ -100,6 +100,21 @@ __global__ void __launch_bounds__(kBlock) k_quadx_observe(const float* __restric
   if (contact) contact[i] = c ? 1 : 0;
 }
 
+// p.resetBasePositionAndOrientation / p.resetBaseVelocity + update_state (pfb_set_base_state; F32: pfb_set_base_velocity) and
+// getBasePositionAndOrientation / getBaseVelocity (pfb_get_base_state); Aviary handles, warp-tiled
+template <bool F32>
+__global__ void __launch_bounds__(kBlock) k_quadx_set_base_state(const __grid_constant__ BaseStateIn a, float* __restrict__ st, int rows, int64_t N) {
+  int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= N) return;
+  set_base_drone<F32>(PFB_KIND_QUADX, a, st, nullptr, rows, N, i, i);
+}
+__global__ void __launch_bounds__(kBlock) k_quadx_get_base_state(const __grid_constant__ BaseStateOut o, const float* __restrict__ st, int rows,
+                                                                 int64_t N) {
+  int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= N) return;
+  qx_get_base_drone(st, rows, i, i, o);
+}
+
 // ---------------------------------------------------------------------------------------------------
 // kernels — QuadX-Hover env (warp-tiled state)
 // ---------------------------------------------------------------------------------------------------
@@ -1001,6 +1016,19 @@ int qx_aviary_step(PfbContext* h, int n_steps, const float* noise, cudaStream_t 
 int qx_observe(PfbContext* h, cudaStream_t s) {
   if (qx_tiled(h)) k_quadx_observe<true><<<grid_for(h->n), kBlock, 0, s>>>(h->buf.state, h->buf.istate, qx_rows(h), h->buf.drone_state, h->buf.aux_state, h->buf.contact, h->n);
   else k_quadx_observe<false><<<grid_for(h->n), kBlock, 0, s>>>(h->buf.state, h->buf.istate, qx_rows(h), h->buf.drone_state, h->buf.aux_state, h->buf.contact, h->n);
+  LAUNCH_CHECK(h);
+  return 0;
+}
+
+int qx_set_base_state(PfbContext* h, const BaseStateIn& a, cudaStream_t s) {
+  if (a.lin32 || a.ang32) k_quadx_set_base_state<true><<<grid_for(h->n), kBlock, 0, s>>>(a, h->buf.state, qx_rows(h), h->n);
+  else k_quadx_set_base_state<false><<<grid_for(h->n), kBlock, 0, s>>>(a, h->buf.state, qx_rows(h), h->n);
+  LAUNCH_CHECK(h);
+  return 0;
+}
+
+int qx_get_base_state(PfbContext* h, const BaseStateOut& o, cudaStream_t s) {
+  k_quadx_get_base_state<<<grid_for(h->n), kBlock, 0, s>>>(o, h->buf.state, qx_rows(h), h->n);
   LAUNCH_CHECK(h);
   return 0;
 }

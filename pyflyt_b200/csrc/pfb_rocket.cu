@@ -28,21 +28,20 @@ __global__ void __launch_bounds__(kBlock) k_rk_reset(const __grid_constant__ Roc
     for (int k = 0; k < 7; ++k) setpoint[7 * i + k] = 0.0f;
 }
 
-// p.resetBaseVelocity(id, lin, ang) (rocket_base_env.py:228): world-frame velocities -> state rows
-__global__ void __launch_bounds__(kBlock) k_rk_set_velocity(float* __restrict__ st, int32_t* __restrict__ ist, const float* __restrict__ lin,
-                                                            const float* __restrict__ ang, int64_t N) {
+// p.resetBasePositionAndOrientation / p.resetBaseVelocity + update_state (pfb_set_base_state; F32: pfb_set_base_velocity,
+// which rocket_base_env.py:228 calls) and getBasePositionAndOrientation / getBaseVelocity (pfb_get_base_state)
+template <bool F32>
+__global__ void __launch_bounds__(kBlock) k_rk_set_base_state(const __grid_constant__ BaseStateIn a, float* __restrict__ st,
+                                                              int32_t* __restrict__ ist, int64_t N) {
   int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= N) return;
-  RocketRegs s;
-  rocket_load(st, ist, N, i, s);
-  s.vx = (vreal)lin[3 * i]; s.vy = (vreal)lin[3 * i + 1]; s.vz = (vreal)lin[3 * i + 2];
-  // the state carries the BODY rate: w_b = R^T w_world
-  float ox = ang[3 * i], oy = ang[3 * i + 1], oz = ang[3 * i + 2];
-  const Rot<rreal>& R = s.R;
-  s.wx = (float)R.m00 * ox + (float)R.m10 * oy + (float)R.m20 * oz;
-  s.wy = (float)R.m01 * ox + (float)R.m11 * oy + (float)R.m21 * oz;
-  s.wz = (float)R.m02 * ox + (float)R.m12 * oy + (float)R.m22 * oz;
-  rocket_store(st, ist, N, i, s);
+  set_base_drone<F32>(PFB_KIND_ROCKET, a, st, ist, 0, N, i, i);
+}
+__global__ void __launch_bounds__(kBlock) k_rk_get_base_state(const __grid_constant__ BaseStateOut o, const float* __restrict__ st,
+                                                              const int32_t* __restrict__ ist, int64_t N) {
+  int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= N) return;
+  rk_get_base_drone(st, ist, N, i, i, o);
 }
 
 template <bool INJECT>
@@ -328,8 +327,15 @@ int rk_reset(PfbContext* h, const uint8_t* mask, cudaStream_t s) {
   return 0;
 }
 
-int rk_set_velocity(PfbContext* h, const float* lin, const float* ang, cudaStream_t s) {
-  k_rk_set_velocity<<<grid_for(h->n), kBlock, 0, s>>>(h->buf.state, h->buf.istate, lin, ang, h->n);
+int rk_set_base_state(PfbContext* h, const BaseStateIn& a, cudaStream_t s) {
+  if (a.lin32 || a.ang32) k_rk_set_base_state<true><<<grid_for(h->n), kBlock, 0, s>>>(a, h->buf.state, h->buf.istate, h->n);
+  else k_rk_set_base_state<false><<<grid_for(h->n), kBlock, 0, s>>>(a, h->buf.state, h->buf.istate, h->n);
+  LAUNCH_CHECK(h);
+  return 0;
+}
+
+int rk_get_base_state(PfbContext* h, const BaseStateOut& o, cudaStream_t s) {
+  k_rk_get_base_state<<<grid_for(h->n), kBlock, 0, s>>>(o, h->buf.state, h->buf.istate, h->n);
   LAUNCH_CHECK(h);
   return 0;
 }

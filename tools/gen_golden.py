@@ -762,6 +762,119 @@ def ground_fixtures():
         fb.World.contact_response = False
 
 
+def fly_base_state(name, drone_type, drone_options, start_pos, start_orn, modes, setpoints, resets, n_steps, seed):
+    """Aviary-level flight of ``drone_type`` (a list, one reference Aviary) with base-state resets between ``aviary.step()``
+    calls, as a script on top of the Aviary does them: ``resets`` = {step: dict(mask=[n], pos=[n][3], orn=[n][3] Euler, lin=[n][3],
+    ang=[n][3])} (keys absent = not given) are applied before that step with ``resetBasePositionAndOrientation`` (then
+    ``resetBaseVelocity`` with whatever velocities are given) and ``drones[i].update_state()`` for every masked drone.
+    ``modes``: [n] flight modes set once; ``setpoints``: {step: [n] per-drone setpoints} applied with ``set_all_setpoints``.
+    The npz stores the reset steps, masks and values (quaternions, x y z w), and per step the states, aux states (padded to 9),
+    contact flags and raw base states.  Named base_state_* so that no other replay's glob picks it up."""
+    n = len(drone_type)
+    rng = ril.ScriptedNoise(seed)
+    env = Aviary(start_pos=np.array(start_pos, dtype=np.float64), start_orn=np.array(start_orn, dtype=np.float64), drone_type=list(drone_type),
+                 drone_options=[dict(d) for d in drone_options], np_random=rng)
+    env.set_mode([int(m) for m in modes])
+    R = len(resets)
+    r_steps = np.array(sorted(resets), dtype=np.int64)
+    r_mask, r_has = np.zeros((R, n), dtype=np.uint8), np.zeros((R, 3), dtype=bool)  # has: pose, lin, ang
+    r_pos, r_quat, r_lin, r_ang = np.zeros((R, n, 3)), np.zeros((R, n, 4)), np.zeros((R, n, 3)), np.zeros((R, n, 3))
+    r_quat[..., 3] = 1.0
+    states, auxs, contacts, raws, sps = [], [], [], [], []
+    for i in range(n_steps):
+        if i in setpoints:
+            env.set_all_setpoints([np.array(r, dtype=np.float64) for r in setpoints[i]])
+        if i in resets:
+            k, ev = int(np.searchsorted(r_steps, i)), resets[i]
+            r_mask[k] = ev["mask"]
+            r_has[k] = ["pos" in ev, "lin" in ev, "ang" in ev]
+            for d in np.flatnonzero(r_mask[k]):
+                drone = env.drones[d]
+                if "pos" in ev:
+                    r_pos[k, d] = ev["pos"][d]
+                    r_quat[k, d] = env.getQuaternionFromEuler(ev["orn"][d])
+                    env.resetBasePositionAndOrientation(drone.Id, r_pos[k, d], r_quat[k, d])
+                if "lin" in ev or "ang" in ev:
+                    r_lin[k, d] = ev["lin"][d] if "lin" in ev else 0.0
+                    r_ang[k, d] = ev["ang"][d] if "ang" in ev else 0.0
+                    env.resetBaseVelocity(drone.Id, r_lin[k, d] if "lin" in ev else None, r_ang[k, d] if "ang" in ev else None)
+                drone.update_state()
+        sps.append(_padded_rows([d.setpoint for d in env.drones], 7))
+        env.step()
+        states.append(np.array([d.state for d in env.drones]))
+        auxs.append(_padded_rows([d.aux_state for d in env.drones], 9))
+        contacts.append(np.array([bool(env.contact_array[env.planeId, d.Id]) for d in env.drones]))
+        raws.append(np.array([np.concatenate([*env.getBasePositionAndOrientation(d.Id), *env.getBaseVelocity(d.Id)]) for d in env.drones]))
+    noise = np.array(rng.normal_log)
+    assert noise.size == n_steps * int(env.updates_per_step) * n, (noise.size, n_steps, n)
+    np.savez_compressed(
+        os.path.join(OUT, f"{name}.npz"),
+        kind="base_state",
+        drone_type=json.dumps(list(drone_type)),
+        n_drones=n,
+        drone_options=json.dumps(drone_options),
+        start_pos=np.array(start_pos, dtype=np.float64),
+        start_orn=np.array(start_orn, dtype=np.float64),
+        modes=np.array(modes, dtype=np.int64),
+        contact_response=bool(__import__("pybullet").World.contact_response),
+        reset_steps=r_steps, reset_mask=r_mask, reset_has=r_has, reset_pos=r_pos, reset_quat=r_quat, reset_lin=r_lin, reset_ang=r_ang,
+        setpoints=np.array(sps),
+        noise=noise,
+        state=np.array(states),
+        aux=np.array(auxs),
+        contact=np.array(contacts),
+        raw=np.array(raws),
+    )
+    print(name, "final pos", np.array(states[-1])[:, 3], "contacts", int(np.sum(contacts)), "draws", noise.size)
+
+
+def base_state_fixtures():
+    """Scripts that move drones by hand between Aviary steps (resetBasePositionAndOrientation / resetBaseVelocity +
+    update_state, as rocket_base_env.py:228 and custom task code do), replayed by BatchedAviary.set_base_state."""
+    import pybullet as fb  # oracle/fakebullet
+
+    cf2x, prim = dict(drone_model="cf2x"), dict(drone_model="primitive_drone")
+    # 1. two QuadX holding (0, 0, 2) in mode 7: one teleported far away and tilted, the other thrown; the PIDs recover with
+    #    their memories intact
+    hold = {0: [[0.0, 0.0, 0.0, 2.0]] * 2}
+    fly_base_state("base_state_quadx", ["quadx", "quadx"], [cf2x, prim], [[0.0, 0.0, 2.0]] * 2, [[0.05, -0.05, 0.2], [-0.04, 0.03, -0.1]], [7, 7], hold,
+                   {100: dict(mask=[1, 0], pos=[[6.0, -4.0, 9.0], [0.0] * 3], orn=[[0.5, -0.35, 1.0], [0.0] * 3]),
+                    200: dict(mask=[0, 1], lin=[[0.0] * 3, [4.0, 0.0, 3.0]], ang=[[0.0] * 3, [2.0, -1.0, 0.5]])}, 300, seed=401)
+    # 2. fixed-wing and acrowing in mode 0, relaunched at 40 m, yaw 1.2, with 20 m/s along the new heading
+    for model, sd in (("fixedwing", 402), ("acrowing", 403)):
+        relaunch = dict(mask=[1], pos=[[0.0, 0.0, 40.0]], orn=[[0.0, 0.0, 1.2]], lin=[[20.0 * np.cos(1.2), 20.0 * np.sin(1.2), 0.0]])
+        fly_base_state(f"base_state_{model}", ["fixedwing"], [dict(drone_model=model)], [[0.0, 0.0, 30.0]], [[0.0, 0.05, 0.0]], [0],
+                       {0: [[0.0, 0.1, 0.0, 0.7]], 200: [[0.2, -0.1, 0.1, 0.5]]}, {150: relaunch}, 300, seed=sd)
+    # 3. a rocket dropping from 200 m, re-posed upright at 100 m, given (3, -2, -30) m/s and a spin in the same call
+    fly_base_state("base_state_rocket", ["rocket"], [dict(drone_model="rocket")], [[0.0, 0.0, 200.0]], [[0.3, -0.2, 0.1]], [0],
+                   {0: [[0.2, -0.1, 0.1, 1.0, 0.4, 0.1, -0.1]]},
+                   {100: dict(mask=[1], pos=[[5.0, -3.0, 100.0]], orn=[[0.0, 0.0, 0.4]], lin=[[3.0, -2.0, -30.0]], ang=[[0.5, -0.3, 1.0]])}, 300, seed=404)
+    # 4. with the contact response, one drone per reference Aviary (as the ground_* fixtures): at rest on the floor, lifted and
+    #    tilted by a pose reset, falls and lands again.  The rocket is lifted upright and turned: tilted, it rocks on its legs
+    #    for longer than the fixture lasts
+    fb.World.contact_response = True
+    try:
+        fly_base_state("base_state_ground_cf2x", ["quadx"], [cf2x], [[0.0, 0.0, 0.01]], [[0.0, 0.0, 0.0]], [-1], {0: [[0.0] * 4]},
+                       {120: dict(mask=[1], pos=[[0.5, -0.3, 1.2]], orn=[[0.4, -0.2, 0.8]])}, 480, seed=405)
+        fly_base_state("base_state_ground_fixedwing", ["fixedwing"], [dict(drone_model="fixedwing")], [[0.0, 0.0, 0.5]], [[0.0, 0.0, 0.0]], [0],
+                       {0: [[0.0, 0.0, 0.0, 0.0]]}, {200: dict(mask=[1], pos=[[2.0, 1.0, 2.5]], orn=[[0.25, 0.15, 0.5]])}, 720, seed=406)
+        fly_base_state("base_state_ground_rocket", ["rocket"], [dict(drone_model="rocket")], [[0.0, 0.0, 3.0]], [[0.0, 0.0, 0.0]], [0], {0: [[0.0] * 7]},
+                       {150: dict(mask=[1], pos=[[1.0, -1.0, 2.9]], orn=[[0.0, 0.0, 0.3]])}, 450, seed=407)
+    finally:
+        fb.World.contact_response = False
+    # 5. one Aviary of four kinds, no floor contact: only drones 1 and 3 reset at step 80 (pose and both velocities)
+    kinds = ["quadx", "fixedwing", "rocket", "quadx"]
+    opts = [cf2x, dict(drone_model="fixedwing"), dict(drone_model="rocket"), prim]
+    pos = [[0.0, 0.0, 20.0], [12.0, 0.0, 60.0], [24.0, 0.0, 150.0], [36.0, 0.0, 30.0]]
+    orn = [[0.05, -0.04, 0.2], [0.0, 0.05, 0.0], [np.pi / 2, 0.0, 0.2], [-0.03, 0.02, 0.4]]
+    sp = {0: [[0.0, 0.0, 0.0, 20.0], [0.1, 0.1, 0.0, 0.7], [0.2, -0.2, 0.1, 1.0, 0.5, 0.1, 0.1], [36.0, 0.0, 0.3, 30.0]]}
+    z3 = [0.0] * 3
+    fly_base_state("base_state_mixed", kinds, opts, pos, orn, [7, 0, 0, 7], sp,
+                   {80: dict(mask=[0, 1, 0, 1], pos=[z3, [10.0, 5.0, 70.0], z3, [33.0, -2.0, 25.0]], orn=[z3, [0.0, 0.05, -0.7], z3, [0.3, 0.1, 0.5]],
+                             lin=[z3, [18.0 * np.cos(-0.7), 18.0 * np.sin(-0.7), 0.0], z3, [1.0, -2.0, 0.5]], ang=[z3, [0.1, 0.0, 0.0], z3, [0.5, 0.2, -0.3]])},
+                   200, seed=408)
+
+
 def fly_dogfight(name, seed, n_steps, action_seed, team_size=1, sparse=False, action_scale=0.6, lethal_distance=20.0, lethal_angle=0.07,
                  spawn_min_radius=10.0, spawn_max_radius=50.0, damage_per_hit=0.003, pitch_bias=0.0):
     """MAFixedwingDogfightEnv (pz_envs/fixedwing_envs/ma_fixedwing_dogfight_env.py) with scripted actions; a new
@@ -1137,3 +1250,5 @@ if __name__ == "__main__":
         mixed_kind_fixtures()
     if which in ("all", "rates"):
         rate_fixtures()
+    if which in ("all", "basestate"):
+        base_state_fixtures()
