@@ -110,6 +110,7 @@ struct PfbContext {
   int8_t* d_modes;
   // mixed-kind Aviary handle (pfb_create_mixed, pfb_mixed.cu): the drones of each kind and their slots; nullptr = one kind
   struct MixedKinds* mixed;
+  const struct HandleOps* ops;  // what the handle's kind runs, set once at creation
 };
 
 // The device lookup, then a zeroed handle for n drones / envs on `device` with its Philox key and counters, which `setup(c)`
@@ -188,10 +189,6 @@ static inline int grid_for(int64_t n) { return (int)((n + kBlock - 1) / kBlock);
 // An Aviary handle (no env epilogue) whose config asked for the contact RESPONSE: the QuadX and fixed-wing Aviary steps run
 // their CONTACT instantiations.  The rocket carries the switch in RocketParams.contact_response; env handles ignore it.
 static inline bool aviary_contact_response(const PfbContext* h) { return h->env.env_kind == PFB_ENV_NONE && h->env.contact_response != 0; }
-
-// QuadX state layout: warp-tiled (pfb_quadx.cuh) on every QuadX handle except QuadX-Waypoints (field-major rows + istate)
-static inline bool qx_tiled(const PfbContext* h) { return h->model.kind == PFB_KIND_QUADX && h->env.env_kind != PFB_ENV_QUADX_WAYPOINTS; }
-static inline int qx_rows(const PfbContext* h) { return h->env.env_kind == PFB_ENV_MA_QUADX_HOVER ? (int)pfb::QM_ROWS : (int)pfb::QX_ROWS; }
 
 // per-step bookkeeping shared by every env kind (rotating counters and lists, tail CTAs)
 struct StepPlan {
@@ -331,86 +328,77 @@ int tail_env_reset(PfbContext* h, const uint8_t* mask, cudaStream_t s, Reset&& r
   return 0;
 }
 
-// QuadX translation unit (pfb_quadx.cu): Aviary surface, QuadX-Hover and MAQuadXHover
+// ---- what a handle runs: one constant table per handle kind, which pfb_create picks by (vehicle kind, env kind) and
+// pfb_create_mixed sets; the C-ABI entry points check their arguments and call through PfbContext::ops
+struct HandleOps {
+  int kind, env_kind;  // the pair pfb_create looks the table up by (the mixed table: -1, PFB_ENV_NONE)
+  // buffer shape: pfb_state_rows, pfb_istate_rows, pfb_state_layout, pfb_setpoint_dim, pfb_aux_dim, pfb_obs_dim
+  int state_rows, istate_rows, layout, setpoint_dim, aux_dim;
+  int (*obs_dim)(const PfbContext* h);
+  // the mixed table: rows and floats of the kinds present, in place of state_rows, istate_rows and the layout's float count
+  int (*mixed_state_rows)(const PfbContext* h);
+  int (*mixed_istate_rows)(const PfbContext* h);
+  int64_t (*mixed_state_floats)(const PfbContext* h);
+  // Aviary surface: every handle has reset, set_mode (which checks `mode` against the kind's range), aviary_step and observe
+  int (*reset)(PfbContext* h, const uint8_t* mask, cudaStream_t s);
+  int (*set_mode)(PfbContext* h, int mode, cudaStream_t s);
+  // pfb_set_modes with modes that differ, on an Aviary handle: a single-kind table runs once d_modes holds the checked modes; the
+  // mixed table checks `modes` against each drone's kind itself.  nullptr = every mode list of the kind is uniform (rocket)
+  int (*set_modes)(PfbContext* h, const int8_t* modes, cudaStream_t s);
+  int (*aviary_step)(PfbContext* h, int n_steps, const float* noise, cudaStream_t s);
+  int (*observe)(PfbContext* h, cudaStream_t s);
+  // base state: a.lin32 / a.ang32 set = pfb_set_base_velocity, which every table with set_base_state accepts (Aviary handles,
+  // and Rocket-Landing, whose reset calls it: rocket_base_env.py:228); the other env handles have neither
+  int (*set_base_state)(PfbContext* h, const BaseStateIn& a, cudaStream_t s);
+  int (*get_base_state)(PfbContext* h, const BaseStateOut& o, cudaStream_t s);
+  // env epilogue, nullptr on Aviary handles.  `dyn_smem`: dynamic shared memory the step launch requests and never touches
+  // (pfb_env_step_mapped; only QuadX-Hover's step honours it, 0 = every CTA resident in one wave)
+  int (*env_reset)(PfbContext* h, const uint8_t* mask, const float* noise, cudaStream_t s);
+  int (*env_step)(PfbContext* h, float* actions, const float* noise, bool randact, size_t dyn_smem, cudaStream_t s);
+  int (*env_rollout)(PfbContext* h, int n_steps, cudaStream_t s);  // nullptr = n_steps env_step calls with on-device actions
+  // autoreset spares: floats of d_spare per env, offset of a record's valid word (tail-CTA kinds), entries of d_consumed per env
+  // (QuadX-Hover builds spares inside its step launches; 0 = rebuilt on the side stream); a wind change runs invalidate_spares
+  int spare_rows, spare_valid_row, consumed_rows;
+  int (*invalidate_spares)(PfbContext* h, cudaStream_t s);
+};
+
+// invalidate_spares of the tail-CTA kinds: every record is marked invalid, so each env's next reset integrates its warm-up inline
+inline int tail_invalidate_spares(PfbContext* h, cudaStream_t s) {
+  CUDA_OK(cudaMemset2DAsync(h->d_spare + h->ops->spare_valid_row, (size_t)h->ops->spare_rows * sizeof(float), 0, sizeof(float), (size_t)h->n, s));
+  return 0;
+}
+
+// QuadX translation unit (pfb_quadx.cu): the Aviary surface, which the QuadX-Waypoints table (pfb_quadx_wp.cu) points at too
 int qx_reset(PfbContext* h, const uint8_t* mask, cudaStream_t s);
 int qx_set_mode(PfbContext* h, int mode, cudaStream_t s);
-int qx_set_modes(PfbContext* h, cudaStream_t s);  // after d_modes holds the modes
 int qx_aviary_step(PfbContext* h, int n_steps, const float* noise, cudaStream_t s);
 int qx_observe(PfbContext* h, cudaStream_t s);
-// base state (pfb_set_base_state / pfb_set_base_velocity: a.lin32 or a.ang32 set; pfb_get_base_state), Aviary handles: one launch
-int qx_set_base_state(PfbContext* h, const BaseStateIn& a, cudaStream_t s);
-int qx_get_base_state(PfbContext* h, const BaseStateOut& o, cudaStream_t s);
-int hover_spare_rows();     // floats of d_spare per env
-int hover_consumed_rows();  // entries of d_consumed per env
-int hover_env_reset(PfbContext* h, const uint8_t* mask, const float* noise, cudaStream_t s);
-// `dyn_smem`: dynamic shared memory the step launch requests and never touches (pfb_env_step_mapped; 0 = every CTA resident in one wave)
-int hover_env_step(PfbContext* h, float* actions, const float* noise, bool randact, size_t dyn_smem, cudaStream_t s);
-int hover_env_rollout(PfbContext* h, int n_steps, cudaStream_t s);  // n_steps env steps with on-device actions, fused where it can
-// with the device idle: finish the half-built spares, empty their queue and mark every spare record invalid (pfb_set_wind)
-int hover_invalidate_spares(PfbContext* h, cudaStream_t s);
 
-// fixedwing translation unit (pfb_fixedwing.cu)
+// fixedwing translation unit (pfb_fixedwing.cu): the parameter tables, and the Aviary surface, which the Dogfight table
+// (pfb_dogfight.cu) points at too
 int fw_build_params(const PfbModel& m, const PfbEnvConfig* env, pfb::FixedwingParams& p, pfb::WaypointParams& w);
-int fw_state_rows();
-int fw_istate_rows();
-int fw_obs_dim(const PfbContext* h);
 int fw_reset(PfbContext* h, const uint8_t* mask, cudaStream_t s);
 int fw_set_mode(PfbContext* h, int mode, cudaStream_t s);
-int fw_set_modes(PfbContext* h, cudaStream_t s);  // after d_modes holds the modes: zero the setpoints, flag the handle
 int fw_aviary_step(PfbContext* h, int n_steps, const float* noise, cudaStream_t s);
 int fw_observe(PfbContext* h, cudaStream_t s);
-int fw_set_base_state(PfbContext* h, const BaseStateIn& a, cudaStream_t s);
-int fw_get_base_state(PfbContext* h, const BaseStateOut& o, cudaStream_t s);
-int fw_env_reset(PfbContext* h, const uint8_t* mask, const float* noise, cudaStream_t s);
-int fw_env_step(PfbContext* h, float* actions, const float* noise, bool randact, cudaStream_t s);
-int fw_spare_rows();
-int fw_spare_valid_row();  // float offset of the valid word in a spare record
 
 // rocket translation unit (pfb_rocket.cu)
 int rk_build_params(const PfbModel& m, const PfbEnvConfig* env, pfb::RocketParams& p, pfb::LandingParams& l);
-int rk_state_rows();
-int rk_istate_rows();
-int rk_obs_dim(const PfbContext* h);
-int rk_reset(PfbContext* h, const uint8_t* mask, cudaStream_t s);
-int rk_aviary_step(PfbContext* h, int n_steps, const float* noise, cudaStream_t s);
-int rk_observe(PfbContext* h, cudaStream_t s);
-int rk_set_base_state(PfbContext* h, const BaseStateIn& a, cudaStream_t s);
-int rk_get_base_state(PfbContext* h, const BaseStateOut& o, cudaStream_t s);
-int rk_env_reset(PfbContext* h, const uint8_t* mask, const float* noise, cudaStream_t s);
-int rk_env_step(PfbContext* h, float* actions, const float* noise, bool randact, cudaStream_t s);
-int rk_spare_rows();
-int rk_spare_valid_row();  // float offset of the valid word in a spare record
 
 // dogfight translation unit (pfb_dogfight.cu): fixedwing vehicles, arenas of 2*team_size adjacent envs
 int df_build_params(const PfbEnvConfig* env, pfb::DogfightParams& d);
-int df_obs_dim(const PfbContext* h);
-int df_env_reset(PfbContext* h, const uint8_t* mask, const float* noise, cudaStream_t s);
-int df_env_step(PfbContext* h, float* actions, const float* noise, bool randact, cudaStream_t s);
-int df_spare_rows();
-int df_spare_valid_row();  // float offset of the valid word in a spare record
 int df_split_physics(PfbContext* h, const float* actions, const float* noise, float* payload, const uint64_t* peers, int world, int64_t slot0,
                      const uint64_t* peer_flags, int rank, int epoch, int first, int do_reset, int sub, cudaStream_t s);
 int df_split_combat(PfbContext* h, const float* table, int64_t first_gid, int64_t num_arenas, int last, const int* wait_flags, int world, int epoch,
                     cudaStream_t s);
 
-// mixed-kind Aviary handles (pfb_mixed.cu): what the C-ABI entry points run when h->mixed is set
-int mx_state_rows(const PfbContext* h);
-int mx_istate_rows(const PfbContext* h);
-int64_t mx_state_floats(const PfbContext* h);
-int mx_reset(PfbContext* h, const uint8_t* mask, cudaStream_t s);
-int mx_set_mode(PfbContext* h, int mode, cudaStream_t s);
-int mx_set_modes(PfbContext* h, const int8_t* modes, cudaStream_t s);
-int mx_aviary_step(PfbContext* h, int n_steps, const float* noise, cudaStream_t s);
-int mx_observe(PfbContext* h, cudaStream_t s);
-int mx_set_base_state(PfbContext* h, const BaseStateIn& a, cudaStream_t s);
-int mx_get_base_state(PfbContext* h, const BaseStateOut& o, cudaStream_t s);
+// mixed-kind Aviary handles (pfb_mixed.cu)
 void mx_destroy(PfbContext* h);
 
-// QuadX-Waypoints translation unit (pfb_quadx_wp.cu)
-int qwp_state_rows();
-int qwp_istate_rows();
-int qwp_obs_dim(const PfbContext* h);
-int qwp_spare_rows();
-int qwp_spare_valid_row();  // float offset of the valid word in a spare record
-int qwp_env_reset(PfbContext* h, const uint8_t* mask, const float* noise, cudaStream_t s);
-int qwp_env_step(PfbContext* h, float* actions, const float* noise, bool randact, cudaStream_t s);
+// the tables of the handle kinds, each next to the code it points at
+extern const HandleOps kQuadXAviaryOps, kHoverOps, kMAQuadXHoverOps;  // pfb_quadx.cu
+extern const HandleOps kQuadXWaypointsOps;                            // pfb_quadx_wp.cu
+extern const HandleOps kFixedwingAviaryOps, kFixedwingWaypointsOps;   // pfb_fixedwing.cu
+extern const HandleOps kDogfightOps;                                  // pfb_dogfight.cu
+extern const HandleOps kRocketAviaryOps, kRocketLandingOps;           // pfb_rocket.cu
+extern const HandleOps kMixedOps;                                     // pfb_mixed.cu

@@ -47,7 +47,7 @@ int df_build_params(const PfbEnvConfig* env, DogfightParams& d) {
   d.spawn_max_radius = (float)env->spawn_max_radius;
   return 0;
 }
-int df_obs_dim(const PfbContext* h) { return 23 + 14 * (2 * h->df.team_size - 1); }
+static int df_obs_dim(const PfbContext* h) { return 23 + 14 * (2 * h->df.team_size - 1); }
 
 // spare post-reset states (the QuadX-Hover reset pipeline, DESIGN.md §4): one env-major record of 160 floats per AGENT —
 // the FW_* / DF_* state words, received-hits counter, validity, flags, episode number, and the agent's first observation
@@ -55,8 +55,6 @@ int df_obs_dim(const PfbContext* h) { return 23 + 14 * (2 * h->df.team_size - 1)
 enum { DSP_HITS = FW_ROWS, DSP_VALID = FW_ROWS + 1, DSP_FLAGS = FW_ROWS + 2, DSP_EPISODE = FW_ROWS + 3, DSP_OBS = 64, DSP_ROWS = 160 };
 static_assert(FW_ROWS + 4 <= DSP_OBS && DSP_OBS + 23 + 14 * 3 <= DSP_ROWS, "spare record too small");
 constexpr int kDfObsPast = 19;  // index of past_actions inside the observation (3 + 3 + 3 + 3 + 5 + 1 + 1)
-int df_spare_rows() { return DSP_ROWS; }
-int df_spare_valid_row() { return DSP_VALID; }
 
 struct DfAgent {
   float health, acc_reward;
@@ -461,7 +459,7 @@ static auto df_launcher(PfbContext* h, float* actions, const float* noise) {
   };
 }
 
-int df_env_reset(PfbContext* h, const uint8_t* mask, const float* noise, cudaStream_t s) {
+static int df_env_reset(PfbContext* h, const uint8_t* mask, const float* noise, cudaStream_t s) {
   const uint32_t seq = 0x80000000u | (uint32_t)h->reset_seq++;
   const int A = 2 * h->df.team_size;
   if (h->n % A) return fail("the number of envs (%lld) must be a multiple of the arena size %d", (long long)h->n, A);
@@ -478,11 +476,22 @@ int df_env_reset(PfbContext* h, const uint8_t* mask, const float* noise, cudaStr
   return 0;
 }
 
-int df_env_step(PfbContext* h, float* actions, const float* noise, bool randact, cudaStream_t s) {
+static int df_env_step(PfbContext* h, float* actions, const float* noise, bool randact, size_t, cudaStream_t s) {
   const int A = 2 * h->df.team_size;
   if (h->n % A) return fail("the number of envs (%lld) must be a multiple of the arena size %d", (long long)h->n, A);
   return tail_env_step(h, noise, randact, s, df_launcher(h, actions, noise));
 }
+
+// the fixed-wing Aviary surface (pfb_fixedwing.cu) over the FW_* rows of every agent
+const HandleOps kDogfightOps = {
+    .kind = PFB_KIND_FIXEDWING, .env_kind = PFB_ENV_DOGFIGHT,
+    .state_rows = FW_ROWS, .istate_rows = FI_ROWS, .layout = PFB_LAYOUT_FIELD_MAJOR, .setpoint_dim = 4, .aux_dim = 6,
+    .obs_dim = df_obs_dim,
+    .reset = fw_reset, .set_mode = fw_set_mode, .aviary_step = fw_aviary_step, .observe = fw_observe,
+    .env_reset = df_env_reset, .env_step = df_env_step,
+    .spare_rows = DSP_ROWS, .spare_valid_row = DSP_VALID,
+    .invalidate_spares = tail_invalidate_spares,
+};
 
 // ===================================================================================================
 // Split ("agent-major") variant — BASELINE.json configs[4] as written: the agents of one arena live on

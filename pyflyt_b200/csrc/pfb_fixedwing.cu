@@ -16,9 +16,7 @@ int fw_build_params(const PfbModel& m, const PfbEnvConfig* env, FixedwingParams&
 }
 
 static inline int fw_setpoint_dim(const PfbContext* h) { return h->env.env_kind == PFB_ENV_NONE ? 6 : 4; }
-int fw_state_rows() { return FW_ROWS; }
-int fw_istate_rows() { return FI_ROWS; }
-int fw_obs_dim(const PfbContext* h) { return (h->wp.angle_representation == 0 ? 22 : 23) + 3 * h->wp.num_targets; }
+static int fw_obs_dim(const PfbContext* h) { return (h->wp.angle_representation == 0 ? 22 : 23) + 3 * h->wp.num_targets; }
 
 // ---------------------------------------------------------------------------------------------------
 // kernels — Aviary surface
@@ -228,8 +226,6 @@ __device__ __forceinline__ void wp_reset_env(const FixedwingParams& p, const Way
 // ---- spare post-reset states (pfb_tail_step.cuh): a record holds the FW_* state words INCLUDING the episode's targets and
 // new_distance
 enum { WSP_ROWS = 64 };
-int fw_spare_rows() { return WSP_ROWS; }
-int fw_spare_valid_row() { return FW_ROWS + SPARE_VALID; }
 
 // the Fixedwing-Waypoints env for tail_step (pfb_tail_step.cuh)
 template <bool INJECT, bool RANDACT>
@@ -384,13 +380,16 @@ int fw_reset(PfbContext* h, const uint8_t* mask, cudaStream_t s) {
 }
 
 int fw_set_mode(PfbContext* h, int mode, cudaStream_t s) {
+  const int lo = kModeLo[PFB_KIND_FIXEDWING], hi = kModeHi[PFB_KIND_FIXEDWING];
+  if (mode < lo || mode > hi)  // the message of fixedwing.py:216-219
+    return fail("`mode` must be between %d and %d or be registered in self.registered_controllers.keys()=dict_keys([]), got %d.", lo, hi, mode);
   if (mode == -1 && fw_setpoint_dim(h) < 6) return fail("mode -1 needs the 6-wide setpoint buffer of the Aviary surface");
   CUDA_OK(cudaMemsetAsync(h->buf.setpoint, 0, (size_t)h->n * fw_setpoint_dim(h) * sizeof(float), s));  // fixedwing.py:224-227
   h->mode = mode;
   return 0;
 }
 
-int fw_set_modes(PfbContext* h, cudaStream_t s) {
+static int fw_set_modes(PfbContext* h, const int8_t*, cudaStream_t s) {
   CUDA_OK(cudaMemsetAsync(h->buf.setpoint, 0, (size_t)h->n * fw_setpoint_dim(h) * sizeof(float), s));  // every drone's set_mode
   h->mode = kModePerDrone;
   return 0;
@@ -434,14 +433,14 @@ int fw_aviary_step(PfbContext* h, int n_steps, const float* noise, cudaStream_t 
   return 0;
 }
 
-int fw_set_base_state(PfbContext* h, const BaseStateIn& a, cudaStream_t s) {
+static int fw_set_base_state(PfbContext* h, const BaseStateIn& a, cudaStream_t s) {
   if (a.lin32 || a.ang32) k_fw_set_base_state<true><<<grid_for(h->n), kBlock, 0, s>>>(a, h->buf.state, h->buf.istate, h->n);
   else k_fw_set_base_state<false><<<grid_for(h->n), kBlock, 0, s>>>(a, h->buf.state, h->buf.istate, h->n);
   LAUNCH_CHECK(h);
   return 0;
 }
 
-int fw_get_base_state(PfbContext* h, const BaseStateOut& o, cudaStream_t s) {
+static int fw_get_base_state(PfbContext* h, const BaseStateOut& o, cudaStream_t s) {
   k_fw_get_base_state<<<grid_for(h->n), kBlock, 0, s>>>(o, h->buf.state, h->buf.istate, h->n);
   LAUNCH_CHECK(h);
   return 0;
@@ -472,7 +471,7 @@ static auto fwwp_launcher(PfbContext* h, float* actions, const float* noise) {
   };
 }
 
-int fw_env_reset(PfbContext* h, const uint8_t* mask, const float* noise, cudaStream_t s) {
+static int fw_env_reset(PfbContext* h, const uint8_t* mask, const float* noise, cudaStream_t s) {
   const uint32_t seq = 0x80000000u | (uint32_t)h->reset_seq++;
   auto reset = [&](int g) -> int {
     if (noise)
@@ -488,6 +487,24 @@ int fw_env_reset(PfbContext* h, const uint8_t* mask, const float* noise, cudaStr
   return 0;
 }
 
-int fw_env_step(PfbContext* h, float* actions, const float* noise, bool randact, cudaStream_t s) {
+static int fw_env_step(PfbContext* h, float* actions, const float* noise, bool randact, size_t, cudaStream_t s) {
   return tail_env_step(h, noise, randact, s, fwwp_launcher(h, actions, noise));
 }
+
+const HandleOps kFixedwingAviaryOps = {
+    .kind = PFB_KIND_FIXEDWING, .env_kind = PFB_ENV_NONE,
+    .state_rows = FW_ROWS, .istate_rows = FI_ROWS, .layout = PFB_LAYOUT_FIELD_MAJOR, .setpoint_dim = 6, .aux_dim = 6,
+    .obs_dim = fw_obs_dim,
+    .reset = fw_reset, .set_mode = fw_set_mode, .set_modes = fw_set_modes, .aviary_step = fw_aviary_step, .observe = fw_observe,
+    .set_base_state = fw_set_base_state, .get_base_state = fw_get_base_state,
+};
+
+const HandleOps kFixedwingWaypointsOps = {
+    .kind = PFB_KIND_FIXEDWING, .env_kind = PFB_ENV_FIXEDWING_WAYPOINTS,
+    .state_rows = FW_ROWS, .istate_rows = FI_ROWS, .layout = PFB_LAYOUT_FIELD_MAJOR, .setpoint_dim = 4, .aux_dim = 6,
+    .obs_dim = fw_obs_dim,
+    .reset = fw_reset, .set_mode = fw_set_mode, .aviary_step = fw_aviary_step, .observe = fw_observe,
+    .env_reset = fw_env_reset, .env_step = fw_env_step,
+    .spare_rows = WSP_ROWS, .spare_valid_row = FW_ROWS + SPARE_VALID,
+    .invalidate_spares = tail_invalidate_spares,
+};

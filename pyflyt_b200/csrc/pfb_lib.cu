@@ -1,5 +1,5 @@
-// pfb_lib.cu — the C-ABI of libpyflyt_b200.so (include/pyflyt_b200.h): argument checks, handle lifetime, and dispatch
-// to the vehicle translation units (pfb_quadx.cu, pfb_quadx_wp.cu, pfb_fixedwing.cu, pfb_rocket.cu, pfb_dogfight.cu).
+// pfb_lib.cu — the C-ABI of libpyflyt_b200.so (include/pyflyt_b200.h): argument checks, handle lifetime, and calls through
+// the handle's operations table (HandleOps, pfb_context.h) into the vehicle translation units (pfb_quadx.cu, ...).
 #include <cuda_runtime.h>
 
 #include <cmath>
@@ -132,15 +132,13 @@ static int single_setup(PfbContext* c, const PfbModel* model, const PfbEnvConfig
   c->hover.ma = (env && env->env_kind == PFB_ENV_MA_QUADX_HOVER) ? 1 : 0;
   if (c->hover.ma && env->autoreset)
     return fail("MAQuadXHover is a per-agent epilogue: arenas are reset by the caller (pfb_env_reset with a mask), autoreset must be 0");
-  if (env && env->env_kind != PFB_ENV_NONE) {
-    const bool ok = (model->kind == PFB_KIND_QUADX && env->env_kind == PFB_ENV_QUADX_HOVER) ||
-                    (model->kind == PFB_KIND_QUADX && env->env_kind == PFB_ENV_QUADX_WAYPOINTS) ||
-                    (model->kind == PFB_KIND_QUADX && env->env_kind == PFB_ENV_MA_QUADX_HOVER) ||
-                    (model->kind == PFB_KIND_FIXEDWING && env->env_kind == PFB_ENV_FIXEDWING_WAYPOINTS) ||
-                    (model->kind == PFB_KIND_FIXEDWING && env->env_kind == PFB_ENV_DOGFIGHT) ||
-                    (model->kind == PFB_KIND_ROCKET && env->env_kind == PFB_ENV_ROCKET_LANDING);
-    if (!ok) return fail("env kind %d is not available for vehicle kind %d in this library", env->env_kind, model->kind);
-  }
+  static const HandleOps* const kSingleKindOps[] = {&kQuadXAviaryOps,     &kHoverOps,    &kMAQuadXHoverOps, &kQuadXWaypointsOps,
+                                                    &kFixedwingAviaryOps, &kFixedwingWaypointsOps, &kDogfightOps,
+                                                    &kRocketAviaryOps,    &kRocketLandingOps};
+  const int env_kind = env ? env->env_kind : PFB_ENV_NONE;
+  for (const HandleOps* t : kSingleKindOps)
+    if (t->kind == model->kind && t->env_kind == env_kind) c->ops = t;
+  if (!c->ops) return fail("env kind %d is not available for vehicle kind %d in this library", env->env_kind, model->kind);
   if (env && env->env_kind == PFB_ENV_QUADX_WAYPOINTS) {
     if (env->num_targets < 1 || env->num_targets > kMaxTargets) return fail("num_targets must be in 1..%d, got %d", kMaxTargets, env->num_targets);
     c->qwp.env_step_ratio = env->env_step_ratio;
@@ -156,22 +154,14 @@ static int single_setup(PfbContext* c, const PfbModel* model, const PfbEnvConfig
     c->qwp.min_height = 0.1f;  // quadx_waypoints_env.py:88
   }
   CUDA_OK(cudaMalloc(&c->d_done_list, 4 * (size_t)n_envs * sizeof(int32_t)));
-  if (env && env->autoreset && (env->env_kind == PFB_ENV_QUADX_HOVER || env->env_kind == PFB_ENV_FIXEDWING_WAYPOINTS ||
-                                 env->env_kind == PFB_ENV_QUADX_WAYPOINTS || env->env_kind == PFB_ENV_ROCKET_LANDING ||
-                                 env->env_kind == PFB_ENV_DOGFIGHT)) {
+  if (env && env->autoreset && c->ops->spare_rows) {
     // spare post-reset states: env-major records (QuadX-Hover: four per env, buffer = episode number & 3, rebuilt by builder
     // CTAs inside the step launches; the other env kinds: one per env, rebuilt on a library-owned side stream)
-    const bool hover = env->env_kind == PFB_ENV_QUADX_HOVER;
-    size_t rec = (size_t)hover_spare_rows();  // floats per env
-    if (env->env_kind == PFB_ENV_QUADX_WAYPOINTS) rec = (size_t)qwp_spare_rows();
-    else if (env->env_kind == PFB_ENV_FIXEDWING_WAYPOINTS) rec = (size_t)fw_spare_rows();
-    else if (env->env_kind == PFB_ENV_ROCKET_LANDING) rec = (size_t)rk_spare_rows();
-    else if (env->env_kind == PFB_ENV_DOGFIGHT) rec = (size_t)df_spare_rows();
-    c->spare_bytes = rec * (size_t)n_envs * sizeof(float);
+    c->spare_bytes = (size_t)c->ops->spare_rows * (size_t)n_envs * sizeof(float);
     CUDA_OK(cudaMalloc(&c->d_spare, c->spare_bytes));
     CUDA_OK(cudaMemset(c->d_spare, 0, c->spare_bytes));
-    if (hover) {
-      CUDA_OK(cudaMalloc(&c->d_consumed, (size_t)hover_consumed_rows() * (size_t)n_envs * sizeof(int2)));  // (env, episode) per reset of a fused launch
+    if (c->ops->consumed_rows) {
+      CUDA_OK(cudaMalloc(&c->d_consumed, (size_t)c->ops->consumed_rows * (size_t)n_envs * sizeof(int2)));  // (env, episode) per reset of a fused launch
       CUDA_OK(cudaMalloc(&c->d_elist, 4 * (size_t)n_envs * sizeof(uint32_t)));
       CUDA_OK(cudaMemset(c->d_elist, 0, 4 * (size_t)n_envs * sizeof(uint32_t)));
       CUDA_OK(cudaMalloc(&c->d_episode, (size_t)n_envs * sizeof(uint32_t)));
@@ -246,25 +236,20 @@ int pfb_set_env_offset(PfbHandle h, uint64_t first_global_env) {
   return 0;
 }
 
-static inline bool is_fw(PfbHandle h) { return h->model.kind == PFB_KIND_FIXEDWING; }
-static inline bool is_rk(PfbHandle h) { return h->model.kind == PFB_KIND_ROCKET; }
-static inline bool is_qwp(PfbHandle h) { return h->model.kind == PFB_KIND_QUADX && h->env.env_kind == PFB_ENV_QUADX_WAYPOINTS; }
-static inline bool is_ma(PfbHandle h) { return h->model.kind == PFB_KIND_QUADX && h->env.env_kind == PFB_ENV_MA_QUADX_HOVER; }
-static inline bool is_df(PfbHandle h) { return h->model.kind == PFB_KIND_FIXEDWING && h->env.env_kind == PFB_ENV_DOGFIGHT; }
 // A mixed-kind handle (pfb_create_mixed) carves its state buffer by kind: rows of the widest kind present, PFB_LAYOUT_BY_KIND,
 // setpoints and aux of the widest kind (rocket), and its obs buffer receives the hi / lo position words of pfb_observe_state
-int pfb_state_rows(PfbHandle h) { if (h && h->mixed) return mx_state_rows(h); return is_rk(h) ? rk_state_rows() : (is_fw(h) ? fw_state_rows() : (is_qwp(h) ? qwp_state_rows() : qx_rows(h))); }
-int pfb_state_layout(PfbHandle h) { if (h && h->mixed) return PFB_LAYOUT_BY_KIND; return h && qx_tiled(h) ? PFB_LAYOUT_WARP_TILED : PFB_LAYOUT_FIELD_MAJOR; }
+int pfb_state_rows(PfbHandle h) { return h->ops->mixed_state_rows ? h->ops->mixed_state_rows(h) : h->ops->state_rows; }
+int pfb_state_layout(PfbHandle h) { return h ? h->ops->layout : PFB_LAYOUT_FIELD_MAJOR; }
 int64_t pfb_state_floats(PfbHandle h) {
   if (!h) return 0;
-  if (h->mixed) return mx_state_floats(h);
-  if (qx_tiled(h)) return ((h->n + kTileLanes - 1) / kTileLanes) * qx_tile_floats(qx_rows(h));  // padded to whole tiles
-  return (int64_t)pfb_state_rows(h) * h->n;
+  if (h->ops->mixed_state_floats) return h->ops->mixed_state_floats(h);
+  if (h->ops->layout == PFB_LAYOUT_WARP_TILED) return ((h->n + kTileLanes - 1) / kTileLanes) * qx_tile_floats(h->ops->state_rows);  // whole tiles
+  return (int64_t)h->ops->state_rows * h->n;
 }
-int pfb_istate_rows(PfbHandle h) { if (h && h->mixed) return mx_istate_rows(h); return is_rk(h) ? rk_istate_rows() : (is_fw(h) ? fw_istate_rows() : (is_qwp(h) ? qwp_istate_rows() : QI_ROWS)); }
-int pfb_setpoint_dim(PfbHandle h) { if (h && h->mixed) return 7; return is_rk(h) ? 7 : ((is_fw(h) && h->env.env_kind == PFB_ENV_NONE) ? 6 : 4); }
-int pfb_obs_dim(PfbHandle h) { if (h && h->mixed) return 6; return is_df(h) ? df_obs_dim(h) : is_rk(h) ? rk_obs_dim(h) : (is_fw(h) ? fw_obs_dim(h) : (is_qwp(h) ? qwp_obs_dim(h) : (h->hover.angle_representation == 0 ? 20 : 21) + (is_ma(h) ? 3 : 0))); }
-int pfb_aux_dim(PfbHandle h) { if (h && h->mixed) return 9; return is_rk(h) ? 9 : (is_fw(h) ? 6 : 4); }
+int pfb_istate_rows(PfbHandle h) { return h->ops->mixed_istate_rows ? h->ops->mixed_istate_rows(h) : h->ops->istate_rows; }
+int pfb_setpoint_dim(PfbHandle h) { return h->ops->setpoint_dim; }
+int pfb_obs_dim(PfbHandle h) { return h->ops->obs_dim(h); }
+int pfb_aux_dim(PfbHandle h) { return h->ops->aux_dim; }
 
 int pfb_bind(PfbHandle h, const PfbBuffers* b) {
   if (!h || !b) return fail("pfb_bind: null argument");
@@ -287,38 +272,21 @@ int pfb_bind(PfbHandle h, const PfbBuffers* b) {
 int pfb_reset(PfbHandle h, const uint8_t* mask, void* stream) {
   if (h) h->fused_ready = 0;
   REQUIRE_BOUND(h);
-  cudaStream_t s = (cudaStream_t)stream;
-  if (h->mixed) return mx_reset(h, mask, s);
-  if (is_fw(h)) return fw_reset(h, mask, s);
-  if (is_rk(h)) return rk_reset(h, mask, s);
-  return qx_reset(h, mask, s);
+  return h->ops->reset(h, mask, (cudaStream_t)stream);
 }
 
 int pfb_set_mode(PfbHandle h, int mode, void* stream) {
   REQUIRE_BOUND(h);
-  cudaStream_t s = (cudaStream_t)stream;
-  if (h->mixed) return mx_set_mode(h, mode, s);
-  const int lo = kModeLo[h->model.kind], hi = kModeHi[h->model.kind];
-  if (mode < lo || mode > hi) {  // the messages of quadx.py:259-262, fixedwing.py:216-219, base_drone.py:252-255
-    if (is_rk(h)) return fail("`mode` must be either 0 or be registered in self.registered_controllers.keys()=dict_keys([]), got %d.", mode);
-    if (is_fw(h))
-      return fail("`mode` must be between %d and %d or be registered in self.registered_controllers.keys()=dict_keys([]), got %d.", lo, hi, mode);
-    return fail("`mode` must be between %d and %d, got %d", lo, hi, mode);
-  }
-  if (is_fw(h)) return fw_set_mode(h, mode, s);
-  if (is_rk(h)) {  // the rocket's one mode: nothing to preset
-    h->mode = 0;
-    return 0;
-  }
-  return qx_set_mode(h, mode, s);
+  return h->ops->set_mode(h, mode, (cudaStream_t)stream);
 }
 
 int pfb_set_modes(PfbHandle h, const int8_t* modes, void* stream) {
   if (!h || !modes) return fail("pfb_set_modes: null argument");
-  if (h->env.env_kind != PFB_ENV_NONE)
+  if (h->ops->env_step)
     return fail("pfb_set_modes: only Aviary handles fly one flight mode per drone; a handle with an env epilogue flies its env's flight_mode");
   REQUIRE_BOUND(h);
-  if (h->mixed) return mx_set_modes(h, modes, (cudaStream_t)stream);
+  cudaStream_t s = (cudaStream_t)stream;
+  if (h->ops == &kMixedOps) return h->ops->set_modes(h, modes, s);  // checks each drone against its own kind
   const int lo = kModeLo[h->model.kind], hi = kModeHi[h->model.kind];
   bool uniform = true;
   for (int64_t i = 0; i < h->n; ++i) {
@@ -327,7 +295,6 @@ int pfb_set_modes(PfbHandle h, const int8_t* modes, void* stream) {
     uniform = uniform && modes[i] == modes[0];
   }
   if (uniform) return pfb_set_mode(h, modes[0], stream);  // one mode: the uniform kernels
-  cudaStream_t s = (cudaStream_t)stream;
   const size_t padded = (size_t)grid_for(h->n) * kBlock;  // whole tiles, like d_model_index
   if (!h->d_modes) {
     CUDA_OK(cudaMalloc(&h->d_modes, padded));
@@ -335,31 +302,22 @@ int pfb_set_modes(PfbHandle h, const int8_t* modes, void* stream) {
   }
   // stream-ordered: a step still queued on `s` reads the previous modes
   CUDA_OK(cudaMemcpyAsync(h->d_modes, modes, (size_t)h->n, cudaMemcpyHostToDevice, s));
-  if (is_fw(h)) return fw_set_modes(h, s);
-  return qx_set_modes(h, s);
+  return h->ops->set_modes(h, modes, s);
 }
 
 int pfb_aviary_step(PfbHandle h, int n_steps, const float* noise, void* stream) {
   REQUIRE_BOUND(h);
   if (n_steps <= 0) return fail("n_steps must be positive");
-  cudaStream_t s = (cudaStream_t)stream;
-  if (h->mixed) return mx_aviary_step(h, n_steps, noise, s);
-  if (is_fw(h)) return fw_aviary_step(h, n_steps, noise, s);
-  if (is_rk(h)) return rk_aviary_step(h, n_steps, noise, s);
-  return qx_aviary_step(h, n_steps, noise, s);
+  return h->ops->aviary_step(h, n_steps, noise, (cudaStream_t)stream);
 }
 
 int pfb_set_base_velocity(PfbHandle h, const float* lin_vel, const float* ang_vel, void* stream) {
   REQUIRE_BOUND(h);
   if (!lin_vel || !ang_vel) return fail("pfb_set_base_velocity: null argument");
-  if (h->env.env_kind != PFB_ENV_NONE && !is_rk(h))  // Rocket-Landing's reset calls it (rocket_base_env.py:228)
+  if (!h->ops->set_base_state)
     return fail("pfb_set_base_velocity: only Aviary handles and Rocket-Landing handles; this env builds its autoreset spares from the state");
   const BaseStateIn a = {nullptr, nullptr, nullptr, nullptr, nullptr, lin_vel, ang_vel};
-  cudaStream_t s = (cudaStream_t)stream;
-  if (h->mixed) return mx_set_base_state(h, a, s);
-  if (is_fw(h)) return fw_set_base_state(h, a, s);
-  if (is_rk(h)) return rk_set_base_state(h, a, s);
-  return qx_set_base_state(h, a, s);
+  return h->ops->set_base_state(h, a, (cudaStream_t)stream);
 }
 
 // env handles keep autoreset spares and episode bookkeeping built from the state: their base state is the env's business
@@ -376,11 +334,7 @@ int pfb_set_base_state(PfbHandle h, const uint8_t* mask, const double* pos, cons
   if (!pos != !quat) return fail("pfb_set_base_state: pos and quat come together (a pose) or not at all");
   if (!pos && !lin_vel && !ang_vel) return 0;
   const BaseStateIn a = {mask, pos, quat, lin_vel, ang_vel, nullptr, nullptr};
-  cudaStream_t s = (cudaStream_t)stream;
-  if (h->mixed) return mx_set_base_state(h, a, s);
-  if (is_fw(h)) return fw_set_base_state(h, a, s);
-  if (is_rk(h)) return rk_set_base_state(h, a, s);
-  return qx_set_base_state(h, a, s);
+  return h->ops->set_base_state(h, a, (cudaStream_t)stream);
 }
 
 int pfb_get_base_state(PfbHandle h, double* pos, double* quat, double* lin_vel, double* ang_vel, void* stream) {
@@ -388,24 +342,17 @@ int pfb_get_base_state(PfbHandle h, double* pos, double* quat, double* lin_vel, 
   if (require_aviary(h, "pfb_get_base_state")) return -1;
   if (!pos && !quat && !lin_vel && !ang_vel) return 0;
   const BaseStateOut o = {pos, quat, lin_vel, ang_vel};
-  cudaStream_t s = (cudaStream_t)stream;
-  if (h->mixed) return mx_get_base_state(h, o, s);
-  if (is_fw(h)) return fw_get_base_state(h, o, s);
-  if (is_rk(h)) return rk_get_base_state(h, o, s);
-  return qx_get_base_state(h, o, s);
+  return h->ops->get_base_state(h, o, (cudaStream_t)stream);
 }
 
 int pfb_observe_state(PfbHandle h, void* stream) {
   REQUIRE_BOUND(h);
-  if (h->mixed) return mx_observe(h, (cudaStream_t)stream);
-  if (is_fw(h)) return fw_observe(h, (cudaStream_t)stream);
-  if (is_rk(h)) return rk_observe(h, (cudaStream_t)stream);
-  return qx_observe(h, (cudaStream_t)stream);
+  return h->ops->observe(h, (cudaStream_t)stream);
 }
 
 static int require_env(PfbHandle h) {
-  if (h->mixed) return fail("a mixed-kind handle is an Aviary handle: the env entry points fly one vehicle kind");
-  if (h->env.env_kind == PFB_ENV_NONE) return fail("handle was created without an env epilogue");
+  if (h->ops == &kMixedOps) return fail("a mixed-kind handle is an Aviary handle: the env entry points fly one vehicle kind");
+  if (!h->ops->env_step) return fail("handle was created without an env epilogue");
   if (!h->buf.obs || !h->buf.reward || !h->buf.term || !h->buf.trunc) return fail("obs/reward/term/trunc buffers are not bound");
   return 0;
 }
@@ -414,21 +361,7 @@ int pfb_env_reset(PfbHandle h, const uint8_t* mask, const float* noise, void* st
   REQUIRE_BOUND(h);
   if (require_env(h)) return -1;
   h->fused_ready = 0;
-  cudaStream_t s = (cudaStream_t)stream;
-  if (is_df(h)) return df_env_reset(h, mask, noise, s);
-  if (is_fw(h)) return fw_env_reset(h, mask, noise, s);
-  if (is_rk(h)) return rk_env_reset(h, mask, noise, s);
-  if (is_qwp(h)) return qwp_env_reset(h, mask, noise, s);
-  return hover_env_reset(h, mask, noise, s);
-}
-
-// `dyn_smem`: dynamic shared memory the QuadX-Hover step launch requests and never touches (pfb_env_step_mapped)
-static int env_step_impl(PfbHandle h, float* actions, const float* noise, bool randact, size_t dyn_smem, cudaStream_t s) {
-  if (is_df(h)) return df_env_step(h, actions, noise, randact, s);
-  if (is_fw(h)) return fw_env_step(h, actions, noise, randact, s);
-  if (is_rk(h)) return rk_env_step(h, actions, noise, randact, s);
-  if (is_qwp(h)) return qwp_env_step(h, actions, noise, randact, s);
-  return hover_env_step(h, actions, noise, randact, dyn_smem, s);
+  return h->ops->env_reset(h, mask, noise, (cudaStream_t)stream);
 }
 
 int pfb_sizeof_wind(void) { return (int)sizeof(PfbWind); }
@@ -450,13 +383,7 @@ int pfb_set_wind(PfbHandle h, const PfbWind* wind) {
     CUDA_OK(cudaSetDevice(h->device));
     if (h->side) CUDA_OK(cudaStreamSynchronize(h->side));
     CUDA_OK(cudaDeviceSynchronize());
-    if (h->env.env_kind == PFB_ENV_QUADX_HOVER) {
-      if (hover_invalidate_spares(h, 0)) return -1;
-    } else {
-      const int valid = is_df(h) ? df_spare_valid_row() : is_rk(h) ? rk_spare_valid_row() : is_qwp(h) ? qwp_spare_valid_row() : fw_spare_valid_row();
-      const size_t rows = (size_t)(is_df(h) ? df_spare_rows() : is_rk(h) ? rk_spare_rows() : is_qwp(h) ? qwp_spare_rows() : fw_spare_rows());
-      CUDA_OK(cudaMemset2DAsync(h->d_spare + valid, rows * sizeof(float), 0, sizeof(float), (size_t)h->n, 0));
-    }
+    if (h->ops->invalidate_spares(h, 0)) return -1;
     CUDA_OK(cudaDeviceSynchronize());
   }
   h->qx.wind = w;
@@ -469,9 +396,9 @@ int pfb_set_wind(PfbHandle h, const PfbWind* wind) {
 
 int pfb_set_models(PfbHandle h, const PfbModel* models, int k, const uint8_t* index_host) {
   if (!h || !models || !index_host) return fail("pfb_set_models: null argument");
-  if (h->mixed) return fail("pfb_set_models: a mixed-kind handle takes its models at pfb_create_mixed");
+  if (h->ops == &kMixedOps) return fail("pfb_set_models: a mixed-kind handle takes its models at pfb_create_mixed");
   if (h->model.kind != PFB_KIND_QUADX) return fail("pfb_set_models: only QuadX handles fly several vehicle models");
-  if (is_ma(h)) return fail("pfb_set_models: MAQuadXHover handles fly one vehicle model");
+  if (h->ops == &kMAQuadXHoverOps) return fail("pfb_set_models: MAQuadXHover handles fly one vehicle model");
   if (k < 1 || k > PFB_MAX_QUADX_MODELS) return fail("pfb_set_models: k = %d, must be in 1..%d", k, PFB_MAX_QUADX_MODELS);
   QuadXParams tables[PFB_MAX_QUADX_MODELS];
   if (pfb_quadx_tables(models, k, tables)) return -1;
@@ -530,15 +457,15 @@ int pfb_env_step(PfbHandle h, const float* actions, const float* noise, void* st
   REQUIRE_BOUND(h);
   if (require_env(h)) return -1;
   if (actions && ((uintptr_t)actions & 15)) return fail("pfb_env_step: actions must be 16-byte aligned");
-  return env_step_impl(h, actions ? const_cast<float*>(actions) : h->buf.setpoint, noise, false, 0, (cudaStream_t)stream);
+  return h->ops->env_step(h, actions ? const_cast<float*>(actions) : h->buf.setpoint, noise, false, 0, (cudaStream_t)stream);
 }
 
 int pfb_env_rollout(PfbHandle h, int n_steps, void* stream) {
   REQUIRE_BOUND(h);
   if (require_env(h)) return -1;
-  if (qx_tiled(h)) return hover_env_rollout(h, n_steps, (cudaStream_t)stream);  // an env handle: QuadX-Hover or MAQuadXHover
+  if (h->ops->env_rollout) return h->ops->env_rollout(h, n_steps, (cudaStream_t)stream);
   for (int k = 0; k < n_steps; ++k)
-    if (env_step_impl(h, h->buf.setpoint, nullptr, true, 0, (cudaStream_t)stream)) return -1;
+    if (h->ops->env_step(h, h->buf.setpoint, nullptr, true, 0, (cudaStream_t)stream)) return -1;
   return 0;
 }
 
@@ -552,7 +479,7 @@ int pfb_env_step_host(PfbHandle h, const float* host_actions, float* host_obs, f
   cudaStream_t s = (cudaStream_t)stream;
   const int O = pfb_obs_dim(h);
   CUDA_OK(cudaMemcpyAsync(h->buf.setpoint, host_actions, (size_t)h->n * pfb_setpoint_dim(h) * sizeof(float), cudaMemcpyHostToDevice, s));
-  if (env_step_impl(h, h->buf.setpoint, nullptr, false, 0, s)) return -1;
+  if (h->ops->env_step(h, h->buf.setpoint, nullptr, false, 0, s)) return -1;
   // obs | reward | term | trunc laid out back to back on both sides (what the Python mirror allocates): one copy, one
   // PCIe transaction stream instead of four latency-bound ones
   const size_t ob = (size_t)h->n * O * sizeof(float), rb = (size_t)h->n * sizeof(float), fb = (size_t)h->n;
@@ -595,7 +522,7 @@ int pfb_env_step_mapped(PfbHandle h, const float* host_actions, float* host_obs,
   if (((uintptr_t)da & 15) || ((uintptr_t)dob & 15)) return fail("pfb_env_step_mapped: actions and obs must be 16-byte aligned");
   const PfbBuffers saved = h->buf;
   h->buf.obs = (float*)dob; h->buf.reward = (float*)dr; h->buf.term = (uint8_t*)dte; h->buf.trunc = (uint8_t*)dtr;
-  const int rc = env_step_impl(h, (float*)da, nullptr, false, kMappedDynSmem, (cudaStream_t)stream);
+  const int rc = h->ops->env_step(h, (float*)da, nullptr, false, kMappedDynSmem, (cudaStream_t)stream);
   h->buf = saved;
   return rc;
 }
@@ -606,7 +533,7 @@ int pfb_dogfight_payload_dim(void) { return 20; }
 int pfb_dogfight_physics(PfbHandle h, const float* actions, const float* noise, float* payload_out, int first, int do_reset, int aviary_index,
                          void* stream) {
   REQUIRE_BOUND(h);
-  if (!is_df(h)) return fail("handle is not a dogfight env");
+  if (h->ops != &kDogfightOps) return fail("handle is not a dogfight env");
   if (!payload_out) return fail("pfb_dogfight_physics: null payload buffer");
   return df_split_physics(h, actions ? actions : h->buf.setpoint, noise, payload_out, nullptr, 0, 0, nullptr, 0, 0, first, do_reset, aviary_index,
                           (cudaStream_t)stream);
@@ -616,7 +543,7 @@ int pfb_dogfight_physics_peer(PfbHandle h, const float* actions, const float* no
                              int64_t slot_offset_floats, const uint64_t* peer_flags_dev, int rank, int epoch, int first, int do_reset,
                              int aviary_index, void* stream) {
   REQUIRE_BOUND(h);
-  if (!is_df(h)) return fail("handle is not a dogfight env");
+  if (h->ops != &kDogfightOps) return fail("handle is not a dogfight env");
   if (!peer_tables_dev || world < 1) return fail("pfb_dogfight_physics_peer: need the device array of peer table pointers");
   return df_split_physics(h, actions ? actions : h->buf.setpoint, noise, nullptr, peer_tables_dev, world, slot_offset_floats, peer_flags_dev, rank,
                           epoch, first, do_reset, aviary_index, (cudaStream_t)stream);
@@ -624,7 +551,7 @@ int pfb_dogfight_physics_peer(PfbHandle h, const float* actions, const float* no
 
 int pfb_dogfight_combat(PfbHandle h, const float* payload_table, int64_t first_global_agent, int64_t num_arenas, int last, void* stream) {
   REQUIRE_BOUND(h);
-  if (!is_df(h)) return fail("handle is not a dogfight env");
+  if (h->ops != &kDogfightOps) return fail("handle is not a dogfight env");
   if (require_env(h)) return -1;
   return df_split_combat(h, payload_table, first_global_agent, num_arenas, last, nullptr, 0, 0, (cudaStream_t)stream);
 }
@@ -632,7 +559,7 @@ int pfb_dogfight_combat(PfbHandle h, const float* payload_table, int64_t first_g
 int pfb_dogfight_combat_wait(PfbHandle h, const float* payload_table, int64_t first_global_agent, int64_t num_arenas, int last,
                              const int32_t* flags, int world, int epoch, void* stream) {
   REQUIRE_BOUND(h);
-  if (!is_df(h)) return fail("handle is not a dogfight env");
+  if (h->ops != &kDogfightOps) return fail("handle is not a dogfight env");
   if (require_env(h)) return -1;
   if (!flags) return fail("pfb_dogfight_combat_wait: null flag array");
   return df_split_combat(h, payload_table, first_global_agent, num_arenas, last, flags, world, epoch, (cudaStream_t)stream);
@@ -644,7 +571,7 @@ int pfb_dogfight_split_step(PfbHandle h, const float* actions, const uint64_t* p
                             const float* local_tables, const int32_t* local_flags, int world, int rank, int epoch0,
                             int64_t first_global_agent, int64_t num_arenas, void* stream) {
   REQUIRE_BOUND(h);
-  if (!is_df(h)) return fail("handle is not a dogfight env");
+  if (h->ops != &kDogfightOps) return fail("handle is not a dogfight env");
   if (require_env(h)) return -1;
   if (!peer_tables_dev || !peer_flags_dev || !local_tables || !local_flags) return fail("pfb_dogfight_split_step: null argument");
   const int64_t na = 2 * num_arenas;

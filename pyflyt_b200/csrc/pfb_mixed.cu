@@ -290,13 +290,13 @@ static int kind_state_rows(int k) { return k == 0 ? (int)QX_ROWS : (k == 1 ? (in
 static int kind_istate_rows(int k) { return k == 0 ? (int)QI_ROWS : (k == 1 ? (int)FI_ROWS : (int)RI_ROWS); }
 static int grid_of(const MixedKinds* m, int k) { return grid_for(m->count[k]); }
 
-int mx_state_rows(const PfbContext* h) {
+static int mx_state_rows(const PfbContext* h) {
   int r = 0;
   for (int k = 0; k < kKinds; ++k)
     if (h->mixed->count[k] && kind_state_rows(k) > r) r = kind_state_rows(k);
   return r;
 }
-int mx_istate_rows(const PfbContext* h) {
+static int mx_istate_rows(const PfbContext* h) {
   int r = 0;
   for (int k = 0; k < kKinds; ++k)
     if (h->mixed->count[k] && kind_istate_rows(k) > r) r = kind_istate_rows(k);
@@ -308,7 +308,7 @@ static int64_t state_offset(const MixedKinds* m, int kind) {
   for (int k = 0; k < kind; ++k) off += (kind_state_floats(k, m->count[k]) + kRegionAlign - 1) / kRegionAlign * kRegionAlign;
   return off;
 }
-int64_t mx_state_floats(const PfbContext* h) { return state_offset(h->mixed, kKinds); }
+static int64_t mx_state_floats(const PfbContext* h) { return state_offset(h->mixed, kKinds); }
 
 // the kinds' regions of the bound buffers: state at state_offset, istate as the kinds' [I_k][count_k] blocks back to back
 // (sum <= pfb_istate_rows * n)
@@ -330,7 +330,7 @@ static MixedRows rows_of(const PfbContext* h) {
 }
 static int grid_all(const MixedKinds* m) { return grid_of(m, 0) + grid_of(m, 1) + grid_of(m, 2); }
 
-int mx_reset(PfbContext* h, const uint8_t* mask, cudaStream_t s) {
+static int mx_reset(PfbContext* h, const uint8_t* mask, cudaStream_t s) {
   MixedKinds* m = h->mixed;
   k_mixed_reset<<<grid_all(m), kBlock, 0, s>>>(rows_of(h), h->fw, h->rk, h->buf.setpoint, h->buf.start_pos, h->buf.start_orn, mask);
   LAUNCH_CHECK(h);
@@ -346,7 +346,7 @@ static int set_slot_modes(PfbContext* h, cudaStream_t s) {
   return 0;
 }
 
-int mx_set_mode(PfbContext* h, int mode, cudaStream_t s) {
+static int mx_set_mode(PfbContext* h, int mode, cudaStream_t s) {
   MixedKinds* m = h->mixed;
   for (int64_t u = 0; u < h->n; ++u) {  // nothing changes unless the mode is valid for every drone
     const int k = m->h_kind[u];
@@ -358,7 +358,7 @@ int mx_set_mode(PfbContext* h, int mode, cudaStream_t s) {
   return set_slot_modes(h, s);
 }
 
-int mx_set_modes(PfbContext* h, const int8_t* modes, cudaStream_t s) {
+static int mx_set_modes(PfbContext* h, const int8_t* modes, cudaStream_t s) {
   MixedKinds* m = h->mixed;
   for (int64_t u = 0; u < h->n; ++u) {
     const int k = m->h_kind[u];
@@ -401,7 +401,7 @@ static void launch_steps(const PfbContext* h, const float* noise, int n_steps, u
                                 : (noise ? launch_step<true, false, RATES>(h, ps, noise, n_steps, seq, s) : launch_step<false, false, RATES>(h, ps, noise, n_steps, seq, s))));
 }
 
-int mx_aviary_step(PfbContext* h, int n_steps, const float* noise, cudaStream_t s) {
+static int mx_aviary_step(PfbContext* h, int n_steps, const float* noise, cudaStream_t s) {
   const uint32_t seq = (uint32_t)h->aviary_seq++;
   if (h->mixed->d_slot_ratio) launch_steps<true>(h, noise, n_steps, seq, s);
   else launch_steps<false>(h, noise, n_steps, seq, s);
@@ -409,7 +409,7 @@ int mx_aviary_step(PfbContext* h, int n_steps, const float* noise, cudaStream_t 
   return 0;
 }
 
-int mx_observe(PfbContext* h, cudaStream_t s) {
+static int mx_observe(PfbContext* h, cudaStream_t s) {
   MixedObserve a;
   a.r = rows_of(h);
   a.drone_state = h->buf.drone_state;
@@ -421,18 +421,30 @@ int mx_observe(PfbContext* h, cudaStream_t s) {
   return 0;
 }
 
-int mx_set_base_state(PfbContext* h, const BaseStateIn& a, cudaStream_t s) {
+static int mx_set_base_state(PfbContext* h, const BaseStateIn& a, cudaStream_t s) {
   if (a.lin32 || a.ang32) k_mixed_set_base_state<true><<<grid_all(h->mixed), kBlock, 0, s>>>(rows_of(h), a);
   else k_mixed_set_base_state<false><<<grid_all(h->mixed), kBlock, 0, s>>>(rows_of(h), a);
   LAUNCH_CHECK(h);
   return 0;
 }
 
-int mx_get_base_state(PfbContext* h, const BaseStateOut& o, cudaStream_t s) {
+static int mx_get_base_state(PfbContext* h, const BaseStateOut& o, cudaStream_t s) {
   k_mixed_get_base_state<<<grid_all(h->mixed), kBlock, 0, s>>>(rows_of(h), o);
   LAUNCH_CHECK(h);
   return 0;
 }
+
+// the hi / lo position words of pfb_observe_state
+static int mx_obs_dim(const PfbContext*) { return 6; }
+
+const HandleOps kMixedOps = {
+    .kind = -1, .env_kind = PFB_ENV_NONE,
+    .layout = PFB_LAYOUT_BY_KIND, .setpoint_dim = 7, .aux_dim = 9,  // the widest kind's (rocket)
+    .obs_dim = mx_obs_dim,
+    .mixed_state_rows = mx_state_rows, .mixed_istate_rows = mx_istate_rows, .mixed_state_floats = mx_state_floats,
+    .reset = mx_reset, .set_mode = mx_set_mode, .set_modes = mx_set_modes, .aviary_step = mx_aviary_step, .observe = mx_observe,
+    .set_base_state = mx_set_base_state, .get_base_state = mx_get_base_state,
+};
 
 void mx_destroy(PfbContext* h) {
   MixedKinds* m = h->mixed;
@@ -453,6 +465,7 @@ static int mixed_setup(PfbContext* c, const PfbModel* models, int k, const uint8
   if (!m) return fail("out of host memory");
   memset(m, 0, sizeof(*m));
   c->mixed = m;
+  c->ops = &kMixedOps;
   c->model = models[0];
   c->env.env_kind = PFB_ENV_NONE;
   c->env.contact_response = (aviary_cfg && aviary_cfg->contact_response) ? 1 : 0;

@@ -953,8 +953,9 @@ __global__ void __launch_bounds__(kBlock)
 // ---------------------------------------------------------------------------------------------------
 // launchers
 // ---------------------------------------------------------------------------------------------------
-int hover_spare_rows() { return SP_ROWS * kSpareBufs; }
-int hover_consumed_rows() { return kRolloutMaxSteps / 2 + 1; }  // an env resets at most every second step of a fused launch
+// QuadX state layout: warp-tiled (pfb_quadx.cuh) on every QuadX handle except QuadX-Waypoints (field-major rows + istate)
+static inline bool qx_tiled(const PfbContext* h) { return h->model.kind == PFB_KIND_QUADX && h->env.env_kind != PFB_ENV_QUADX_WAYPOINTS; }
+static inline int qx_rows(const PfbContext* h) { return h->env.env_kind == PFB_ENV_MA_QUADX_HOVER ? (int)QM_ROWS : (int)QX_ROWS; }
 
 int qx_reset(PfbContext* h, const uint8_t* mask, cudaStream_t s) {
   if (qx_tiled(h)) k_quadx_reset<true><<<grid_for(h->n), kBlock, 0, s>>>(h->buf.state, h->buf.istate, qx_rows(h), h->buf.setpoint, h->buf.start_pos, h->buf.start_orn, mask, h->n);
@@ -972,7 +973,7 @@ int qx_set_mode(PfbContext* h, int mode, cudaStream_t s) {
   return 0;
 }
 
-int qx_set_modes(PfbContext* h, cudaStream_t s) {
+static int qx_set_modes(PfbContext* h, const int8_t*, cudaStream_t s) {
   k_quadx_set_modes<<<grid_for(h->n), kBlock, 0, s>>>(h->buf.state, qx_rows(h), h->buf.setpoint, h->d_modes, h->n);
   LAUNCH_CHECK(h);
   h->mode = kModePerDrone;
@@ -1020,20 +1021,22 @@ int qx_observe(PfbContext* h, cudaStream_t s) {
   return 0;
 }
 
-int qx_set_base_state(PfbContext* h, const BaseStateIn& a, cudaStream_t s) {
+static int qx_set_base_state(PfbContext* h, const BaseStateIn& a, cudaStream_t s) {
   if (a.lin32 || a.ang32) k_quadx_set_base_state<true><<<grid_for(h->n), kBlock, 0, s>>>(a, h->buf.state, qx_rows(h), h->n);
   else k_quadx_set_base_state<false><<<grid_for(h->n), kBlock, 0, s>>>(a, h->buf.state, qx_rows(h), h->n);
   LAUNCH_CHECK(h);
   return 0;
 }
 
-int qx_get_base_state(PfbContext* h, const BaseStateOut& o, cudaStream_t s) {
+static int qx_get_base_state(PfbContext* h, const BaseStateOut& o, cudaStream_t s) {
   k_quadx_get_base_state<<<grid_for(h->n), kBlock, 0, s>>>(o, h->buf.state, qx_rows(h), h->n);
   LAUNCH_CHECK(h);
   return 0;
 }
 
-int hover_env_reset(PfbContext* h, const uint8_t* mask, const float* noise, cudaStream_t s) {
+static int hover_obs_dim(const PfbContext* h) { return (h->hover.angle_representation == 0 ? 20 : 21) + (h->hover.ma ? 3 : 0); }
+
+static int hover_env_reset(PfbContext* h, const uint8_t* mask, const float* noise, cudaStream_t s) {
   const int mode = h->hover.flight_mode;
   // resets draw from their own Philox stream; the high bit keeps them apart from in-step autoresets
   const uint32_t seq = 0x80000000u | (uint32_t)h->reset_seq++;
@@ -1050,6 +1053,31 @@ int hover_env_reset(PfbContext* h, const uint8_t* mask, const float* noise, cuda
     LAUNCH_CHECK(h);
   }
   h->mode = mode;
+  return 0;
+}
+
+// k_hover_drain over the builder CTAs of a step launch: finish the spares whose first half the last step launch integrated (list
+// (k + 2) % 4 of the next step k, with the episode numbers its phase 0 left in d_elist); the caller checks that k >= 2
+static int hover_drain(PfbContext* h, cudaStream_t s) {
+  const uint64_t k = h->step_seq;
+  const int tiles = grid_for(h->n);
+  const int builders = h->sm_count < tiles ? h->sm_count : tiles;
+  QX_PARAMS_SWITCH(h, PFB_MODE_SWITCH(h->hover.flight_mode, (k_hover_drain<MODE, PS><<<builders, kBlock, 0, s>>>(
+                                                                 ps, h->hover, h->rng, h->d_counters + ((k + 2) % 4), h->d_done_list + ((k + 2) % 4) * h->n,
+                                                                 h->d_elist + ((k + 2) % 4) * h->n, h->buf.start_pos, h->buf.start_orn, h->d_spare,
+                                                                 h->d_episode, builders, h->n))));
+  LAUNCH_CHECK(h);
+  return 0;
+}
+
+// k_hover_spare_topup behind a SAME_STEP or fused launch, same stream: rebuild the `*count` spares it listed in d_consumed
+static int hover_topup(PfbContext* h, int32_t* count, cudaStream_t s) {
+  const int tiles = grid_for(h->n);
+  const int grid = 8 * h->sm_count < tiles ? 8 * h->sm_count : tiles;
+  QX_PARAMS_SWITCH(h, PFB_MODE_SWITCH(h->hover.flight_mode, (k_hover_spare_topup<MODE, PS><<<grid, kBlock, 0, s>>>(
+                                                                 ps, h->hover, h->rng, h->buf.start_pos, h->buf.start_orn, h->d_spare, count,
+                                                                 h->d_consumed, h->n))));
+  LAUNCH_CHECK(h);
   return 0;
 }
 
@@ -1080,20 +1108,13 @@ static int hover_same_launch(PfbContext* h, float* actions, bool randact, int T,
     CUDA_OK(cudaEventRecord(h->prof_ev[2 * h->prof_n + 1], s));
     h->prof_n += 1;
   }
-  if (spare_copy) {
-    int topup_grid = 8 * h->sm_count;
-    if (topup_grid > tiles) topup_grid = tiles;
-    QX_PARAMS_SWITCH(h, PFB_MODE_SWITCH(mode, (k_hover_spare_topup<MODE, PS><<<topup_grid, kBlock, 0, s>>>(ps, h->hover, h->rng, h->buf.start_pos,
-                                                                                                           h->buf.start_orn, h->d_spare, cnt, h->d_consumed,
-                                                                                                           h->n))));
-    LAUNCH_CHECK(h);
-  }
+  if (spare_copy && hover_topup(h, cnt, s)) return -1;
   h->same_launches += 1;
   h->step_seq += (uint64_t)T;
   return 0;
 }
 
-int hover_env_step(PfbContext* h, float* actions, const float* noise, bool randact, size_t dyn_smem, cudaStream_t s) {
+static int hover_env_step(PfbContext* h, float* actions, const float* noise, bool randact, size_t dyn_smem, cudaStream_t s) {
   const int mode = h->hover.flight_mode;
   if (h->env.autoreset == PFB_AUTORESET_SAME_STEP) {
     if (noise) return fail("injected noise (parity mode) is only supported with autoreset = 0");
@@ -1160,22 +1181,12 @@ static int hover_rollout_fused(PfbContext* h, int n_steps, cudaStream_t s) {
   const int tiles = grid_for(h->n);
   if (!h->fused_ready) {
     // finish what the single-step pipeline left half done, then bring every env's spares kRolloutAhead ahead
-    const uint64_t k = h->step_seq;
-    const int builders = h->sm_count < tiles ? h->sm_count : tiles;
-    if (k >= 2) {
-      QX_PARAMS_SWITCH(h, PFB_MODE_SWITCH(mode, (k_hover_drain<MODE, PS><<<builders, kBlock, 0, s>>>(
-                                                     ps, h->hover, h->rng, h->d_counters + ((k + 2) % 4), h->d_done_list + ((k + 2) % 4) * h->n,
-                                                     h->d_elist + ((k + 2) % 4) * h->n, h->buf.start_pos, h->buf.start_orn, h->d_spare, h->d_episode,
-                                                     builders, h->n))));
-      LAUNCH_CHECK(h);
-    }
+    if (h->step_seq >= 2 && hover_drain(h, s)) return -1;
     QX_PARAMS_SWITCH(h, PFB_MODE_SWITCH(mode, (k_hover_spare_ahead<MODE, PS><<<tiles, kBlock, 0, s>>>(ps, h->hover, h->rng, h->buf.start_pos, h->buf.start_orn,
                                                                                                       h->d_spare, h->d_episode, h->n))));
     LAUNCH_CHECK(h);
     h->fused_ready = 1;
   }
-  int topup_grid = 8 * h->sm_count;
-  if (topup_grid > tiles) topup_grid = tiles;
   while (n_steps > 0) {
     const int T = n_steps < kRolloutMaxSteps ? n_steps : kRolloutMaxSteps;
     const uint64_t k0 = h->step_seq, k_last = k0 + (uint64_t)T - 1;
@@ -1185,10 +1196,7 @@ static int hover_rollout_fused(PfbContext* h, int n_steps, cudaStream_t s) {
                                                    h->buf.trunc, h->buf.info, h->buf.start_pos, h->buf.start_orn, h->d_spare, h->d_episode, h->d_counters + 5,
                                                    h->d_consumed, h->d_counters + (k_last % 4), h->d_done_list + (k_last % 4) * h->n, (uint32_t)k0, T, h->n))));
     LAUNCH_CHECK(h);
-    QX_PARAMS_SWITCH(h, PFB_MODE_SWITCH(mode, (k_hover_spare_topup<MODE, PS><<<topup_grid, kBlock, 0, s>>>(ps, h->hover, h->rng, h->buf.start_pos,
-                                                                                                           h->buf.start_orn, h->d_spare, h->d_counters + 5,
-                                                                                                           h->d_consumed, h->n))));
-    LAUNCH_CHECK(h);
+    if (hover_topup(h, h->d_counters + 5, s)) return -1;
     h->step_seq += (uint64_t)T;
     n_steps -= T;
   }
@@ -1199,16 +1207,10 @@ static int hover_rollout_fused(PfbContext* h, int n_steps, cudaStream_t s) {
 // taken off the queue the next launch would finish them from; the envs finished on the last launch stay queued, so that launch
 // builds their next spares.  Then every record fails its validity check: each env's next reset runs the cold path under
 // episode[i], the number the spare path would have used, and the builders / k_hover_spare_ahead replace the records.
-int hover_invalidate_spares(PfbContext* h, cudaStream_t s) {
+static int hover_invalidate_spares(PfbContext* h, cudaStream_t s) {
   const uint64_t k = h->step_seq;
   if (k >= 2) {
-    const int tiles = grid_for(h->n);
-    const int builders = h->sm_count < tiles ? h->sm_count : tiles;
-    QX_PARAMS_SWITCH(h, PFB_MODE_SWITCH(h->hover.flight_mode, (k_hover_drain<MODE, PS><<<builders, kBlock, 0, s>>>(
-                                                                   ps, h->hover, h->rng, h->d_counters + ((k + 2) % 4), h->d_done_list + ((k + 2) % 4) * h->n,
-                                                                   h->d_elist + ((k + 2) % 4) * h->n, h->buf.start_pos, h->buf.start_orn, h->d_spare,
-                                                                   h->d_episode, builders, h->n))));
-    LAUNCH_CHECK(h);
+    if (hover_drain(h, s)) return -1;
     CUDA_OK(cudaMemsetAsync(h->d_counters + ((k + 2) % 4), 0, sizeof(int32_t), s));
   }
   CUDA_OK(cudaMemset2DAsync(h->d_spare + SP_VALID, SP_ROWS * sizeof(float), 0, sizeof(float), (size_t)kSpareBufs * h->n, s));
@@ -1216,7 +1218,7 @@ int hover_invalidate_spares(PfbContext* h, cudaStream_t s) {
   return 0;
 }
 
-int hover_env_rollout(PfbContext* h, int n_steps, cudaStream_t s) {
+static int hover_env_rollout(PfbContext* h, int n_steps, cudaStream_t s) {
   if (h->env.autoreset == PFB_AUTORESET_SAME_STEP) {  // the same kernel as a single step, kRolloutMaxSteps steps per launch
     for (int k = 0; k < n_steps; k += kRolloutMaxSteps)
       if (hover_same_launch(h, h->buf.setpoint, true, n_steps - k < kRolloutMaxSteps ? n_steps - k : kRolloutMaxSteps, s)) return -1;
@@ -1227,3 +1229,31 @@ int hover_env_rollout(PfbContext* h, int n_steps, cudaStream_t s) {
     if (hover_env_step(h, h->buf.setpoint, nullptr, true, 0, s)) return -1;
   return 0;
 }
+
+const HandleOps kQuadXAviaryOps = {
+    .kind = PFB_KIND_QUADX, .env_kind = PFB_ENV_NONE,
+    .state_rows = QX_ROWS, .istate_rows = QI_ROWS, .layout = PFB_LAYOUT_WARP_TILED, .setpoint_dim = 4, .aux_dim = 4,
+    .obs_dim = hover_obs_dim,
+    .reset = qx_reset, .set_mode = qx_set_mode, .set_modes = qx_set_modes, .aviary_step = qx_aviary_step, .observe = qx_observe,
+    .set_base_state = qx_set_base_state, .get_base_state = qx_get_base_state,
+};
+
+const HandleOps kHoverOps = {
+    .kind = PFB_KIND_QUADX, .env_kind = PFB_ENV_QUADX_HOVER,
+    .state_rows = QX_ROWS, .istate_rows = QI_ROWS, .layout = PFB_LAYOUT_WARP_TILED, .setpoint_dim = 4, .aux_dim = 4,
+    .obs_dim = hover_obs_dim,
+    .reset = qx_reset, .set_mode = qx_set_mode, .aviary_step = qx_aviary_step, .observe = qx_observe,
+    .env_reset = hover_env_reset, .env_step = hover_env_step, .env_rollout = hover_env_rollout,
+    .spare_rows = SP_ROWS * kSpareBufs,
+    .consumed_rows = kRolloutMaxSteps / 2 + 1,  // an env resets at most every second step of a fused launch
+    .invalidate_spares = hover_invalidate_spares,
+};
+
+// MAQuadXHover: no autoreset, so no spares; its rollout falls back to single steps inside hover_env_rollout
+const HandleOps kMAQuadXHoverOps = {
+    .kind = PFB_KIND_QUADX, .env_kind = PFB_ENV_MA_QUADX_HOVER,
+    .state_rows = QM_ROWS, .istate_rows = QI_ROWS, .layout = PFB_LAYOUT_WARP_TILED, .setpoint_dim = 4, .aux_dim = 4,
+    .obs_dim = hover_obs_dim,
+    .reset = qx_reset, .set_mode = qx_set_mode, .aviary_step = qx_aviary_step, .observe = qx_observe,
+    .env_reset = hover_env_reset, .env_step = hover_env_step, .env_rollout = hover_env_rollout,
+};

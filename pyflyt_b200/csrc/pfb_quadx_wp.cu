@@ -20,9 +20,7 @@ enum { FLAG_QW_COMPLETE = 64 };
 constexpr int kQwObsMax = 21 + 4 * kMaxTargets;
 constexpr int kQwObsStride = kQwObsMax | 1;
 
-int qwp_state_rows() { return QW_ROWS; }
-int qwp_istate_rows() { return QWI_ROWS; }
-int qwp_obs_dim(const PfbContext* h) { return (h->hover.angle_representation == 0 ? 20 : 21) + (h->qwp.use_yaw_targets ? 4 : 3) * h->qwp.num_targets; }
+static int qwp_obs_dim(const PfbContext* h) { return (h->hover.angle_representation == 0 ? 20 : 21) + (h->qwp.use_yaw_targets ? 4 : 3) * h->qwp.num_targets; }
 
 struct QwState {
   float t0x, t0y, t0z, t0yaw;  // next target
@@ -161,8 +159,6 @@ __device__ __forceinline__ void qw_reset_env(const QuadXParams& p, const QxWaypo
 // ---- spare post-reset states (pfb_tail_step.cuh): a record holds the QW_* state words INCLUDING the episode's targets,
 // new_distance and yaw error
 enum { QSP_ROWS = 128 };
-int qwp_spare_rows() { return QSP_ROWS; }
-int qwp_spare_valid_row() { return QW_ROWS + SPARE_VALID; }
 
 // the QuadX-Waypoints env for tail_step (pfb_tail_step.cuh)
 template <int MODE, bool INJECT, bool RANDACT, class PS>
@@ -336,7 +332,7 @@ static auto qwp_launcher(PfbContext* h, float* actions, const float* noise) {
   };
 }
 
-int qwp_env_reset(PfbContext* h, const uint8_t* mask, const float* noise, cudaStream_t s) {
+static int qwp_env_reset(PfbContext* h, const uint8_t* mask, const float* noise, cudaStream_t s) {
   const uint32_t seq = 0x80000000u | (uint32_t)h->reset_seq++;
   const int mode = h->hover.flight_mode;
   auto reset = [&](int g) -> int {
@@ -352,6 +348,17 @@ int qwp_env_reset(PfbContext* h, const uint8_t* mask, const float* noise, cudaSt
   return 0;
 }
 
-int qwp_env_step(PfbContext* h, float* actions, const float* noise, bool randact, cudaStream_t s) {
+static int qwp_env_step(PfbContext* h, float* actions, const float* noise, bool randact, size_t, cudaStream_t s) {
   return tail_env_step(h, noise, randact, s, qwp_launcher(h, actions, noise));
 }
+
+// the QuadX Aviary surface (pfb_quadx.cu) over the field-major QW_* rows
+const HandleOps kQuadXWaypointsOps = {
+    .kind = PFB_KIND_QUADX, .env_kind = PFB_ENV_QUADX_WAYPOINTS,
+    .state_rows = QW_ROWS, .istate_rows = QWI_ROWS, .layout = PFB_LAYOUT_FIELD_MAJOR, .setpoint_dim = 4, .aux_dim = 4,
+    .obs_dim = qwp_obs_dim,
+    .reset = qx_reset, .set_mode = qx_set_mode, .aviary_step = qx_aviary_step, .observe = qx_observe,
+    .env_reset = qwp_env_reset, .env_step = qwp_env_step,
+    .spare_rows = QSP_ROWS, .spare_valid_row = QW_ROWS + SPARE_VALID,
+    .invalidate_spares = tail_invalidate_spares,
+};

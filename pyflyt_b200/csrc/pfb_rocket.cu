@@ -9,9 +9,7 @@
 using namespace pfb;
 
 int rk_build_params(const PfbModel& m, const PfbEnvConfig* env, RocketParams& p, LandingParams& l) { return rk_build_params_impl(m, env, p, l); }
-int rk_state_rows() { return RK_ROWS; }
-int rk_istate_rows() { return RI_ROWS; }
-int rk_obs_dim(const PfbContext* h) { return (h->land.angle_representation == 0 ? 12 : 13) + 7 + 9 + 1; }
+static int rk_obs_dim(const PfbContext* h) { return (h->land.angle_representation == 0 ? 12 : 13) + 7 + 9 + 1; }
 
 // ---------------------------------------------------------------------------------------------------
 // kernels — Aviary surface
@@ -186,8 +184,6 @@ constexpr int kLandBlocks = 8;
 
 // ---- spare post-reset states (pfb_tail_step.cuh): a record holds the RK_* state words
 enum { LSP_ROWS = 64 };
-int rk_spare_rows() { return LSP_ROWS; }
-int rk_spare_valid_row() { return RK_ROWS + SPARE_VALID; }
 
 // the Rocket-Landing env for tail_step (pfb_tail_step.cuh)
 template <bool INJECT, bool RANDACT>
@@ -320,27 +316,34 @@ __global__ void __launch_bounds__(kBlock)
 // ---------------------------------------------------------------------------------------------------
 // launchers
 // ---------------------------------------------------------------------------------------------------
-int rk_reset(PfbContext* h, const uint8_t* mask, cudaStream_t s) {
+static int rk_reset(PfbContext* h, const uint8_t* mask, cudaStream_t s) {
   k_rk_reset<<<grid_for(h->n), kBlock, 0, s>>>(h->rk, h->buf.state, h->buf.istate, h->buf.setpoint, h->buf.start_pos, h->buf.start_orn, mask, h->n);
   LAUNCH_CHECK(h);
   if (!mask) h->mode = 0;
   return 0;
 }
 
-int rk_set_base_state(PfbContext* h, const BaseStateIn& a, cudaStream_t s) {
+static int rk_set_base_state(PfbContext* h, const BaseStateIn& a, cudaStream_t s) {
   if (a.lin32 || a.ang32) k_rk_set_base_state<true><<<grid_for(h->n), kBlock, 0, s>>>(a, h->buf.state, h->buf.istate, h->n);
   else k_rk_set_base_state<false><<<grid_for(h->n), kBlock, 0, s>>>(a, h->buf.state, h->buf.istate, h->n);
   LAUNCH_CHECK(h);
   return 0;
 }
 
-int rk_get_base_state(PfbContext* h, const BaseStateOut& o, cudaStream_t s) {
+static int rk_get_base_state(PfbContext* h, const BaseStateOut& o, cudaStream_t s) {
   k_rk_get_base_state<<<grid_for(h->n), kBlock, 0, s>>>(o, h->buf.state, h->buf.istate, h->n);
   LAUNCH_CHECK(h);
   return 0;
 }
 
-int rk_aviary_step(PfbContext* h, int n_steps, const float* noise, cudaStream_t s) {
+static int rk_set_mode(PfbContext* h, int mode, cudaStream_t) {  // the rocket's one mode: nothing to preset
+  if (mode < kModeLo[PFB_KIND_ROCKET] || mode > kModeHi[PFB_KIND_ROCKET])  // the message of base_drone.py:252-255
+    return fail("`mode` must be either 0 or be registered in self.registered_controllers.keys()=dict_keys([]), got %d.", mode);
+  h->mode = 0;
+  return 0;
+}
+
+static int rk_aviary_step(PfbContext* h, int n_steps, const float* noise, cudaStream_t s) {
   const uint32_t seq = (uint32_t)h->aviary_seq++;
   const int g = grid_for(h->n);
   if (noise) k_rk_aviary_step<true><<<g, kBlock, 0, s>>>(h->rk, h->rng, h->buf.state, h->buf.istate, h->buf.setpoint, noise, n_steps, seq, h->n);
@@ -349,7 +352,7 @@ int rk_aviary_step(PfbContext* h, int n_steps, const float* noise, cudaStream_t 
   return 0;
 }
 
-int rk_observe(PfbContext* h, cudaStream_t s) {
+static int rk_observe(PfbContext* h, cudaStream_t s) {
   k_rk_observe<<<grid_for(h->n), kBlock, 0, s>>>(h->buf.state, h->buf.istate, h->buf.drone_state, h->buf.aux_state, h->buf.contact, h->n);
   LAUNCH_CHECK(h);
   return 0;
@@ -374,7 +377,7 @@ static auto land_launcher(PfbContext* h, float* actions, const float* noise) {
   };
 }
 
-int rk_env_reset(PfbContext* h, const uint8_t* mask, const float* noise, cudaStream_t s) {
+static int rk_env_reset(PfbContext* h, const uint8_t* mask, const float* noise, cudaStream_t s) {
   const uint32_t seq = 0x80000000u | (uint32_t)h->reset_seq++;
   // an explicit env.reset() honours the bound start_pos / start_orn unless randomize_drop is configured
   const int randomize = h->land.randomize_drop;
@@ -392,6 +395,26 @@ int rk_env_reset(PfbContext* h, const uint8_t* mask, const float* noise, cudaStr
   return 0;
 }
 
-int rk_env_step(PfbContext* h, float* actions, const float* noise, bool randact, cudaStream_t s) {
+static int rk_env_step(PfbContext* h, float* actions, const float* noise, bool randact, size_t, cudaStream_t s) {
   return tail_env_step(h, noise, randact, s, land_launcher(h, actions, noise));
 }
+
+// every mode list a rocket handle accepts is uniform (mode 0): pfb_set_modes never gets to set_modes
+const HandleOps kRocketAviaryOps = {
+    .kind = PFB_KIND_ROCKET, .env_kind = PFB_ENV_NONE,
+    .state_rows = RK_ROWS, .istate_rows = RI_ROWS, .layout = PFB_LAYOUT_FIELD_MAJOR, .setpoint_dim = 7, .aux_dim = 9,
+    .obs_dim = rk_obs_dim,
+    .reset = rk_reset, .set_mode = rk_set_mode, .aviary_step = rk_aviary_step, .observe = rk_observe,
+    .set_base_state = rk_set_base_state, .get_base_state = rk_get_base_state,
+};
+
+const HandleOps kRocketLandingOps = {
+    .kind = PFB_KIND_ROCKET, .env_kind = PFB_ENV_ROCKET_LANDING,
+    .state_rows = RK_ROWS, .istate_rows = RI_ROWS, .layout = PFB_LAYOUT_FIELD_MAJOR, .setpoint_dim = 7, .aux_dim = 9,
+    .obs_dim = rk_obs_dim,
+    .reset = rk_reset, .set_mode = rk_set_mode, .aviary_step = rk_aviary_step, .observe = rk_observe,
+    .set_base_state = rk_set_base_state,  // pfb_set_base_velocity: the env's reset calls it (rocket_base_env.py:228)
+    .env_reset = rk_env_reset, .env_step = rk_env_step,
+    .spare_rows = LSP_ROWS, .spare_valid_row = RK_ROWS + SPARE_VALID,
+    .invalidate_spares = tail_invalidate_spares,
+};
