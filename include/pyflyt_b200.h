@@ -59,6 +59,10 @@ extern "C" {
 #define PFB_SHAPE_CYLINDER 1
 #define PFB_SHAPE_SPHERE 2
 
+/* Static (fixed-base) bodies per Aviary handle, and their collision primitives in all (pfb_add_static_body) */
+#define PFB_MAX_STATIC_BODIES 8
+#define PFB_MAX_STATIC_SHAPES 16
+
 /* One collision primitive used for the ground / pad contact FLAG (no contact response). */
 typedef struct PfbShape {
   int32_t kind;
@@ -369,6 +373,34 @@ int pfb_set_base_state(PfbHandle h, const uint8_t* mask, const double* pos, cons
 int pfb_get_base_state(PfbHandle h, double* pos, double* quat, double* lin_vel, double* ang_vel, void* stream);
 /* Fills drone_state / aux_state / contact (Aviary.state(i), aux_state(i), contact_array).            */
 int pfb_observe_state(PfbHandle h, void* stream);
+
+/* ---- static bodies (DESIGN.md §4h): the reference's loadURDF(..., useFixedBase=True) of a landing pad, a helipad or a
+ * rooftop.  Aviary handles only.  A body is 1..PFB_MAX_STATIC_SHAPES boxes and cylinders (PfbShape: `at` / `rot` in the
+ * body's base link frame; box half extents, cylinder radius and half length), each upright once posed: a box may be yawed,
+ * a cylinder's axis is vertical.  Every drone's world holds its own copy of each body.  A primitive is UNDER drone i when
+ * its footprint holds the base's (x, y) and z + R_b >= its top (R_b: the model's contact reach); the contact flag of a body
+ * is the drone's flag against the top of each primitive under it, and the contact response (contact_response) runs against
+ * the highest surface under the drone (the floor, z = 0, or a top).  Side faces are not solid.  pfb_reset with mask = NULL
+ * removes every static body (Aviary.reset calls resetSimulation).                                                        */
+typedef PfbShape PfbStaticShape;
+/* Reads the collision primitives of a URDF (fixed joints; boxes, cylinders, spheres) in its base link frame, scaled by
+ * global_scaling, and the origin of the base link's inertial frame in that frame (which may be offset, not rotated).
+ * *n_shapes = their number; at most `cap` are written (more: an error).  Meshes are refused.                           */
+int pfb_static_shapes_from_urdf(const char* urdf_path, double global_scaling, PfbStaticShape* out, int cap, int* n_shapes,
+                                double inertial_origin[3]);
+/* loadURDF(useFixedBase=True): adds body *body_id = 0, 1, ... to every drone's world with its base LINK frame at pos[3],
+ * quat[4] (x, y, z, w; host fp64; upright).  inertial_origin[3] (NULL = 0): the base inertial frame in the link frame, which
+ * pfb_set_static_pose places.                                                                                           */
+int pfb_add_static_body(PfbHandle h, const PfbStaticShape* shapes, int n_shapes, const double pos[3], const double quat[4],
+                        const double inertial_origin[3], int* body_id, void* stream);
+/* resetBasePositionAndOrientation of static body `body` in the worlds of the drones of `mask` ([N], NULL = all): device fp64
+ * pos [N][3], quat [N][4] (x, y, z, w) of its base INERTIAL frame, as PyBullet's reset places it.  Every quaternion of a
+ * drone in the mask must be upright (a yaw about z: 1 - R22 <= 1e-9), else the call fails and changes nothing.  The check
+ * reads the quaternions back to the host: this call synchronises `stream`.                                              */
+int pfb_set_static_pose(PfbHandle h, int body, const double* pos, const double* quat, const uint8_t* mask, void* stream);
+/* bits[i] (device [N]): what drone i touched during the last pfb_aviary_step, bit 0 the floor, bit 1 + k static body k;
+ * zero from the first body added after a full pfb_reset until the next step.                                            */
+int pfb_get_static_contacts(PfbHandle h, uint32_t* bits, void* stream);
 
 /* ---- gymnasium-env surface ----------------------------------------------------------------------- */
 /* env.reset(): begin_reset + end_reset (quadx_base_env.py:149-212): pose reset, set_mode, warm-up

@@ -83,6 +83,10 @@ def lib() -> C.CDLL:
     L.pfb_set_modes.argtypes = [vp, vp, vp]
     L.pfb_aviary_step.argtypes = [vp, i32, vp, vp]
     L.pfb_observe_state.argtypes = [vp, vp]
+    L.pfb_static_shapes_from_urdf.argtypes = [C.c_char_p, C.c_double, vp, i32, vp, vp]
+    L.pfb_add_static_body.argtypes = [vp, vp, i32, vp, vp, vp, vp, vp]
+    L.pfb_set_static_pose.argtypes = [vp, i32, vp, vp, vp, vp]
+    L.pfb_get_static_contacts.argtypes = [vp, vp, vp]
     L.pfb_set_base_velocity.argtypes = [vp, vp, vp, vp]
     L.pfb_set_base_state.argtypes = [vp, vp, vp, vp, vp, vp, vp]
     L.pfb_get_base_state.argtypes = [vp, vp, vp, vp, vp, vp]
@@ -117,6 +121,7 @@ EXPORTS = [
     "pfb_istate_rows", "pfb_setpoint_dim",
     "pfb_obs_dim", "pfb_aux_dim", "pfb_bind", "pfb_reset", "pfb_set_mode", "pfb_set_modes", "pfb_aviary_step", "pfb_observe_state",
     "pfb_set_base_velocity", "pfb_set_base_state", "pfb_get_base_state",
+    "pfb_static_shapes_from_urdf", "pfb_add_static_body", "pfb_set_static_pose", "pfb_get_static_contacts",
     "pfb_env_reset", "pfb_env_step", "pfb_env_rollout", "pfb_env_step_host", "pfb_env_step_mapped", "pfb_launch_count",
     "pfb_profile_begin", "pfb_profile_read", "pfb_dogfight_payload_dim", "pfb_dogfight_physics", "pfb_dogfight_physics_peer", "pfb_dogfight_combat", "pfb_dogfight_combat_wait", "pfb_dogfight_split_step",
 ]  # every symbol include/pyflyt_b200.h declares

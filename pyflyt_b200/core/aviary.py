@@ -38,6 +38,12 @@ Aviary step), and drone ``i`` runs its controller on the physics steps that are 
 Such a batch is a mixed handle whatever its kinds, with the surface described above (``setpoints`` ``[N, 7]``); a batch whose
 rates turn out equal is the batch built without the option (DESIGN.md §4e).
 
+Static bodies: ``loadURDF(fileName, basePosition, baseOrientation, useFixedBase=True)`` (then ``register_all_new_bodies()``, kept
+for script compatibility) puts a landing pad, a helipad or a rooftop into every drone's world, as the reference's
+``aviary.loadURDF`` does; ``set_static_pose`` moves a body in the worlds of a mask of drones, and ``contact_bodies()`` says
+which body each drone touched.  Up to ``MAX_STATIC_BODIES`` bodies of ``MAX_STATIC_SHAPES`` boxes and cylinders in all,
+upright; only their top faces are solid (DESIGN.md §4h).  ``reset()`` removes them, as the reference's ``resetSimulation`` does.
+
 All state is held in caller-visible ``torch`` tensors; the CUDA library (libpyflyt_b200.so) only sees
 raw device pointers.  There is no CPU path.
 """
@@ -45,18 +51,28 @@ raw device pointers.  There is no CPU path.
 from __future__ import annotations
 
 import ctypes as C
+import os
 from typing import Any, Sequence
 
 import numpy as np
 import torch
 
 from .. import _lib
-from ..models import ModelSetError, PfbEnvConfig, PfbModel, build_mixed_model_set, build_model, build_model_set
+from ..models import ModelSetError, PfbEnvConfig, PfbModel, PfbShape, build_mixed_model_set, build_model, build_model_set
 
 _KINDS = ("quadx", "fixedwing", "rocket")
 _MODE_RANGE = {"quadx": (-1, 7), "fixedwing": (-1, 0), "rocket": (0, 0)}  # quadx.py:259-262, fixedwing.py:216-219, base_drone.py:252-255
 _SETPOINT_LEN = {"quadx": (4,), "fixedwing": (4, 6), "rocket": (7,)}
 _AUX_LEN = {"quadx": 4, "fixedwing": 6, "rocket": 9}
+MAX_STATIC_BODIES = 8  # PFB_MAX_STATIC_BODIES
+MAX_STATIC_SHAPES = 16  # PFB_MAX_STATIC_SHAPES
+
+
+def _upright_error(quat: np.ndarray) -> float:
+    """Largest 1 - R22 over unit quaternions (x, y, z, w): 0 for a pure yaw."""
+    q = np.asarray(quat, dtype=np.float64).reshape(-1, 4)
+    n = np.sum(q * q, axis=1)
+    return float(np.max(2.0 * (q[:, 0] ** 2 + q[:, 1] ** 2) / n)) if len(q) else 0.0
 
 
 def _check_mode(kind: str, mode: int) -> None:
@@ -237,6 +253,7 @@ class BatchedAviary:
         self._buffers = b
         _lib.check(L.pfb_bind(self._h, C.byref(b)))
         self._state_fresh = False
+        self.static_bodies: list[str] = []  # the URDF of each static body (loadURDF), by body index
         self.reset()
 
     # ------------------------------------------------------------------ lifecycle
@@ -259,6 +276,7 @@ class BatchedAviary:
     def reset(self) -> None:
         """aviary.py:218-312: every drone back to its start pose, mode 0, zero setpoint."""
         _lib.check(_lib.lib().pfb_reset(self._h, None, self._s()))
+        self.static_bodies = []  # pfb_reset removed them (resetSimulation)
         self.physics_steps = 0
         self.aviary_steps = 0
         self.elapsed_time = 0.0
@@ -386,6 +404,82 @@ class BatchedAviary:
                                                  C.c_void_p(ang.data_ptr()), self._s()))
         return pos, quat, lin, ang
 
+    # ------------------------------------------------------------------ static bodies (DESIGN.md §4h)
+    def loadURDF(self, fileName: str, basePosition=(0.0, 0.0, 0.0), baseOrientation=None, useFixedBase: bool = True,
+                 globalScaling: float = 1.0) -> int:
+        """The reference's ``aviary.loadURDF`` of a fixed-base body (a landing pad, a helipad, a rooftop), placed in every drone's
+        world with its base link frame at ``basePosition`` / ``baseOrientation`` (x, y, z, w; None = identity).  Returns the
+        body index ``k``: column ``1 + k`` of ``contact_bodies()``.  The body must be boxes and cylinders joined by fixed joints,
+        upright once posed (a yaw only); spheres, meshes, tilted poses and ``useFixedBase=False`` are refused.  Aviary handles
+        only."""
+        if self.env_config is not None and self.env_config.env_kind != 0:
+            raise AviaryInitException("static bodies are for Aviary handles; an env handle (env_config) keeps its own floor and pad.")
+        if not useFixedBase:
+            raise ValueError("only fixed-base bodies (useFixedBase=True) can be loaded: a free body would need contact between bodies.")
+        pos = np.asarray(basePosition, dtype=np.float64).reshape(-1)
+        quat = np.asarray((0.0, 0.0, 0.0, 1.0) if baseOrientation is None else baseOrientation, dtype=np.float64).reshape(-1)
+        if pos.shape != (3,) or quat.shape != (4,):
+            raise ValueError(f"basePosition must have 3 entries and baseOrientation 4, got {pos.shape[0]} and {quat.shape[0]}.")
+        if not abs(float(np.linalg.norm(quat)) - 1.0) <= 1e-6:
+            raise ValueError("baseOrientation must be a unit quaternion (x, y, z, w).")
+        path = str(fileName)
+        if not os.path.isfile(path):
+            raise FileNotFoundError(f"cannot find the URDF {fileName!r}")
+        L = _lib.lib()
+        shapes = (PfbShape * MAX_STATIC_SHAPES)()
+        n = C.c_int(0)
+        inertial = (C.c_double * 3)()
+        _lib.check(L.pfb_static_shapes_from_urdf(path.encode(), float(globalScaling), shapes, MAX_STATIC_SHAPES, C.byref(n), inertial))
+        body = C.c_int(-1)
+        p3, q4 = (C.c_double * 3)(*pos), (C.c_double * 4)(*quat)
+        _lib.check(L.pfb_add_static_body(self._h, shapes, n.value, p3, q4, inertial, C.byref(body), self._s()))
+        self.static_bodies.append(path)
+        return int(body.value)
+
+    def register_all_new_bodies(self) -> None:
+        """The reference registers new bodies for its contact array (aviary.py:314-320); here every loaded body is registered
+        by ``loadURDF``.  Kept so that scripts run unchanged."""
+
+    def set_static_pose(self, body: int, pos, quat=None, mask=None) -> None:
+        """``resetBasePositionAndOrientation`` of static body ``body`` in the worlds of the drones of ``mask`` ([N] bool; None =
+        every drone): ``pos`` [N, 3] or [3], ``quat`` [N, 4] or [4] (x, y, z, w; None = identity), fp64, upright (a yaw only).
+        As in PyBullet, the pose is that of the body's base INERTIAL frame (``loadURDF``'s ``basePosition`` places its base link
+        frame; the two differ by the inertial origin of the URDF's base link).  Each drone's world keeps its own pose, so every
+        drone may get a different one (randomised pads)."""
+        n = self.num_drones
+        if not 0 <= int(body) < len(self.static_bodies):
+            raise ValueError(f"no static body {body}: {len(self.static_bodies)} loaded since the last reset().")
+        p = np.broadcast_to(np.asarray(pos, dtype=np.float64), (n, 3)) if np.asarray(pos).ndim == 1 else np.asarray(pos, dtype=np.float64)
+        q = np.asarray((0.0, 0.0, 0.0, 1.0) if quat is None else quat, dtype=np.float64)
+        q = np.broadcast_to(q, (n, 4)) if q.ndim == 1 else q
+        if p.shape != (n, 3) or q.shape != (n, 4):
+            raise ValueError(f"pos must be shape ({n}, 3) or (3,) and quat ({n}, 4) or (4,), got {p.shape} and {q.shape}.")
+        err = float(np.max(np.abs(np.linalg.norm(q, axis=1) - 1.0))) if n else 0.0
+        if not err <= 1e-6:
+            raise ValueError(f"quat must be unit quaternions (x, y, z, w): a norm differs from 1 by {err:.3g} (> 1e-6).")
+        if not _upright_error(q) <= 1e-9:
+            raise ValueError("static bodies stay upright: quat must be a yaw about the world z axis (tilted static bodies are not modelled).")
+        pt = torch.as_tensor(np.ascontiguousarray(p), device=self.device)
+        qt = torch.as_tensor(np.ascontiguousarray(q), device=self.device)
+        m = None
+        if mask is not None:
+            m = torch.as_tensor(mask, device=self.device)
+            if tuple(m.shape) != (n,):
+                raise ValueError(f"mask must be shape ({n},), got {tuple(m.shape)}.")
+            m = m.to(torch.uint8).contiguous()
+        _lib.check(_lib.lib().pfb_set_static_pose(self._h, int(body), C.c_void_p(pt.data_ptr()), C.c_void_p(qt.data_ptr()),
+                                                  None if m is None else C.c_void_p(m.data_ptr()), self._s()))
+
+    def contact_bodies(self) -> torch.Tensor:
+        """(N, 1 + M) bool, M = static bodies loaded: column 0 the floor, column 1 + k static body k, touched during the last
+        ``step()`` — the reference's ``contact_array[drone.Id, body_id]``.  ``contact_array`` is their ``any``."""
+        if not self.static_bodies:
+            return self.contact_array.reshape(-1, 1)
+        bits = torch.empty((self.num_drones,), dtype=torch.int32, device=self.device)
+        _lib.check(_lib.lib().pfb_get_static_contacts(self._h, C.c_void_p(bits.data_ptr()), self._s()))
+        cols = torch.arange(1 + len(self.static_bodies), dtype=torch.int32, device=self.device)
+        return ((bits[:, None] >> cols[None, :]) & 1).bool()
+
     def _refresh(self):
         if not self._state_fresh:
             _lib.check(_lib.lib().pfb_observe_state(self._h, self._s()))
@@ -416,7 +510,8 @@ class BatchedAviary:
 
     @property
     def contact_array(self) -> torch.Tensor:
-        """(N,) bool: ground contact during the last step (aviary.py:322, 523-525, per world)."""
+        """(N,) bool: contact with the floor or any static body during the last step (aviary.py:322, 523-525, per world; the
+        reference's ``np.any(contact_array[drone.Id])``)."""
         self._refresh()
         return self._contact.bool()
 

@@ -111,7 +111,26 @@ struct PfbContext {
   // mixed-kind Aviary handle (pfb_create_mixed, pfb_mixed.cu): the drones of each kind and their slots; nullptr = one kind
   struct MixedKinds* mixed;
   const struct HandleOps* ops;  // what the handle's kind runs, set once at creation
+  // static bodies of an Aviary handle (pfb_add_static_body, pfb_static.cu); nullptr until the first one is added
+  struct StaticBodies* statics;
 };
+
+// ---- static bodies (pfb_static.cu; DESIGN.md §4h) ----------------------------------------------------------------------------
+static_assert(pfb::kMaxStaticBodies == PFB_MAX_STATIC_BODIES && pfb::kMaxStaticShapes == PFB_MAX_STATIC_SHAPES, "static-body caps");
+struct StaticBodies {
+  pfb::StaticWorld world;  // the primitive table every step launch with static bodies takes as a kernel parameter
+  int n_bodies;
+  double inertial[pfb::kMaxStaticBodies][3];  // each body's base inertial origin in its link frame (pfb_set_static_pose places it)
+  float* d_pose;           // [kStaticPoseRows * kMaxStaticBodies][n]: x, y, z, cos yaw, sin yaw of body b in drone i's world
+  uint32_t* d_bits;        // [n], user order: bit 0 the floor, bit 1 + b body b, touched during the last Aviary step
+};
+// The static bodies an Aviary step launch flies against; nullptr = none: the handle launches the kernels it launched before
+// static bodies existed
+static inline const StaticBodies* step_statics(const PfbContext* h) {
+  return (h->statics && h->statics->n_bodies > 0) ? h->statics : nullptr;
+}
+void static_destroy(PfbContext* h);
+void static_clear(PfbContext* h);  // a full pfb_reset: the bodies go, as the reference's resetSimulation removes them
 
 // The device lookup, then a zeroed handle for n drones / envs on `device` with its Philox key and counters, which `setup(c)`
 // completes (0 or the result of fail()).  On every failure path everything allocated is freed and *out is left alone.

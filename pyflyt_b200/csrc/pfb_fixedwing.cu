@@ -70,6 +70,32 @@ __global__ void __launch_bounds__(kBlock, kMinBlocks)
   fixedwing_store(st, ist, N, i, s);
 }
 
+// n_steps x Aviary.step() against the static bodies of each drone's world (pfb_add_static_body; Aviary handles, 6-wide setpoints):
+// one flight mode MODE, or MODE = kStaticPerDrone = drone i in modes[i].  bits[i]: what drone i touched during its last Aviary step.
+constexpr int kStaticPerDrone = 1;
+template <int MODE, bool INJECT, bool CONTACT>
+__global__ void __launch_bounds__(kBlock, kMinBlocks)
+    k_fw_aviary_step_static(const __grid_constant__ FixedwingParams p, const __grid_constant__ RngParams rng, const __grid_constant__ StaticWorld world,
+                            const float* __restrict__ pose, uint32_t* __restrict__ bits, float* __restrict__ st, int32_t* __restrict__ ist,
+                            const float* __restrict__ setpoint, const int8_t* __restrict__ modes, const float* __restrict__ noise, int n_steps,
+                            uint32_t seq, int64_t N) {
+  int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= N) return;
+  StaticCtx w{&world, pose, N, i, 0u};
+  FixedwingRegs s;
+  fixedwing_load(st, ist, N, i, s);
+  load_setpoint<6, 6>(setpoint, i, s.sp);
+  const int mode = MODE == kStaticPerDrone ? modes[i] : MODE;
+  auto nz = make_noise<INJECT>(noise, N, i, rng, seq, TAG_AVIARY, p.noise_loc, p.ratio);
+  if (fixedwing_full_model(p)) {
+    for (int k = 0; k < n_steps; ++k) fixedwing_aviary_step_any<true, CONTACT>(p, s, mode, nz, &w);
+  } else {
+    for (int k = 0; k < n_steps; ++k) fixedwing_aviary_step_any<false, CONTACT>(p, s, mode, nz, &w);
+  }
+  fixedwing_store(st, ist, N, i, s);
+  bits[i] = w.bits;
+}
+
 // k_fw_aviary_step with drone i in flight mode modes[i] (pfb_set_modes; step body fixedwing_aviary_step_any)
 template <bool INJECT, bool CONTACT>
 __global__ void __launch_bounds__(kBlock, kMinBlocks)
@@ -399,6 +425,19 @@ int fw_aviary_step(PfbContext* h, int n_steps, const float* noise, cudaStream_t 
   const uint32_t seq = (uint32_t)h->aviary_seq++;
   const int g = grid_for(h->n);
   const bool contact = aviary_contact_response(h);
+  if (const StaticBodies* sb = step_statics(h)) {  // Aviary handles only (6-wide setpoints)
+#define FWS_ARGS h->fw, h->rng, sb->world, sb->d_pose, sb->d_bits, h->buf.state, h->buf.istate, h->buf.setpoint, h->d_modes, noise, n_steps, seq, h->n
+#define FWS_LAUNCH(M) \
+    if (contact) { if (noise) k_fw_aviary_step_static<M, true, true><<<g, kBlock, 0, s>>>(FWS_ARGS); else k_fw_aviary_step_static<M, false, true><<<g, kBlock, 0, s>>>(FWS_ARGS); } \
+    else { if (noise) k_fw_aviary_step_static<M, true, false><<<g, kBlock, 0, s>>>(FWS_ARGS); else k_fw_aviary_step_static<M, false, false><<<g, kBlock, 0, s>>>(FWS_ARGS); }
+    if (h->mode == kModePerDrone) { FWS_LAUNCH(kStaticPerDrone) }
+    else if (h->mode == 0) { FWS_LAUNCH(0) }
+    else { FWS_LAUNCH(-1) }
+#undef FWS_LAUNCH
+#undef FWS_ARGS
+    LAUNCH_CHECK(h);
+    return 0;
+  }
   if (h->mode == kModePerDrone) {  // pfb_set_modes: Aviary handles only (6-wide setpoints)
 #define FWM_ARGS h->fw, h->rng, h->buf.state, h->buf.istate, h->buf.setpoint, h->d_modes, noise, n_steps, seq, h->n
     if (contact) {

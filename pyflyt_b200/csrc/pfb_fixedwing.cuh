@@ -205,6 +205,40 @@ PFB_HD bool ground_contact(const ContactParams& cp, float pz, float r20, float r
   return hit;
 }
 
+// Surface height under the drone at (px, py, pz) of world i and its contact bits (DESIGN.md §4h).  A static primitive is under
+// the drone when its footprint (a disc, or a yawed rectangle) holds (px, py) and pz + reach >= its top, reach = the model's
+// contact reach about its base origin (contact_zmax / ContactParams::zmax).  The surface is the highest of the floor (0) and
+// the tops under the drone; touch(top) is the drone's contact flag against the plane z = top, bit 0 = touch(0), bit 1 + b =
+// touch(top) against any primitive of body b under the drone.  Side faces are not solid.
+template <class Touch>
+PFB_HD float static_surface(const StaticWorld& w, const float* pose, int64_t n, int64_t i, float px, float py, float pz, float reach,
+                            Touch&& touch, uint32_t& bits) {
+  float surf = 0.0f;
+  uint32_t b = touch(0.0f) ? 1u : 0u;
+#pragma unroll 1
+  for (int k = 0; k < w.n_shapes; ++k) {
+    const int body = w.body[k];
+    const float* q = pose + (int64_t)kStaticPoseRows * body * n + i;
+    const float bx = q[0], by = q[n], bz = q[2 * n], c = q[3 * n], sn = q[4 * n];
+    const float top = bz + w.at[k][2] + w.half[k][2];
+    if (pz + reach < top) continue;  // the drone is below this top face: side faces are not solid
+    const float dx = px - (bx + c * w.at[k][0] - sn * w.at[k][1]);
+    const float dy = py - (by + sn * w.at[k][0] + c * w.at[k][1]);
+    bool inside;
+    if (w.kind[k] == 0) {  // the rectangle's own axes: body yaw + primitive yaw
+      const float cy = c * w.cyaw[k] - sn * w.syaw[k], sy = sn * w.cyaw[k] + c * w.syaw[k];
+      inside = fabsf(cy * dx + sy * dy) <= w.half[k][0] && fabsf(cy * dy - sy * dx) <= w.half[k][1];
+    } else {
+      inside = dx * dx + dy * dy <= w.half[k][0] * w.half[k][0];
+    }
+    if (!inside) continue;
+    surf = fmaxf(surf, top);
+    if (touch(top)) b |= 2u << body;
+  }
+  bits = b;
+  return surf;
+}
+
 // ---- contact RESPONSE (opt-in: PfbEnvConfig.contact_response): the arithmetic of oracle/fakebullet/pybullet.py::_solve_contacts
 // and oracle/pfb_oracle.c::solve_contacts, in the BODY frame (the inverse central inertia is constant there): candidate points =
 // 8 per collision primitive (box corners; 4 + 4 cylinder rim points), kContactIterations sweeps, per penetrating point a
@@ -232,7 +266,9 @@ PFB_HD Vec3 contact_point(const QuadXParams& p, int k, float lx, float ly, float
   return Vec3{p.shape_at[k][0] + lx, p.shape_at[k][1] + ly, p.shape_at[k][2] + lz};
 }
 
-template <class Shapes>
+// Tag: NoStatic, or StaticCtx on the static-body path, which passes a surface height that varies; its own copy of the solver
+// keeps the floor-only kernels' copy, into which the compiler may fold their constant height 0, as it was.
+template <class Tag = NoStatic, class Shapes>
 #if defined(__CUDACC__)
 static __host__ __device__ __noinline__
 #else
@@ -296,14 +332,14 @@ ContactVel solve_contacts(const Shapes* cp, float pz, float top, Vec3 n /* world
 // Contact impulses on the predicted velocities of `s` (world linear velocity, body angular velocity), before its pose is
 // integrated: the solve runs in the body frame of the pose at the START of the substep (rotation s.R, base altitude pz0).
 // M, c, I..: mass, COM offset and inertia about the COM (base frame).
-template <class Shapes, class Regs>
+template <class Tag, class Shapes, class Regs>
 PFB_HD void apply_contact_impulses(const Shapes* cp, Regs& s, float pz0, float top, float M, Vec3 c, float Ixx, float Ixy, float Ixz,
                                    float Iyy, float Iyz, float Izz, float dt) {
   const float m00 = (float)s.R.m00, m01 = (float)s.R.m01, m02 = (float)s.R.m02, m10 = (float)s.R.m10, m11 = (float)s.R.m11,
               m12 = (float)s.R.m12, m20 = (float)s.R.m20, m21 = (float)s.R.m21, m22 = (float)s.R.m22;
   const float vwx = (float)s.vx, vwy = (float)s.vy, vwz = (float)s.vz;
   const Vec3 vbn = Vec3{m00 * vwx + m10 * vwy + m20 * vwz, m01 * vwx + m11 * vwy + m21 * vwz, m02 * vwx + m12 * vwy + m22 * vwz};
-  const ContactVel cv = solve_contacts(cp, pz0, top, Vec3{m20, m21, m22}, vbn, Vec3{s.wx, s.wy, s.wz}, M, c, Ixx, Ixy, Ixz, Iyy, Iyz, Izz, dt);
+  const ContactVel cv = solve_contacts<Tag>(cp, pz0, top, Vec3{m20, m21, m22}, vbn, Vec3{s.wx, s.wy, s.wz}, M, c, Ixx, Ixy, Ixz, Iyy, Iyz, Izz, dt);
   if (cv.touched) {
     s.vx = (vreal)(m00 * cv.vx + m01 * cv.vy + m02 * cv.vz);
     s.vy = (vreal)(m10 * cv.vx + m11 * cv.vy + m12 * cv.vz);
@@ -318,9 +354,10 @@ PFB_HD void apply_contact_impulses(const Shapes* cp, Regs& s, float pz0, float t
 // same semi-implicit Euler + body-frame exp-map as the quad.
 // CONTACT: contact impulses over `cp` on the predicted velocities when `touching` (the substep's contact flag), before the
 // pose is integrated.
-template <bool CONTACT = false, typename Regs>
+// Tag: as solve_contacts (`top`: the surface height of the response).
+template <bool CONTACT = false, class Tag = NoStatic, typename Regs>
 PFB_HD void rigid_step(const RigidParams& rb, float gravity, float dt_f, float vmax_f, Regs& s, Vec3 F, Vec3 T,
-                       const ContactParams* cp = nullptr, bool touching = false) {
+                       const ContactParams* cp = nullptr, bool touching = false, float top = 0.0f) {
   typedef decltype(s.R.m00) RT;  // the body's rotation-matrix precision (fwreal for aircraft, rreal for the rocket)
   const Rot<RT>& R = s.R;
   const float r20 = (float)R.m20, r21 = (float)R.m21, r22 = (float)R.m22;
@@ -375,7 +412,7 @@ PFB_HD void rigid_step(const RigidParams& rb, float gravity, float dt_f, float v
       const float M = rb.mass, iM = 1.0f / M;
       const Vec3 c = Vec3{rb.mc[0] * iM, rb.mc[1] * iM, rb.mc[2] * iM};
       const float c2 = dot(c, c);
-      apply_contact_impulses(cp, s, (float)s.pz, 0.0f, M, c, rb.I[0] - M * (c2 - c.x * c.x), rb.I[1] + M * c.x * c.y, rb.I[2] + M * c.x * c.z,
+      apply_contact_impulses<Tag>(cp, s, (float)s.pz, top, M, c, rb.I[0] - M * (c2 - c.x * c.x), rb.I[1] + M * c.x * c.y, rb.I[2] + M * c.x * c.z,
                              rb.I[4] - M * (c2 - c.y * c.y), rb.I[5] + M * c.y * c.z, rb.I[8] - M * (c2 - c.z * c.z), dt_f);
     }
     s.px += (xreal)(s.vx * dt);
@@ -493,8 +530,9 @@ PFB_HD void fixedwing_command(const FixedwingRegs& s, float* cmd) {
 // at the batch sizes these vehicles run at (16 384 envs) instruction-level parallelism is the only latency hiding there is:
 // FULL removes the tests at compile time, the surfaces land in ONE basic block and their chains interleave.
 // CONTACT = the ground pushes back (Aviary handles with contact_response): see rigid_step.
-template <bool FULL = false, bool CONTACT = false>
-PFB_HD void fixedwing_substep(const FixedwingParams& p, FixedwingRegs& s, const float* cmd, float xi) {
+// World: NoStatic or StaticCtx, as in quadx_substep.
+template <bool FULL = false, bool CONTACT = false, class World = NoStatic>
+PFB_HD void fixedwing_substep(const FixedwingParams& p, FixedwingRegs& s, const float* cmd, float xi, World* world = nullptr) {
   Vec3 F = Vec3{0.f, 0.f, 0.f}, T = Vec3{0.f, 0.f, 0.f};
   const Vec3 w = Vec3{s.wx, s.wy, s.wz};
   // fully unrolled: the surface tables become immediate constant-bank operands instead of indexed loads
@@ -518,37 +556,52 @@ PFB_HD void fixedwing_substep(const FixedwingParams& p, FixedwingRegs& s, const 
     F = F + Fm;
     T = T + cross(Vec3{p.motor_r[0], p.motor_r[1], p.motor_r[2]}, Fm) + Vec3{p.torque_k * a, 0.0f, 0.0f};
   }
-  const bool c = ground_contact(p.contact, (float)s.pz, (float)s.R.m20, (float)s.R.m21, (float)s.R.m22);
-  s.flags = (s.flags & ~(uint32_t)FLAG_CONTACT_PREV) | (c ? (FLAG_CONTACT_PREV | FLAG_CONTACT_ARRAY) : 0u);
-  rigid_step<CONTACT>(p.rb, p.gravity, p.dt, p.vmax, s, F, T, &p.contact, c);
+  if constexpr (World::kOn) {
+    const float pz = (float)s.pz, r20 = (float)s.R.m20, r21 = (float)s.R.m21, r22 = (float)s.R.m22;
+    uint32_t b;
+    const float top = static_surface(*world->w, world->pose, world->n, world->i, (float)s.px, (float)s.py, pz, p.contact.zmax,
+                                     [&](float t) { return ground_contact(p.contact, pz, r20, r21, r22, t); }, b);
+    world->bits |= b;
+    const bool c = b != 0u;
+    s.flags = (s.flags & ~(uint32_t)FLAG_CONTACT_PREV) | (c ? (FLAG_CONTACT_PREV | FLAG_CONTACT_ARRAY) : 0u);
+    rigid_step<CONTACT, World>(p.rb, p.gravity, p.dt, p.vmax, s, F, T, &p.contact, c, top);
+  } else {
+    const bool c = ground_contact(p.contact, (float)s.pz, (float)s.R.m20, (float)s.R.m21, (float)s.R.m22);
+    s.flags = (s.flags & ~(uint32_t)FLAG_CONTACT_PREV) | (c ? (FLAG_CONTACT_PREV | FLAG_CONTACT_ARRAY) : 0u);
+    rigid_step<CONTACT>(p.rb, p.gravity, p.dt, p.vmax, s, F, T, &p.contact, c);
+  }
   body_update_state(s);
 }
 
-template <int MODE, bool FULL = false, bool CONTACT = false, typename NoiseFn>
-PFB_HD void fixedwing_aviary_step(const FixedwingParams& p, FixedwingRegs& s, NoiseFn& noise) {
+template <int MODE, bool FULL = false, bool CONTACT = false, typename NoiseFn, class World = NoStatic>
+PFB_HD void fixedwing_aviary_step(const FixedwingParams& p, FixedwingRegs& s, NoiseFn& noise, World* world = nullptr) {
   s.flags &= ~(uint32_t)FLAG_CONTACT_ARRAY;
+  if constexpr (World::kOn) world->bits = 0u;
   noise.begin_step();
   float cmd[6];
   fixedwing_command<MODE>(s, cmd);
 #pragma unroll 1
-  for (int u = 0; u < p.ratio; ++u) fixedwing_substep<FULL, CONTACT>(p, s, cmd, noise.get(u));
+  for (int u = 0; u < p.ratio; ++u) fixedwing_substep<FULL, CONTACT>(p, s, cmd, noise.get(u), world);
 }
 // fixedwing_aviary_step with the flight mode a run-time value (one mode per drone): only the command mapping branches on it
-template <bool FULL, bool CONTACT, typename NoiseFn>
-PFB_HD void fixedwing_aviary_step_any(const FixedwingParams& p, FixedwingRegs& s, int mode, NoiseFn& noise) {
+template <bool FULL, bool CONTACT, typename NoiseFn, class World = NoStatic>
+PFB_HD void fixedwing_aviary_step_any(const FixedwingParams& p, FixedwingRegs& s, int mode, NoiseFn& noise, World* world = nullptr) {
   s.flags &= ~(uint32_t)FLAG_CONTACT_ARRAY;
+  if constexpr (World::kOn) world->bits = 0u;
   noise.begin_step();
   float cmd[6];
   if (mode == -1) fixedwing_command<-1>(s, cmd);
   else fixedwing_command<0>(s, cmd);
 #pragma unroll 1
-  for (int u = 0; u < p.ratio; ++u) fixedwing_substep<FULL, CONTACT>(p, s, cmd, noise.get(u));
+  for (int u = 0; u < p.ratio; ++u) fixedwing_substep<FULL, CONTACT>(p, s, cmd, noise.get(u), world);
 }
 // fixedwing_aviary_step_any inside an Aviary step of U substeps at several control rates: the command mapping runs before
 // substep u when u % r == 0 (r = physics_hz / control_hz of this drone, a divisor of U); draw u of the step.  r == U: the above.
-template <bool FULL, bool CONTACT, typename NoiseFn>
-PFB_HD void fixedwing_aviary_step_rates(const FixedwingParams& p, FixedwingRegs& s, int mode, int r, int U, NoiseFn& noise) {
+template <bool FULL, bool CONTACT, typename NoiseFn, class World = NoStatic>
+PFB_HD void fixedwing_aviary_step_rates(const FixedwingParams& p, FixedwingRegs& s, int mode, int r, int U, NoiseFn& noise,
+                                        World* world = nullptr) {
   s.flags &= ~(uint32_t)FLAG_CONTACT_ARRAY;
+  if constexpr (World::kOn) world->bits = 0u;
   noise.begin_step();
   float cmd[6];
 #pragma unroll 1
@@ -557,7 +610,7 @@ PFB_HD void fixedwing_aviary_step_rates(const FixedwingParams& p, FixedwingRegs&
       if (mode == -1) fixedwing_command<-1>(s, cmd);
       else fixedwing_command<0>(s, cmd);
     }
-    fixedwing_substep<FULL, CONTACT>(p, s, cmd, noise.get(u));
+    fixedwing_substep<FULL, CONTACT>(p, s, cmd, noise.get(u), world);
   }
 }
 // launch-uniform test for the FULL instantiation

@@ -203,6 +203,7 @@ int pfb_destroy(PfbHandle h) {
   if (!h) return 0;
   cudaSetDevice(h->device);
   mx_destroy(h);
+  static_destroy(h);
   if (h->d_spare) {
     if (h->side) {
       cudaStreamSynchronize(h->side);
@@ -272,6 +273,7 @@ int pfb_bind(PfbHandle h, const PfbBuffers* b) {
 int pfb_reset(PfbHandle h, const uint8_t* mask, void* stream) {
   if (h) h->fused_ready = 0;
   REQUIRE_BOUND(h);
+  if (!mask) static_clear(h);  // Aviary.reset calls resetSimulation: the static bodies go with it
   return h->ops->reset(h, mask, (cudaStream_t)stream);
 }
 

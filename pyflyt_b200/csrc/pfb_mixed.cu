@@ -177,6 +177,96 @@ __global__ void __launch_bounds__(kBlock, kMinBlocks) k_mixed_aviary_step(const 
   }
 }
 
+// The body of k_mixed_aviary_step with the static bodies of drone u's world, whose bits go to bits[u].  A
+// copy rather than a shared body, so that k_mixed_aviary_step stays the code it was.
+template <bool INJECT, bool CONTACT, bool RATES, class PS>
+__device__ __forceinline__ void mixed_aviary_step_static(const MixedStep<PS>& a, const StaticWorld* world, const float* pose, uint32_t* bits) {
+  const MixedRows& r = a.r;
+  const int b = blockIdx.x;
+  if (b < r.cta_qx) {
+    const int64_t j = (int64_t)b * kBlock + threadIdx.x;
+    if (j >= r.n_qx) return;
+    const int64_t u = r.slot_user[j];
+    StaticCtx w{world, pose, a.n, u, 0u};
+    const QuadXParams& p = qx_model(a.qx, j);
+    const int mode = a.slot_mode[j];
+    QuadXRegs s;
+    int step_count;
+    quadx_load_tile<7, kTileGroupStride>(r.qx_st + qx_tile_base(j, QX_ROWS), s, step_count);
+    quadx_mask_pid(s, mode);
+#pragma unroll
+    for (int c = 0; c < 4; ++c) s.sp[c] = __ldg(a.setpoint + kMixedSetpointDim * u + c);
+    if constexpr (RATES) {
+      const int ratio = a.slot_ratio[j];
+      auto nz = make_noise<INJECT>(a.noise, a.n, u, a.rng, a.seq, TAG_AVIARY, qx_model0(a.qx).noise_loc, a.U);
+      for (int k = 0; k < a.n_steps; ++k) quadx_aviary_step_rates<CONTACT>(p, s, mode, ratio, a.U, nz, &w);
+    } else {
+      auto nz = make_noise<INJECT>(a.noise, a.n, u, a.rng, a.seq, TAG_AVIARY, qx_model0(a.qx).noise_loc, qx_model0(a.qx).ratio);
+      for (int k = 0; k < a.n_steps; ++k) quadx_aviary_step_any<CONTACT>(p, s, mode, nz, &w);
+    }
+    quadx_store_tile<7, kTileGroupStride>(r.qx_st + qx_tile_base(j, QX_ROWS), s, step_count);
+    bits[u] = w.bits;
+  } else if (b < r.cta_qx + r.cta_fw) {
+    const int64_t j = (int64_t)(b - r.cta_qx) * kBlock + threadIdx.x;
+    if (j >= r.n_fw) return;
+    const int64_t u = r.slot_user[r.n_qx + j];
+    StaticCtx w{world, pose, a.n, u, 0u};
+    const int mode = a.slot_mode[r.n_qx + j];
+    const FixedwingParams& p = a.fw;
+    FixedwingRegs s;
+    fixedwing_load(r.fw_st, r.fw_ist, r.n_fw, j, s);
+#pragma unroll
+    for (int c = 0; c < 6; ++c) s.sp[c] = __ldg(a.setpoint + kMixedSetpointDim * u + c);
+    if constexpr (RATES) {
+      const int ratio = a.slot_ratio[r.n_qx + j];
+      auto nz = make_noise<INJECT>(a.noise, a.n, u, a.rng, a.seq, TAG_AVIARY, p.noise_loc, a.U);
+      if (fixedwing_full_model(p)) {
+        for (int k = 0; k < a.n_steps; ++k) fixedwing_aviary_step_rates<true, CONTACT>(p, s, mode, ratio, a.U, nz, &w);
+      } else {
+        for (int k = 0; k < a.n_steps; ++k) fixedwing_aviary_step_rates<false, CONTACT>(p, s, mode, ratio, a.U, nz, &w);
+      }
+    } else {
+      auto nz = make_noise<INJECT>(a.noise, a.n, u, a.rng, a.seq, TAG_AVIARY, p.noise_loc, p.ratio);
+      if (fixedwing_full_model(p)) {
+        for (int k = 0; k < a.n_steps; ++k) fixedwing_aviary_step_any<true, CONTACT>(p, s, mode, nz, &w);
+      } else {
+        for (int k = 0; k < a.n_steps; ++k) fixedwing_aviary_step_any<false, CONTACT>(p, s, mode, nz, &w);
+      }
+    }
+    fixedwing_store(r.fw_st, r.fw_ist, r.n_fw, j, s);
+    bits[u] = w.bits;
+  } else {
+    const int64_t j = (int64_t)(b - r.cta_qx - r.cta_fw) * kBlock + threadIdx.x;
+    if (j >= r.n_rk) return;
+    const int64_t u = r.slot_user[r.n_qx + r.n_fw + j];
+    StaticCtx w{world, pose, a.n, u, 0u};
+    const RocketParams& p = a.rk;
+    RocketRegs s;
+    rocket_load(r.rk_st, r.rk_ist, r.n_rk, j, s);
+#pragma unroll
+    for (int c = 0; c < 7; ++c) s.sp[c] = __ldg(a.setpoint + kMixedSetpointDim * u + c);
+    if constexpr (RATES) {
+      const int ratio = a.slot_ratio[r.n_qx + r.n_fw + j];
+      auto nz = make_noise<INJECT>(a.noise, a.n, u, a.rng, a.seq, TAG_AVIARY, p.noise_loc, a.U);
+      for (int k = 0; k < a.n_steps; ++k) rocket_aviary_step_rates(p, s, ratio, a.U, nz, &w);
+    } else {
+      auto nz = make_noise<INJECT>(a.noise, a.n, u, a.rng, a.seq, TAG_AVIARY, p.noise_loc, p.ratio);
+      for (int k = 0; k < a.n_steps; ++k) rocket_aviary_step(p, s, nz, false, &w);
+    }
+    rocket_store(r.rk_st, r.rk_ist, r.n_rk, j, s);
+    bits[u] = w.bits;
+  }
+}
+
+// k_mixed_aviary_step against the static bodies of each drone's world (pfb_add_static_body); bits[u]: what drone u touched during
+// its last Aviary step
+template <bool INJECT, bool CONTACT, bool RATES, class PS>
+__global__ void __launch_bounds__(kBlock, kMinBlocks)
+    k_mixed_aviary_step_static(const __grid_constant__ MixedStep<PS> a, const __grid_constant__ StaticWorld world, const float* __restrict__ pose,
+                               uint32_t* __restrict__ bits) {
+  mixed_aviary_step_static<INJECT, CONTACT, RATES, PS>(a, &world, pose, bits);
+}
+
 struct MixedObserve {
   MixedRows r;
   float* drone_state;  // [n][12]
@@ -390,7 +480,10 @@ static void launch_step(const PfbContext* h, const PS& ps, const float* noise, i
   a.seq = seq;
   a.slot_ratio = m->d_slot_ratio;
   a.U = m->U;
-  k_mixed_aviary_step<INJECT, CONTACT, RATES, PS><<<grid_all(m), kBlock, 0, s>>>(a);
+  if (const StaticBodies* sb = step_statics(h))
+    k_mixed_aviary_step_static<INJECT, CONTACT, RATES, PS><<<grid_all(m), kBlock, 0, s>>>(a, sb->world, sb->d_pose, sb->d_bits);
+  else
+    k_mixed_aviary_step<INJECT, CONTACT, RATES, PS><<<grid_all(m), kBlock, 0, s>>>(a);
 }
 
 // RATES: several control rates (d_slot_ratio set), chosen by the handle and uniform over the launch

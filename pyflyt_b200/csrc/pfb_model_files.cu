@@ -216,7 +216,9 @@ bool inertial_of(const XmlNode& link, Inertial& o) {
   return ok;
 }
 
-int load_urdf_links(const char* path, std::vector<Link>& links) {
+// link_frame: the primitives and inertial frames in the base LINK frame (static bodies, which loadURDF places by that frame),
+// and every geometry must be a box, a cylinder or a sphere; else in the base inertial frame, meshes and planes skipped
+int load_urdf_links(const char* path, std::vector<Link>& links, bool link_frame = false) {
   std::string text;
   if (!read_file(path, text)) return fail("cannot read URDF %s", path);
   size_t cut = text.find("</robot>");
@@ -279,6 +281,11 @@ int load_urdf_links(const char* path, std::vector<Link>& links) {
 
   Inertial bi;
   if (!inertial_of(*link_nodes[base], bi)) return fail("%s: malformed inertial origin in link '%s'", path, base.c_str());
+  if (link_frame) {  // a static body: its base inertial frame may be offset (pfb_set_static_pose places it), not rotated
+    if (bi.rpy.x != 0.0 || bi.rpy.y != 0.0 || bi.rpy.z != 0.0)
+      return fail("%s: the inertial frame of base link '%s' is rotated; a static body's may only be offset", path, base.c_str());
+    bi.xyz = V3{0, 0, 0};
+  }
   const M3 base_rot_t = transpose(rpy_to_matrix(bi.rpy));
   auto rebase_t = [&](V3 t) { return mul(base_rot_t, t - bi.xyz); };
   auto rebase_r = [&](const M3& r) { return mul(base_rot_t, r); };
@@ -321,6 +328,9 @@ int load_urdf_links(const char* path, std::vector<Link>& links) {
       } else if (const XmlNode* s = geo->child("sphere")) {
         sh.kind = PFB_SHAPE_SPHERE;
         sh.dims[0] = s->get("radius") ? atof(s->get("radius")) : 0.0;
+      } else if (link_frame) {
+        return fail("%s: link '%s' has a collision geometry other than a box, a cylinder or a sphere; static bodies are boxes and cylinders", path,
+                    names[idx].c_str());
       } else {
         continue;  // meshes / planes carry no analytic ground test
       }
@@ -521,6 +531,30 @@ int fill_surface(PfbSurface& s, const Link& link, V3 lift, V3 fwd, const Yaml& y
 }
 
 }  // namespace
+
+extern "C" int pfb_static_shapes_from_urdf(const char* urdf_path, double global_scaling, PfbShape* out, int cap, int* n_shapes,
+                                           double inertial_origin[3]) {
+  if (!urdf_path || !n_shapes || !inertial_origin || (cap > 0 && !out)) return fail("pfb_static_shapes_from_urdf: null argument");
+  if (!(global_scaling > 0.0)) return fail("pfb_static_shapes_from_urdf: globalScaling must be positive, got %g", global_scaling);
+  std::vector<Link> links;
+  if (load_urdf_links(urdf_path, links, true)) return -1;
+  int n = 0;
+  for (const Link& lk : links)
+    for (const Shape& s : lk.shapes) {
+      if (n >= cap) return fail("%s: more than %d collision primitives", urdf_path, cap);
+      PfbShape& sh = out[n++];
+      memset(&sh, 0, sizeof(sh));
+      sh.kind = s.kind;  // half extents / radius and half length, as pfb_model_from_files
+      if (s.kind == PFB_SHAPE_BOX) { for (int c = 0; c < 3; ++c) sh.dims[c] = 0.5 * s.dims[c] * global_scaling; }
+      else if (s.kind == PFB_SHAPE_CYLINDER) { sh.dims[0] = s.dims[0] * global_scaling; sh.dims[1] = 0.5 * s.dims[1] * global_scaling; }
+      else sh.dims[0] = s.dims[0] * global_scaling;
+      put3(sh.at, global_scaling * s.at);
+      memcpy(sh.rot, s.rot.m, sizeof(s.rot.m));
+    }
+  *n_shapes = n;
+  put3(inertial_origin, global_scaling * links[0].com);  // the base link's inertial origin, in its own frame
+  return 0;
+}
 
 extern "C" int pfb_model_from_files(int kind, const char* urdf_path, const char* yaml_path, double physics_hz, double control_hz, PfbModel* out) {
   if (!urdf_path || !yaml_path || !out) return fail("pfb_model_from_files: null argument");

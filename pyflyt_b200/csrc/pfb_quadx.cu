@@ -81,6 +81,37 @@ __global__ void __launch_bounds__(kBlock, kMinBlocks)
   qx_aviary_step_drone<INJECT, CONTACT, 4>(ps, rng, st, rows, i, modes, setpoint, noise, N, i, n_steps, seq);
 }
 
+// n_steps x Aviary.step() against the static bodies of each drone's world (pfb_add_static_body; Aviary handles, warp-tiled): one
+// flight mode MODE, or MODE = kStaticPerDrone = drone i in modes[i] as k_quadx_aviary_step_modes.  bits[i]: what drone i touched
+// during its last Aviary step.
+constexpr int kStaticPerDrone = 8;
+template <int MODE, bool INJECT, class PS, bool CONTACT>
+__global__ void __launch_bounds__(kBlock, kMinBlocks)
+    k_quadx_aviary_step_static(const __grid_constant__ PS ps, const __grid_constant__ RngParams rng, const __grid_constant__ StaticWorld world,
+                               const float* __restrict__ pose, uint32_t* __restrict__ bits, float* __restrict__ st, int rows,
+                               const float* __restrict__ setpoint, const int8_t* __restrict__ modes, const float* __restrict__ noise,
+                               int n_steps, uint32_t seq, int64_t N) {
+  int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= N) return;
+  constexpr int LM = MODE == kStaticPerDrone ? 7 : MODE;  // the rows moved: every PID row for per-drone modes
+  const QuadXParams& p = qx_model(ps, i);
+  StaticCtx w{&world, pose, N, i, 0u};
+  QuadXRegs s;
+  int step_count;
+  quadx_load_tile<LM, kTileGroupStride>(st + qx_tile_base(i, rows), s, step_count);
+  const int mode = MODE == kStaticPerDrone ? modes[i] : MODE;
+  if (MODE == kStaticPerDrone) quadx_mask_pid(s, mode);
+  float4 sp = __ldg(reinterpret_cast<const float4*>(setpoint) + i);
+  s.sp[0] = sp.x; s.sp[1] = sp.y; s.sp[2] = sp.z; s.sp[3] = sp.w;
+  auto nz = make_noise<INJECT>(noise, N, i, rng, seq, TAG_AVIARY, qx_model0(ps).noise_loc, qx_model0(ps).ratio);
+  for (int k = 0; k < n_steps; ++k) {
+    if constexpr (MODE == kStaticPerDrone) quadx_aviary_step_any<CONTACT>(p, s, mode, nz, &w);
+    else quadx_aviary_step<MODE, CONTACT>(p, s, nz, &w);
+  }
+  quadx_store_tile<LM, kTileGroupStride>(st + qx_tile_base(i, rows), s, step_count);
+  bits[i] = w.bits;
+}
+
 // Aviary.state(i) / aux_state(i) / contact_array  -> row-major API buffers
 template <bool TILED>
 __global__ void __launch_bounds__(kBlock) k_quadx_observe(const float* __restrict__ st, const int32_t* __restrict__ ist, int rows,
@@ -985,6 +1016,22 @@ int qx_aviary_step(PfbContext* h, int n_steps, const float* noise, cudaStream_t 
   const uint32_t seq = (uint32_t)h->aviary_seq++;
   const int g = grid_for(h->n);
   const bool contact = aviary_contact_response(h);
+  if (const StaticBodies* sb = step_statics(h)) {  // Aviary handles only, so always warp-tiled
+#define AVS_ARGS ps, h->rng, sb->world, sb->d_pose, sb->d_bits, h->buf.state, qx_rows(h), h->buf.setpoint, h->d_modes, noise, n_steps, seq, h->n
+#define AVS_LAUNCH(M, INJ, CT) QX_PARAMS_SWITCH(h, (k_quadx_aviary_step_static<M, INJ, PS, CT><<<g, kBlock, 0, s>>>(AVS_ARGS)))
+    if (mode == kModePerDrone) {
+      if (contact) { if (noise) { AVS_LAUNCH(kStaticPerDrone, true, true); } else { AVS_LAUNCH(kStaticPerDrone, false, true); } }
+      else { if (noise) { AVS_LAUNCH(kStaticPerDrone, true, false); } else { AVS_LAUNCH(kStaticPerDrone, false, false); } }
+    } else if (contact) {
+      if (noise) { PFB_MODE_SWITCH(mode, AVS_LAUNCH(MODE, true, true)); } else { PFB_MODE_SWITCH(mode, AVS_LAUNCH(MODE, false, true)); }
+    } else {
+      if (noise) { PFB_MODE_SWITCH(mode, AVS_LAUNCH(MODE, true, false)); } else { PFB_MODE_SWITCH(mode, AVS_LAUNCH(MODE, false, false)); }
+    }
+#undef AVS_LAUNCH
+#undef AVS_ARGS
+    LAUNCH_CHECK(h);
+    return 0;
+  }
   if (mode == kModePerDrone) {  // pfb_set_modes: Aviary handles only, so always warp-tiled
 #define AVM_ARGS ps, h->rng, h->buf.state, qx_rows(h), h->buf.setpoint, h->d_modes, noise, n_steps, seq, h->n
     if (contact) {

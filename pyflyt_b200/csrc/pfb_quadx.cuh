@@ -322,11 +322,11 @@ PFB_HD void quadx_update_control(const QuadXParams& p, QuadXRegs& s) {
   s.pwm[3] = clampf(m3, 0.05f, 1.0f);
 }
 
-// lowest point of the collision primitives against the plane z = 0, with the relative
+// lowest point of the collision primitives against the plane z = top (0: the floor), with the relative
 // contact-breaking threshold; evaluated on the pose at the START of the substep.
-PFB_HD bool quadx_ground_contact(const QuadXParams& p, const QuadXRegs& s) {
+PFB_HD bool quadx_ground_contact(const QuadXParams& p, const QuadXRegs& s, float top = 0.0f) {
   const float pz = (float)s.pz;
-  if (pz > p.contact_zmax) return false;  // higher than any primitive can reach: the common case
+  if (pz - top > p.contact_zmax) return false;  // higher than any primitive can reach: the common case
   const float r20 = (float)s.R.m20, r21 = (float)s.R.m21, r22 = (float)s.R.m22;
   bool hit = false;
 #pragma unroll 1
@@ -341,11 +341,43 @@ PFB_HD bool quadx_ground_contact(const QuadXParams& p, const QuadXRegs& s) {
       } else {
         extent = p.shape_dims[k][0];
       }
-      hit = hit || (cz - extent < p.shape_thr[k]);
+      hit = hit || (cz - extent - top < p.shape_thr[k]);
     }
   }
   return hit;
 }
+
+// ---- static bodies of an Aviary handle (pfb_add_static_body; DESIGN.md §4h) ---------------------------------------------
+// Fixed-base boxes and cylinders, upright once posed.  Every drone's world holds its own copy of each body: the primitive table
+// is launch-constant (a kernel parameter), the pose of body b in drone i's world is rows 5 b .. 5 b + 4 (x, y, z, cos yaw,
+// sin yaw of the base link frame) of a field-major [5 * kMaxStaticBodies][n] buffer that only pfb_set_static_pose writes.
+constexpr int kMaxStaticBodies = 8, kMaxStaticShapes = 16, kStaticPoseRows = 5;  // = PFB_MAX_STATIC_BODIES / _SHAPES
+struct StaticWorld {
+  int n_shapes;
+  int body[kMaxStaticShapes];         // the body primitive k belongs to
+  int kind[kMaxStaticShapes];         // PFB_SHAPE_BOX or PFB_SHAPE_CYLINDER
+  float at[kMaxStaticShapes][3];      // centre in the body's base link frame
+  float cyaw[kMaxStaticShapes], syaw[kMaxStaticShapes];  // yaw of the primitive in that frame
+  float half[kMaxStaticShapes][3];    // box: half extents; cylinder: radius, radius, half length
+};
+// The step bodies take a World: NoStatic (the floor only: the kernels every handle without static bodies launches) or
+// StaticCtx (the floor and the static bodies of drone i's world).  bits: what drone i touched during its current Aviary step,
+// bit 0 the floor, bit 1 + b static body b.
+struct NoStatic {
+  static constexpr bool kOn = false;
+  uint32_t bits;
+};
+struct StaticCtx {
+  static constexpr bool kOn = true;
+  const StaticWorld* w;
+  const float* pose;
+  int64_t n, i;
+  uint32_t bits;
+};
+// pfb_fixedwing.cuh: surface height under a drone and its contact bits
+template <class Touch>
+PFB_HD float static_surface(const StaticWorld& w, const float* pose, int64_t n, int64_t i, float px, float py, float pz, float reach,
+                            Touch&& touch, uint32_t& bits);
 
 // Bullet clamps the WORLD angular-velocity coordinates to +-vmax; that can only bite when a body rate
 // exceeds vmax/sqrt(3), so the rotation to the world frame and back lives out of line (cold).  Everything
@@ -378,7 +410,7 @@ Vel3 quadx_clamp_world_velocity(vreal vmax, Vel3 v) {
 }
 
 // contact RESPONSE over a list of collision primitives (pfb_fixedwing.cuh)
-template <class Shapes, class Regs>
+template <class Tag = NoStatic, class Shapes, class Regs>
 PFB_HD void apply_contact_impulses(const Shapes* cp, Regs& s, float pz0, float top, float M, Vec3 c, float Ixx, float Ixy, float Ixz,
                                    float Iyy, float Iyz, float Izz, float dt);
 
@@ -388,8 +420,10 @@ PFB_HD void apply_contact_impulses(const Shapes* cp, Regs& s, float pz0, float t
 // and the I-cache-resident hot loop is what the whole env step runs in.
 // CONTACT = the floor pushes back (Aviary handles with contact_response): on a substep whose contact flag is up, contact
 // impulses act on the predicted velocities before the pose is integrated (cold path; COM at the base origin, diagonal inertia).
-template <bool CONTACT = false>
-PFB_HD void quadx_substep(const QuadXParams& p, QuadXRegs& s, float xi) {
+// World: NoStatic, or StaticCtx (the static bodies of this drone's world: flags against each surface under the base, the
+// response against the highest of them).
+template <bool CONTACT = false, class World = NoStatic>
+PFB_HD void quadx_substep(const QuadXParams& p, QuadXRegs& s, float xi, World* world = nullptr) {
   // ---- motors (motors.py:130-155): lag, multiplicative noise, rpm^2 thrust + reaction torque
   float Fz = 0.0f, tx = 0.0f, ty = 0.0f, tz = 0.0f;
   const float gain = xi * p.noise_ratio;
@@ -423,7 +457,17 @@ PFB_HD void quadx_substep(const QuadXParams& p, QuadXRegs& s, float xi) {
   tz = fmaf(kpqr, signed_square(s.wz), tz);
   // ---- contact flag from the pose at the start of the step (collision detection precedes
   //      integration inside stepSimulation); aviary.py:523-525
-  const bool c = quadx_ground_contact(p, s);
+  bool c;
+  float top = 0.0f;  // surface height under the drone
+  if constexpr (World::kOn) {
+    uint32_t b;
+    top = static_surface(*world->w, world->pose, world->n, world->i, (float)s.px, (float)s.py, (float)s.pz, p.contact_zmax,
+                         [&](float t) { return quadx_ground_contact(p, s, t); }, b);
+    world->bits |= b;
+    c = b != 0u;
+  } else {
+    c = quadx_ground_contact(p, s);
+  }
   s.flags = (s.flags & ~(uint32_t)FLAG_CONTACT_PREV) | (c ? (FLAG_CONTACT_PREV | FLAG_CONTACT_ARRAY) : 0u);
 
   // ---- Newton-Euler about the COM (composite COM offset is zero for the quads; inertia diagonal)
@@ -460,7 +504,7 @@ PFB_HD void quadx_substep(const QuadXParams& p, QuadXRegs& s, float xi) {
     s.wx = w.x; s.wy = w.y; s.wz = w.z;
   }
   if (CONTACT) {
-    if (c) apply_contact_impulses(&p, s, (float)s.pz, 0.0f, 1.0f / p.inv_mass, Vec3{0.f, 0.f, 0.f}, p.Ixx, 0.0f, 0.0f, p.Iyy, 0.0f, p.Izz, p.dt);
+    if (c) apply_contact_impulses<World>(&p, s, (float)s.pz, top, 1.0f / p.inv_mass, Vec3{0.f, 0.f, 0.f}, p.Ixx, 0.0f, 0.0f, p.Iyy, 0.0f, p.Izz, p.dt);
     s.px += (xreal)(s.vx * dt);
     s.py += (xreal)(s.vy * dt);
     s.pz += (xreal)(s.vz * dt);
@@ -494,13 +538,14 @@ PFB_HD void quadx_substep(const QuadXParams& p, QuadXRegs& s, float xi) {
 // Aviary.step(): one control tick + `ratio` physics substeps (aviary.py:506-531 with one drone).
 // Noise protocol: begin_step() prepares the draws of this Aviary step (outside the substep loop),
 // get(u) hands out the draw of substep u.
-template <int MODE, bool CONTACT = false, typename NoiseFn>
-PFB_HD void quadx_aviary_step(const QuadXParams& p, QuadXRegs& s, NoiseFn& noise) {
+template <int MODE, bool CONTACT = false, typename NoiseFn, class World = NoStatic>
+PFB_HD void quadx_aviary_step(const QuadXParams& p, QuadXRegs& s, NoiseFn& noise, World* world = nullptr) {
   s.flags &= ~(uint32_t)FLAG_CONTACT_ARRAY;  // contact_array &= False
+  if constexpr (World::kOn) world->bits = 0u;
   noise.begin_step();
   quadx_update_control<MODE>(p, s);
 #pragma unroll 1
-  for (int u = 0; u < p.ratio; ++u) quadx_substep<CONTACT>(p, s, noise.get(u));
+  for (int u = 0; u < p.ratio; ++u) quadx_substep<CONTACT>(p, s, noise.get(u), world);
 }
 
 // quadx.py:233-373: setpoint preset + PID reset on a mode change
@@ -543,26 +588,28 @@ PFB_HD void quadx_update_control_any(const QuadXParams& p, QuadXRegs& s, int mod
   PFB_QX_MODE_CASES(mode, quadx_update_control<M>(p, s));
 }
 
-template <bool CONTACT = false, typename NoiseFn>
-PFB_HD void quadx_aviary_step_any(const QuadXParams& p, QuadXRegs& s, int mode, NoiseFn& noise) {
+template <bool CONTACT = false, typename NoiseFn, class World = NoStatic>
+PFB_HD void quadx_aviary_step_any(const QuadXParams& p, QuadXRegs& s, int mode, NoiseFn& noise, World* world = nullptr) {
   s.flags &= ~(uint32_t)FLAG_CONTACT_ARRAY;
+  if constexpr (World::kOn) world->bits = 0u;
   noise.begin_step();
   quadx_update_control_any(p, s, mode);
 #pragma unroll 1
-  for (int u = 0; u < p.ratio; ++u) quadx_substep<CONTACT>(p, s, noise.get(u));
+  for (int u = 0; u < p.ratio; ++u) quadx_substep<CONTACT>(p, s, noise.get(u), world);
 }
 
 // quadx_aviary_step_any inside an Aviary step of U substeps whose drones run at several control rates (aviary.py:506-529):
 // this drone, physics_hz / control_hz = r (a divisor of U, the table's own ratio), runs its control tick before substep u when
 // u % r == 0 and takes draw u of the step.  With r == U it is quadx_aviary_step_any.
-template <bool CONTACT = false, typename NoiseFn>
-PFB_HD void quadx_aviary_step_rates(const QuadXParams& p, QuadXRegs& s, int mode, int r, int U, NoiseFn& noise) {
+template <bool CONTACT = false, typename NoiseFn, class World = NoStatic>
+PFB_HD void quadx_aviary_step_rates(const QuadXParams& p, QuadXRegs& s, int mode, int r, int U, NoiseFn& noise, World* world = nullptr) {
   s.flags &= ~(uint32_t)FLAG_CONTACT_ARRAY;
+  if constexpr (World::kOn) world->bits = 0u;
   noise.begin_step();
 #pragma unroll 1
   for (int u = 0; u < U; ++u) {
     if (u % r == 0) quadx_update_control_any(p, s, mode);
-    quadx_substep<CONTACT>(p, s, noise.get(u));
+    quadx_substep<CONTACT>(p, s, noise.get(u), world);
   }
 }
 

@@ -52,6 +52,25 @@ __global__ void __launch_bounds__(kBlock, kMinBlocks)
   rk_aviary_step_drone<INJECT>(p, rng, st, ist, N, i, setpoint, noise, N, i, n_steps, seq);
 }
 
+// k_rk_aviary_step against the static bodies of each drone's world (pfb_add_static_body); bits[i]: what drone i touched during
+// its last Aviary step
+template <bool INJECT>
+__global__ void __launch_bounds__(kBlock, kMinBlocks)
+    k_rk_aviary_step_static(const __grid_constant__ RocketParams p, const __grid_constant__ RngParams rng, const __grid_constant__ StaticWorld world,
+                            const float* __restrict__ pose, uint32_t* __restrict__ bits, float* __restrict__ st, int32_t* __restrict__ ist,
+                            const float* __restrict__ setpoint, const float* __restrict__ noise, int n_steps, uint32_t seq, int64_t N) {
+  int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= N) return;
+  StaticCtx w{&world, pose, N, i, 0u};
+  RocketRegs s;
+  rocket_load(st, ist, N, i, s);
+  load_setpoint<7, 7>(setpoint, i, s.sp);
+  auto nz = make_noise<INJECT>(noise, N, i, rng, seq, TAG_AVIARY, p.noise_loc, p.ratio);
+  for (int k = 0; k < n_steps; ++k) rocket_aviary_step(p, s, nz, false, &w);
+  rocket_store(st, ist, N, i, s);
+  bits[i] = w.bits;
+}
+
 __global__ void __launch_bounds__(kBlock) k_rk_observe(const float* __restrict__ st, const int32_t* __restrict__ ist,
                                                        float* __restrict__ drone_state, float* __restrict__ aux,
                                                        uint8_t* __restrict__ contact, int64_t N) {
@@ -346,6 +365,14 @@ static int rk_set_mode(PfbContext* h, int mode, cudaStream_t) {  // the rocket's
 static int rk_aviary_step(PfbContext* h, int n_steps, const float* noise, cudaStream_t s) {
   const uint32_t seq = (uint32_t)h->aviary_seq++;
   const int g = grid_for(h->n);
+  if (const StaticBodies* sb = step_statics(h)) {
+#define RKS_ARGS h->rk, h->rng, sb->world, sb->d_pose, sb->d_bits, h->buf.state, h->buf.istate, h->buf.setpoint, noise, n_steps, seq, h->n
+    if (noise) k_rk_aviary_step_static<true><<<g, kBlock, 0, s>>>(RKS_ARGS);
+    else k_rk_aviary_step_static<false><<<g, kBlock, 0, s>>>(RKS_ARGS);
+#undef RKS_ARGS
+    LAUNCH_CHECK(h);
+    return 0;
+  }
   if (noise) k_rk_aviary_step<true><<<g, kBlock, 0, s>>>(h->rk, h->rng, h->buf.state, h->buf.istate, h->buf.setpoint, noise, n_steps, seq, h->n);
   else k_rk_aviary_step<false><<<g, kBlock, 0, s>>>(h->rk, h->rng, h->buf.state, h->buf.istate, h->buf.setpoint, nullptr, n_steps, seq, h->n);
   LAUNCH_CHECK(h);

@@ -90,7 +90,9 @@ PFB_HD void rocket_command(const RocketRegs& s, float* cmd) {
 }
 
 // one physics substep: update_physics (rocket.py:280-298) + stepSimulation + update_state
-PFB_HD void rocket_substep(const RocketParams& p, RocketRegs& s, const float* cmd, float xi, bool with_pad) {
+// World: NoStatic or StaticCtx (Aviary handles, with_pad = false), as in quadx_substep.
+template <class World = NoStatic>
+PFB_HD void rocket_substep(const RocketParams& p, RocketRegs& s, const float* cmd, float xi, bool with_pad, World* world = nullptr) {
   Vec3 F = Vec3{0.f, 0.f, 0.f}, T = Vec3{0.f, 0.f, 0.f};
   const Vec3 w = Vec3{s.wx, s.wy, s.wz};
   const bool windy = p.wind.kind != 0;  // uniform: the parameter block is launch-constant
@@ -136,8 +138,18 @@ PFB_HD void rocket_substep(const RocketParams& p, RocketRegs& s, const float* cm
   }
   // contacts from the pose at the start of the step: ground plane everywhere, landing pad under the base
   bool touching = false, over_pad = false;
+  float top = 0.0f;  // static bodies: the surface height under the drone
   const float pz0 = (float)s.pz;  // altitude at the START of the substep (the contact solver's pose)
-  {
+  if constexpr (World::kOn) {
+    const float pz = (float)s.pz, r20 = (float)s.R.m20, r21 = (float)s.R.m21, r22 = (float)s.R.m22;
+    uint32_t b;
+    top = static_surface(*world->w, world->pose, world->n, world->i, (float)s.px, (float)s.py, pz, p.contact.zmax,
+                         [&](float t) { return ground_contact(p.contact, pz, r20, r21, r22, t); }, b);
+    world->bits |= b;
+    touching = b != 0u;
+    s.flags = (s.flags & ~(uint32_t)FLAG_CONTACT_PREV) | (touching ? (FLAG_CONTACT_PREV | FLAG_CONTACT_ARRAY) : 0u) |
+              ((b & 1u) ? FLAG_CONTACT_GROUND : 0u);
+  } else {
     const float pz = (float)s.pz, r20 = (float)s.R.m20, r21 = (float)s.R.m21, r22 = (float)s.R.m22;
     bool g = ground_contact(p.contact, pz, r20, r21, r22, 0.0f);
     bool pad = false;
@@ -194,7 +206,7 @@ PFB_HD void rocket_substep(const RocketParams& p, RocketRegs& s, const float* cm
     s.wx = wc.x; s.wy = wc.y; s.wz = wc.z;
   }
   if (p.contact_response && touching)  // contact impulses on the predicted velocities, before the pose is integrated (cold path)
-    apply_contact_impulses(&p.contact, s, pz0, over_pad ? kPadTop : 0.0f, M, c, Ixx - M * (c2 - c.x * c.x), Ixy + M * c.x * c.y, Ixz + M * c.x * c.z,
+    apply_contact_impulses<World>(&p.contact, s, pz0, World::kOn ? top : (over_pad ? kPadTop : 0.0f), M, c, Ixx - M * (c2 - c.x * c.x), Ixy + M * c.x * c.y, Ixz + M * c.x * c.z,
                            Iyy - M * (c2 - c.y * c.y), Iyz + M * c.y * c.z, Izz - M * (c2 - c.z * c.z), p.dt);
   s.px += (xreal)(s.vx * dt); s.py += (xreal)(s.vy * dt); s.pz += (xreal)(s.vz * dt);
   float h2 = (s.wx * s.wx + s.wy * s.wy + s.wz * s.wz) * (0.25f * p.dt * p.dt);
@@ -217,26 +229,28 @@ PFB_HD void rocket_substep(const RocketParams& p, RocketRegs& s, const float* cm
   body_update_state(s);
 }
 
-template <typename NoiseFn>
-PFB_HD void rocket_aviary_step(const RocketParams& p, RocketRegs& s, NoiseFn& noise, bool with_pad) {
+template <typename NoiseFn, class World = NoStatic>
+PFB_HD void rocket_aviary_step(const RocketParams& p, RocketRegs& s, NoiseFn& noise, bool with_pad, World* world = nullptr) {
   s.flags &= ~(uint32_t)(FLAG_CONTACT_ARRAY | FLAG_CONTACT_PAD | FLAG_CONTACT_GROUND);
+  if constexpr (World::kOn) world->bits = 0u;
   noise.begin_step();
   float cmd[8];
   rocket_command(s, cmd);
 #pragma unroll 1
-  for (int u = 0; u < p.ratio; ++u) rocket_substep(p, s, cmd, noise.get(u), with_pad);
+  for (int u = 0; u < p.ratio; ++u) rocket_substep(p, s, cmd, noise.get(u), with_pad, world);
 }
 // rocket_aviary_step (no pad) inside an Aviary step of U substeps at several control rates: rocket_command runs before
 // substep u when u % r == 0 (r = physics_hz / control_hz of this drone, a divisor of U); draw u of the step.  r == U: the above.
-template <typename NoiseFn>
-PFB_HD void rocket_aviary_step_rates(const RocketParams& p, RocketRegs& s, int r, int U, NoiseFn& noise) {
+template <typename NoiseFn, class World = NoStatic>
+PFB_HD void rocket_aviary_step_rates(const RocketParams& p, RocketRegs& s, int r, int U, NoiseFn& noise, World* world = nullptr) {
   s.flags &= ~(uint32_t)(FLAG_CONTACT_ARRAY | FLAG_CONTACT_PAD | FLAG_CONTACT_GROUND);
+  if constexpr (World::kOn) world->bits = 0u;
   noise.begin_step();
   float cmd[8];
 #pragma unroll 1
   for (int u = 0; u < U; ++u) {
     if (u % r == 0) rocket_command(s, cmd);
-    rocket_substep(p, s, cmd, noise.get(u), false);
+    rocket_substep(p, s, cmd, noise.get(u), false, world);
   }
 }
 

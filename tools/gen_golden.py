@@ -1221,6 +1221,184 @@ def wind_fixtures():
               wind=AnalyticWind("constant", base=(2.0, 1.0, 0.0)))
 
 
+# ---- static bodies (DESIGN.md §4h) ----------------------------------------------------------------------------------------
+STATIC_DIR = os.path.join(OUT, "static")
+
+
+def _static_prims(s):
+    """(top, footprint test) of every collision primitive of the fixed-base body s, world frame (fakebullet's pose of s is its base
+    inertial frame, the primitives' offsets are relative to it)"""
+    Rs = s.R()
+    out = []
+    for lk in s.links:
+        for kind, dims, cr, cR in lk.shapes:
+            if kind not in ("box", "cylinder"):
+                raise ValueError(f"static body {s.path}: a {kind} (boxes and cylinders only)")
+            centre = s.pos + Rs @ cr
+            Rw = Rs @ cR
+            if kind == "box":
+                top = centre[2] + 0.5 * dims[2]
+                inside = (lambda c, R, h: lambda x, y: abs(R[0, 0] * (x - c[0]) + R[1, 0] * (y - c[1])) <= h[0]
+                          and abs(R[0, 1] * (x - c[0]) + R[1, 1] * (y - c[1])) <= h[1])(centre, Rw, 0.5 * np.asarray(dims))
+            else:
+                top = centre[2] + 0.5 * dims[1]
+                inside = (lambda c, r: lambda x, y: (x - c[0]) ** 2 + (y - c[1]) ** 2 <= r * r)(centre, dims[0])
+            out.append((top, inside))
+    return out
+
+
+def _reach(b):
+    """the model's contact reach about its base origin: contact_zmax / ContactParams::zmax of the library (pfb_quadx_host.h)"""
+    r = 0.0
+    for lk in b.links:
+        for kind, dims, cr, cR in lk.shapes:
+            if kind == "box":
+                disc = float(np.linalg.norm(0.5 * np.asarray(dims)))
+            elif kind == "cylinder":
+                disc = float(np.hypot(dims[0], 0.5 * dims[1]))
+            elif kind == "sphere":
+                disc = float(dims[0])
+            else:
+                continue
+            r = max(r, (float(np.linalg.norm(cr)) + disc + 0.02 * disc) * 1.001)
+    return r
+
+
+def _tops_under(b, s):
+    """tops of the primitives of static body s under free body b: footprint holds the base's (x, y), and z + R_b >= top"""
+    x, y, z = b.pos
+    return [top for top, inside in _static_prims(s) if inside(x, y) and z + _reach(b) >= top]
+
+
+class static_rule:
+    """The fake client's contact detection and response surface with the static-body rule of DESIGN.md §4h (boxes yawed, the
+    height guard, one contact pair per static body), for the fixtures of this group only; oracle/fakebullet keeps its own
+    (the untilted cylinder pad of Rocket-Landing) for every other fixture."""
+
+    def __enter__(self):
+        import pybullet as fb
+
+        self.fb, self.saved = fb, (fb.World._detect_contacts, fb.World._surface_height)
+
+        def detect(world):
+            world.contacts = []
+            statics = [s for s in world.bodies.values() if s.fixed_base]
+            for b in world.bodies.values():
+                if b.fixed_base:
+                    continue
+                low = b.lowest_point_and_threshold()
+                if low is None:
+                    continue
+                z, thr = low
+                for s in statics:
+                    if s.is_plane:
+                        top = s.pos[2]
+                    else:
+                        tops = _tops_under(b, s)
+                        if not tops:
+                            continue
+                        top = max(tops)
+                    if z - top < thr:
+                        world.contacts.append((0, s.uid, b.uid, -1, -1))
+                        world.contacts.append((0, b.uid, s.uid, -1, -1))
+
+        def surface(world, b):
+            tops = [0.0]
+            for s in world.bodies.values():
+                if s.fixed_base and not s.is_plane:
+                    tops += _tops_under(b, s)
+            return max(tops)
+
+        fb.World._detect_contacts, fb.World._surface_height = detect, surface
+        fb.World.contact_response = True
+        return self
+
+    def __exit__(self, *exc):
+        self.fb.World._detect_contacts, self.fb.World._surface_height = self.saved
+        self.fb.World.contact_response = False
+
+
+def fly_static(name, drone_type, drone_options, start_pos, start_orn, mode, bodies, setpoint_schedule, n_steps, seed, poses=None):
+    """Each drone in a reference Aviary of its own (its own world), with the static bodies `bodies` = [(urdf file under
+    tests/golden/static, basePosition, baseOrientation)] loaded by aviary.loadURDF(useFixedBase=True) and
+    register_all_new_bodies(); poses[i] = {body: (pos, quat)} moves body k of drone i's world with resetBasePositionAndOrientation
+    (its base inertial frame) before the flight.  Records per drone and step the state, aux state and contact_array[drone.Id, body]
+    (bit 0 the floor, bit 1 + k body k) and the raw draws of each world, which the replays inject."""
+    n = len(start_pos)
+    states, auxs, bits, raws, noises = [], [], [], [], []
+    for i in range(n):
+        rng = ril.ScriptedNoise(seed + i)
+        env = Aviary(start_pos=np.array([start_pos[i]], dtype=np.float64), start_orn=np.array([start_orn[i]], dtype=np.float64),
+                     drone_type=drone_type, drone_options=dict(drone_options), np_random=rng)
+        ids = [env.loadURDF(os.path.join(STATIC_DIR, f), basePosition=p, baseOrientation=q, useFixedBase=True) for f, p, q in bodies]
+        env.register_all_new_bodies()
+        for k, (pos, quat) in (poses[i] if poses else {}).items():
+            env.resetBasePositionAndOrientation(ids[k], pos, quat)
+        env.set_mode(mode)
+        d = env.drones[0]
+        st, ax, bt, rw = [], [], [], []
+        for t in range(n_steps):
+            if t in setpoint_schedule:
+                env.set_setpoint(0, np.array(setpoint_schedule[t][i] if isinstance(setpoint_schedule[t], dict) else setpoint_schedule[t], dtype=np.float64))
+            env.step()
+            st.append(np.array(d.state))
+            ax.append(np.array(d.aux_state, dtype=np.float64))
+            row = env.contact_array[d.Id]
+            bt.append(int(row[env.planeId]) | sum(int(row[bid]) << (1 + k) for k, bid in enumerate(ids)))
+            pos, quat = env.getBasePositionAndOrientation(d.Id)
+            v, w = env.getBaseVelocity(d.Id)
+            rw.append(np.concatenate([pos, quat, v, w]))
+        states.append(st), auxs.append(ax), bits.append(bt), raws.append(rw), noises.append(np.array(rng.normal_log))
+    sched = {str(k): (v if not isinstance(v, dict) else {str(a): list(b) for a, b in v.items()}) for k, v in setpoint_schedule.items()}
+    np.savez_compressed(
+        os.path.join(OUT, f"{name}.npz"),
+        drone_type=drone_type, drone_options=json.dumps(drone_options), mode=mode,
+        start_pos=np.array(start_pos, dtype=np.float64), start_orn=np.array(start_orn, dtype=np.float64),
+        bodies=json.dumps([(f, list(p), list(q)) for f, p, q in bodies]),
+        poses=json.dumps([{str(k): (list(p), list(q)) for k, (p, q) in pz.items()} for pz in poses] if poses else []),
+        setpoints=json.dumps({k: np.asarray(v, dtype=np.float64).tolist() if not isinstance(v, dict) else v for k, v in sched.items()}),
+        noise=np.stack(noises, axis=-1),  # [draws][n]
+        state=np.array(states).transpose(1, 0, 2, 3), aux=np.array(auxs).transpose(1, 0, 2), bits=np.array(bits, dtype=np.uint32).T,
+        raw=np.array(raws).transpose(1, 0, 2),
+    )
+    print(name, "final pos", [s[-1][3] for s in states], "bits", [b[-1] for b in bits], "draws", noises[0].shape)
+
+
+def static_fixtures():
+    """The unmodified reference Aviary with fixed-base bodies (loadURDF + register_all_new_bodies), read through
+    contact_array[drone.Id, body], on the fake client with the static-body rule and the contact response (static_rule)."""
+    yaw30 = [0.0, 0.0, np.sin(np.pi / 12), np.cos(np.pi / 12)]
+    cf2x = dict(drone_model="cf2x")
+    with static_rule():
+        # cf2x in mode 7: take off from a 1 m platform, cross to a second one yawed 30 degrees, land on it and rest
+        fly_static("static_cf2x_platform_hop", "quadx", cf2x, [[0.0, 0.0, 1.02]], [[0.0, 0.0, 0.0]], 7,
+                   [("platform_box.urdf", [0.0, 0.0, 0.0], [0.0, 0.0, 0.0, 1.0]), ("platform_box.urdf", [3.0, 1.5, 0.0], yaw30)],
+                   {0: [0.0, 0.0, 0.0, 2.0], 240: [3.0, 1.5, 0.0, 2.0], 600: [3.0, 1.5, 0.0, 0.5]}, 960, seed=401)
+        # primitive_drone dropped tilted, half over a platform's edge (motors idle)
+        fly_static("static_primitive_edge_drop", "quadx", dict(drone_model="primitive_drone"), [[1.0, 0.3, 2.2]], [[0.4, 0.2, 0.0]], -1,
+                   [("platform_box.urdf", [0.0, 0.0, 0.0], [0.0, 0.0, 0.0, 1.0])], {0: [0.0, 0.0, 0.0, 0.0]}, 480, seed=402)
+        # cf2x flying beside a 4 m tower (30 degrees yawed box) and under its 1.5 m helipad, never touching either
+        fly_static("static_cf2x_beside_under", "quadx", cf2x, [[1.0, 0.0, 1.0]], [[0.0, 0.0, 0.0]], 7,
+                   [("helipad_tower.urdf", [0.0, 0.0, 0.0], [0.0, 0.0, 0.0, 1.0])],
+                   {0: [1.0, 0.0, 0.0, 3.0], 200: [0.0, 1.0, 0.0, 3.5], 400: [-0.8, -0.8, 0.0, 2.0]}, 600, seed=403)
+        # fixed-wing gliding onto a runway box, throttle off
+        fly_static("static_fixedwing_runway", "fixedwing", dict(drone_model="fixedwing"), [[0.0, 0.0, 1.5]], [[0.0, 0.0, 0.0]], 0,
+                   [("runway.urdf", [45.0, 0.0, 0.0], [0.0, 0.0, np.sin(np.pi / 180), np.cos(np.pi / 180)])],
+                   {0: [0.0, -0.1, 0.0, 0.0]}, 600, seed=404)
+        # rocket dropped onto a pad off the origin, booster off
+        fly_static("static_rocket_pad", "rocket", dict(drone_model="rocket"), [[6.3, -4.2, 5.0]], [[0.0, 0.0, 0.0]], 0,
+                   [("pad_cylinder.urdf", [6.0, -4.0, 0.0], [0.0, 0.0, 0.0, 1.0])], {0: [0, 0, 0, 0, 0, 0, 0]}, 480, seed=405)
+        # per-drone poses: three worlds, the platform moved by resetBasePositionAndOrientation (base inertial frame) in each,
+        # cf2x descending onto it near the rotated footprint's edge
+        poses = [{0: ([0.5, 0.0, 0.5], [0.0, 0.0, np.sin(0.3), np.cos(0.3)])},
+                 {0: ([-1.0, 2.0, 1.0], [0.0, 0.0, np.sin(-0.6), np.cos(-0.6)])},
+                 {0: ([2.0, -1.0, 0.2], [0.0, 0.0, np.sin(0.9), np.cos(0.9)])}]
+        starts = [[1.2, 0.6, 2.0], [-0.3, 2.6, 2.5], [2.9, -0.4, 1.6]]
+        fly_static("static_cf2x_per_drone_poses", "quadx", cf2x, starts, [[0.0, 0.0, 0.0]] * 3, 7,
+                   [("platform_box.urdf", [0.0, 0.0, 0.0], [0.0, 0.0, 0.0, 1.0])],
+                   {0: {i: [starts[i][0], starts[i][1], 0.0, 0.3] for i in range(3)}}, 600, seed=406, poses=poses)
+
+
 if __name__ == "__main__":
     os.makedirs(OUT, exist_ok=True)
     which = sys.argv[1] if len(sys.argv) > 1 else "all"
@@ -1252,3 +1430,5 @@ if __name__ == "__main__":
         rate_fixtures()
     if which in ("all", "basestate"):
         base_state_fixtures()
+    if which in ("all", "static"):
+        static_fixtures()
