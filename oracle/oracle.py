@@ -236,7 +236,7 @@ class Oracle:
         lib().orc_set_start(self._h, _dp(sp), _dp(so))
 
     def df_get_actions(self):
-        """MAFixedwingDogfight: [N][8] past_action | current_action of every agent"""
+        """MAFixedwingDogfight and MAQuadXHover: [N][8] past_action | current_action of every agent"""
         out = np.zeros((self.n, 8))
         lib().orc_df_get_actions(self._h, _dp(out))
         return out

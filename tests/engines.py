@@ -277,6 +277,11 @@ def load_golden(name):
     return np.load(os.path.join(GOLDEN, name if name.endswith(".npz") else name + ".npz"))
 
 
+def fixture_agent_hz(g):
+    """the agent rate a Hover / MAQuadXHover fixture was flown at (fixtures that do not record it: the default, 40 Hz)"""
+    return int(g["agent_hz"]) if "agent_hz" in g.files else 40
+
+
 def fixture_wind(g):
     """the AnalyticWind a fixture was flown in (None = still air)"""
     if "wind_kind" not in g.files:
@@ -321,7 +326,7 @@ def replay_aviary(make_engine, g, every=1):
 def replay_hover(make_engine, g):
     """Replays a quadx_hover fixture (env.reset + scripted env.step + user-loop resets)."""
     model = build_model("quadx", "cf2x")
-    env = hover_config(int(g["flight_mode"]), str(g["angle_representation"]), bool(g["sparse"]), float(g["dome"]))
+    env = hover_config(int(g["flight_mode"]), str(g["angle_representation"]), bool(g["sparse"]), float(g["dome"]), fixture_agent_hz(g))
     eng = make_engine(model, env, 1, np.array([[0.0, 0.0, 1.0]]), np.zeros((1, 3)))
     noise, splits = g["noise"], g["noise_splits"]
     cursor = {"i": 0}
@@ -695,7 +700,8 @@ def replay_ma_hover(make_engine, g):
     are stepped with a zero action (their outputs are not compared)."""
     A = int(g["n_agents"])
     model = build_model("quadx", "cf2x")
-    env = ma_hover_config(int(g["flight_mode"]), str(g["angle_representation"]), bool(g["sparse"]), float(g["dome"]), 40, float(g["max_duration_seconds"]))
+    env = ma_hover_config(int(g["flight_mode"]), str(g["angle_representation"]), bool(g["sparse"]), float(g["dome"]), fixture_agent_hz(g),
+                         float(g["max_duration_seconds"]))
     eng = make_engine(model, env, A, g["start_pos"], g["start_orn"])
     err = dict(obs=0.0, pos=0.0, reward=0.0, flag_mismatch=0, episodes=int(g["n_episodes"]))
     p0 = 10 if str(g["angle_representation"]) == "quaternion" else 9

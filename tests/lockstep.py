@@ -123,9 +123,9 @@ def hover_step(env, seed: int, steps: int, *, env_offset: int = 0, reset_seq: in
     dumped and compared with the replay, the oracle reset on the kernel's schedule."""
     import torch
 
-    av, n, mode = env.aviary, env.num_envs, env.flight_mode
+    av, n, mode, ratio = env.aviary, env.num_envs, env.flight_mode, env.config.env_step_ratio
     run = Run("hover step", n, obs_bar, obs_bar, 4096)
-    dump = torch.zeros((6, n), dtype=torch.float32, device=av.device)
+    dump = torch.zeros((2 * ratio, n), dtype=torch.float32, device=av.device)  # two draws per Aviary step
     av.set_noise_dump(dump)
     streams = Streams(seed, n, env_offset=env_offset, noise_loc=4.0)
     orc = hover_oracle(env, n)
@@ -143,7 +143,7 @@ def hover_step(env, seed: int, steps: int, *, env_offset: int = 0, reset_seq: in
         act = streams.actions(k, mode)
         assert np.array_equal(act_g, act), k
         og, rg, teg, trg, ig = _host(av)
-        nz = streams.step_noise(k)
+        nz = streams.step_noise(k, ratio)
         oo, ro, teo, tro, io = orc.o.env_step(act.astype(np.float64), nz.astype(np.float64))
         teo, tro = teo.astype(bool), tro.astype(bool)
         if done_prev.any():
@@ -152,7 +152,7 @@ def hover_step(env, seed: int, steps: int, *, env_offset: int = 0, reset_seq: in
             oo[done_prev], ro[done_prev], teo[done_prev], tro[done_prev], io[done_prev] = obs_r[done_prev], 0.0, False, False, 0
             episode[idx] += 1
             run.n_resets += len(idx)
-        full = ~done_prev & ~(teg | trg)  # the envs that ran all three Aviary steps
+        full = ~done_prev & ~(teg | trg)  # the envs that ran every Aviary step of the env step
         if full.any():
             run.worst_noise = max(run.worst_noise, float(np.abs(dump.cpu().numpy()[:, full] - nz[:, full]).max()))
         run.flips((teg != teo) | (trg != tro))

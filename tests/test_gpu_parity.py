@@ -43,7 +43,7 @@ def test_floor_contact():
     assert err["contact_mismatch"] == 0 and err["pos"] < 1e-5
 
 
-@pytest.mark.parametrize("name", ["hover_quat_dense", "hover_euler_sparse", "hover_quat_gentle", "hover_mode6"])
+@pytest.mark.parametrize("name", ["hover_quat_dense", "hover_euler_sparse", "hover_quat_gentle", "hover_mode6", "hover_hz24_mode1"])
 def test_hover_env_golden(name):
     err = replay_hover(make_cuda_engine, load_golden(name))
     assert err["flag_mismatch"] == 0

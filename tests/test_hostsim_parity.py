@@ -36,7 +36,7 @@ def test_floor_contact_flags_and_no_drag_in_contact():
     assert err["contact_mismatch"] == 0 and err["pos"] < 1e-5
 
 
-@pytest.mark.parametrize("name", ["hover_quat_dense", "hover_euler_sparse", "hover_quat_gentle", "hover_mode6"])
+@pytest.mark.parametrize("name", ["hover_quat_dense", "hover_euler_sparse", "hover_quat_gentle", "hover_mode6", "hover_hz24_mode1"])
 def test_hover_env(name):
     err = replay_hover(HostSimEngine, load_golden(name))
     assert err["flag_mismatch"] == 0

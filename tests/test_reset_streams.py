@@ -19,7 +19,7 @@ from philox_replay import Streams
 SEED = (1 << 40) + 0x5EED          # k1 = 256: the high key word is in play
 OTHER = 0x1234_5678_9ABC
 OFFSET = (1 << 32) - 500           # env ids 2^32 - 500 .. : the batch straddles the counter's high word
-KINDS = ["hover", "qxwp", "fwwp", "rocket", "dogfight"]
+KINDS = ["hover", "qxwp", "fwwp", "rocket", "dogfight", "mahover"]
 
 
 def make_env(kind, n, seed, env_offset=0, **kw):
@@ -296,11 +296,11 @@ def test_reset_seed_with_mask_is_refused():
 @pytest.mark.gpu
 @pytest.mark.parametrize("kind", KINDS)
 def test_ragged_shard_split_equals_one_handle(kind):
-    """one handle of n envs against two handles split at a point that is not a multiple of 32 (arena-aligned for the dogfight),
-    env offsets base and base + split with the batch straddling 2^32: bit for bit, autoresets included"""
+    """one handle of n envs against two handles split at a point that is not a multiple of 32 (arena-aligned for the dogfight
+    and MAQuadXHover), env offsets base and base + split with the batch straddling 2^32: bit for bit, autoresets included"""
     import torch
 
-    n, split = (1034, 502) if kind == "dogfight" else (1000, 397)
+    n, split = {"dogfight": (1034, 502), "mahover": (1000, 396)}.get(kind, (1000, 397))
     base = (1 << 32) - 450
     whole = make_env(kind, n, SEED, base)
     parts = [make_env(kind, split, SEED, base), make_env(kind, n - split, SEED, base + split)]

@@ -941,13 +941,13 @@ def fly_dogfight(name, seed, n_steps, action_seed, team_size=1, sparse=False, ac
 
 
 def fly_ma_hover(name, seed, n_steps, action_seed, flight_mode=0, angle_representation="quaternion", sparse=False, dome=10.0,
-                 max_duration_seconds=30.0, action_scale=0.3, start_pos=None):
+                 max_duration_seconds=30.0, action_scale=0.3, start_pos=None, agent_hz=40):
     """MAQuadXHoverEnv (pz_envs/quadx_envs/ma_quadx_hover_env.py) with scripted actions; a new episode is started whenever
     every agent is done.  The Aviary's own generator (seeded by reset(seed)) is wrapped so that its draws are recorded."""
     from PyFlyt.pz_envs.quadx_envs.ma_quadx_hover_env import MAQuadXHoverEnv
 
     kw = dict(sparse_reward=sparse, flight_mode=flight_mode, flight_dome_size=dome, max_duration_seconds=max_duration_seconds,
-              angle_representation=angle_representation)
+              angle_representation=angle_representation, agent_hz=agent_hz)
     if start_pos is not None:
         kw.update(start_pos=np.asarray(start_pos, dtype=np.float64), start_orn=np.zeros_like(np.asarray(start_pos, dtype=np.float64)))
     env = MAQuadXHoverEnv(**kw)
@@ -1003,16 +1003,17 @@ def fly_ma_hover(name, seed, n_steps, action_seed, flight_mode=0, angle_represen
         for key, v in e.items():
             flat[f"ep{k}_{key}"] = np.array(v)
     np.savez_compressed(os.path.join(OUT, f"{name}.npz"), kind="ma_quadx_hover", n_agents=A, sparse=sparse, n_episodes=len(episodes), flight_mode=flight_mode,
-                        angle_representation=angle_representation, dome=dome, max_duration_seconds=max_duration_seconds,
+                        angle_representation=angle_representation, dome=dome, max_duration_seconds=max_duration_seconds, agent_hz=agent_hz,
                         start_pos=np.asarray(env.start_pos, dtype=np.float64), start_orn=np.asarray(env.start_orn, dtype=np.float64), **flat)
     print(name, "episodes", len(episodes), "steps", [len(e["actions"]) for e in episodes], "reward range", min(np.nanmin(e["reward"]) for e in episodes), max(np.nanmax(e["reward"]) for e in episodes))
 
 
-def fly_hover(name, seed, n_steps, action_seed, angle_representation, flight_mode=0, sparse=False, dome=3.0, action_scale=1.0, wind=None):
+def fly_hover(name, seed, n_steps, action_seed, angle_representation, flight_mode=0, sparse=False, dome=3.0, action_scale=1.0, wind=None,
+              agent_hz=40):
     from PyFlyt.gym_envs.quadx_envs.quadx_hover_env import QuadXHoverEnv
 
     env = QuadXHoverEnv(
-        sparse_reward=sparse, flight_mode=flight_mode, flight_dome_size=dome, angle_representation=angle_representation
+        sparse_reward=sparse, flight_mode=flight_mode, flight_dome_size=dome, angle_representation=angle_representation, agent_hz=agent_hz
     )
     rng = ril.ScriptedNoise(seed)
     env._np_random = rng  # the env hands its generator to the Aviary (quadx_base_env.py:192)
@@ -1049,6 +1050,7 @@ def fly_hover(name, seed, n_steps, action_seed, angle_representation, flight_mod
         sparse=sparse,
         dome=dome,
         angle_representation=angle_representation,
+        agent_hz=agent_hz,
         reset_obs=obs0,
         actions=np.array(acts),
         obs=np.array(obs),
@@ -1140,6 +1142,16 @@ def ma_hover_fixtures():
     fly_ma_hover("mahover_euler_sparse", seed=203, n_steps=120, action_seed=32, angle_representation="euler", sparse=True, action_scale=0.5)
     fly_ma_hover("mahover_mode6_trunc", seed=205, n_steps=100, action_seed=33, flight_mode=6, max_duration_seconds=1.0, action_scale=0.1, dome=10.0)
     fly_ma_hover("mahover_two_agents_small_dome", seed=207, n_steps=140, action_seed=34, dome=2.0, start_pos=[[0.0, 0.0, 1.0], [0.5, 0.5, 1.5]])
+    agent_rate_fixtures()
+
+
+def agent_rate_fixtures():
+    # agent rates other than 40 Hz: env_step_ratio 1 (an env step ends halfway through a Philox pair) and 5 (past the four
+    # prefetched Aviary steps); a ragged 3-agent arena with euler observations, and mode 1, whose warm-up depends on its noise
+    fly_ma_hover("mahover_hz120_three_euler", seed=209, n_steps=300, action_seed=35, angle_representation="euler", dome=2.0,
+                 max_duration_seconds=1.5, start_pos=[[0.0, 0.0, 1.0], [1.0, 0.0, 1.5], [-0.5, 0.8, 0.8]], agent_hz=120)
+    fly_ma_hover("mahover_hz24_mode1", seed=211, n_steps=90, action_seed=36, flight_mode=1, max_duration_seconds=2.0, dome=3.0, agent_hz=24)
+    fly_hover("hover_hz24_mode1", seed=8, n_steps=120, action_seed=5, angle_representation="quaternion", flight_mode=1, action_scale=0.3, agent_hz=24)
 
 
 def dogfight_fixtures():
@@ -1412,6 +1424,8 @@ if __name__ == "__main__":
         dogfight_fixtures()
     if which in ("all", "mahover"):
         ma_hover_fixtures()
+    if which == "agentrates":  # (included in "mahover")
+        agent_rate_fixtures()
     if which in ("all", "qxwp"):
         quadx_waypoints_fixtures()
     if which in ("all", "wind"):
