@@ -1,7 +1,7 @@
-// pfb_aviary.cuh — the per-drone bodies of the Aviary operations, one per vehicle kind: the step in a per-drone flight mode,
-// the state query, the reset, the per-drone set_mode and the base state (set / get).  A body works on row j of its kind's state
-// region (QuadX warp-tiled, fixed-wing and rocket field-major [F][n] + istate [I][n]) and takes drone u's setpoint row (SP floats
-// apart), start pose, noise column or base-state rows.  The single-kind kernels call them with j = u = i; the mixed-kind kernels (pfb_mixed.cu) with u = slot_user[j].
+// pfb_aviary.cuh — the per-drone bodies of the Aviary operations, one per vehicle kind: the state query, the reset, the
+// per-drone set_mode and the base state (set / get), and the world of the Aviary step kernels.  A body works on row j of its
+// kind's state region (QuadX warp-tiled, fixed-wing and rocket field-major [F][n] + istate [I][n]) and takes drone u's setpoint
+// row (SP floats apart), start pose or base-state rows.  The single-kind kernels call them with j = u = i; the mixed-kind kernels (pfb_mixed.cu) with u = slot_user[j].
 // Pointers are passed as parameters, not in structs (a __restrict__ member loses its __restrict__), and a table is bound by
 // reference to the kernel's own __grid_constant__ parameter (a copy of it is staged on the stack).
 #pragma once
@@ -46,51 +46,19 @@ __device__ __forceinline__ void load_setpoint(const float* setpoint, int64_t u, 
   }
 }
 
-// ---- n_steps x Aviary.step() of the drone in row j, in flight mode modes[j] -------------------------------------------------
-// QuadX: every PID row is moved (the mode-7 set); quadx_mask_pid gives the drone the PID memory the uniform kernel of its mode
-// would load, so both store the same words.
-template <bool INJECT, bool CONTACT, int SP, class PS>
-__device__ __forceinline__ void qx_aviary_step_drone(const PS& ps, const RngParams& rng, float* st, int rows, int64_t j, const int8_t* modes,
-                                                     const float* setpoint, const float* noise, int64_t N, int64_t u, int n_steps, uint32_t seq) {
-  const QuadXParams& p = qx_model(ps, j);
-  const int mode = modes[j];
-  QuadXRegs s;
-  int step_count;
-  quadx_load_tile<7, kTileGroupStride>(st + qx_tile_base(j, rows), s, step_count);
-  quadx_mask_pid(s, mode);
-  load_setpoint<SP, 4>(setpoint, u, s.sp);
-  auto nz = make_noise<INJECT>(noise, N, u, rng, seq, TAG_AVIARY, qx_model0(ps).noise_loc, qx_model0(ps).ratio);
-  for (int k = 0; k < n_steps; ++k) quadx_aviary_step_any<CONTACT>(p, s, mode, nz);
-  quadx_store_tile<7, kTileGroupStride>(st + qx_tile_base(j, rows), s, step_count);
-}
-// fixed-wing: the launch-uniform fixedwing_full_model choice of the uniform kernels; only the command mapping branches on the mode
-template <bool INJECT, bool CONTACT, int SP>
-__device__ __forceinline__ void fw_aviary_step_drone(const FixedwingParams& p, const RngParams& rng, float* st, int32_t* ist, int64_t n, int64_t j,
-                                                     const int8_t* modes, const float* setpoint, const float* noise, int64_t N, int64_t u,
-                                                     int n_steps, uint32_t seq) {
-  const int mode = modes[j];
-  FixedwingRegs s;
-  fixedwing_load(st, ist, n, j, s);
-  load_setpoint<SP, 6>(setpoint, u, s.sp);
-  auto nz = make_noise<INJECT>(noise, N, u, rng, seq, TAG_AVIARY, p.noise_loc, p.ratio);
-  if (fixedwing_full_model(p)) {
-    for (int k = 0; k < n_steps; ++k) fixedwing_aviary_step_any<true, CONTACT>(p, s, mode, nz);
-  } else {
-    for (int k = 0; k < n_steps; ++k) fixedwing_aviary_step_any<false, CONTACT>(p, s, mode, nz);
-  }
-  fixedwing_store(st, ist, n, j, s);
-}
-// rocket: one flight mode; the contact response is p.contact_response
-template <bool INJECT>
-__device__ __forceinline__ void rk_aviary_step_drone(const RocketParams& p, const RngParams& rng, float* st, int32_t* ist, int64_t n, int64_t j,
-                                                     const float* setpoint, const float* noise, int64_t N, int64_t u, int n_steps, uint32_t seq) {
-  RocketRegs s;
-  rocket_load(st, ist, n, j, s);
-  load_setpoint<7, 7>(setpoint, u, s.sp);
-  auto nz = make_noise<INJECT>(noise, N, u, rng, seq, TAG_AVIARY, p.noise_loc, p.ratio);
-  for (int k = 0; k < n_steps; ++k) rocket_aviary_step(p, s, nz, false);
-  rocket_store(st, ist, n, j, s);
-}
+// ---- the world an Aviary step kernel flies its drones in (World = NoStatic or StaticCtx, pfb_quadx.cuh) ---------------------
+// The static-body table is the kernel's __grid_constant__ parameter of type WorldTable<World>::T: an empty struct on the
+// floor-only path, so that its parameter bank does not carry the StaticWorld.  The kernel binds drone i's world to it in place,
+// World w{&table, pose, n, i, 0u}; returned by a helper instead, it moves instructions in some kernels (DESIGN.md §4h).  A
+// NoStatic world is never dereferenced (every use in the substeps is behind `if constexpr (World::kOn)`).
+template <class World>
+struct WorldTable {
+  using T = NoStaticTable;
+};
+template <>
+struct WorldTable<StaticCtx> {
+  using T = StaticWorld;
+};
 
 // ---- Aviary.state(i) / aux_state(i) / contact_array of the drone in row j, and the hi / lo words of its position ------------
 // Returns the contact flag.

@@ -326,6 +326,41 @@ int tail_env_step(PfbContext* h, const float* noise, bool randact, cudaStream_t 
   return 0;
 }
 
+// ---- host side of the Aviary step (pfb_aviary_step) of every vehicle kind and of the mixed-kind handle ----
+// Each kind passes one generic lambda `launch(AviaryVariant<INJECT, CONTACT, World>{sb})` that launches its step kernel and
+// returns 0 or the result of fail().  INJECT: injected noise; CONTACT: aviary_contact_response(h); World: pfb::StaticCtx with
+// the handle's static bodies `sb` (step_statics), or pfb::NoStatic with sb = nullptr.  The kernel takes world_table(v),
+// v.pose() and v.bits().
+template <bool INJECT, bool CONTACT, class World>
+struct AviaryVariant {
+  static constexpr bool inject = INJECT, contact = CONTACT;
+  using world = World;
+  const StaticBodies* sb;
+  const float* pose() const { return sb ? sb->d_pose : nullptr; }
+  uint32_t* bits() const { return sb ? sb->d_bits : nullptr; }
+};
+
+// the static-body table argument of the step kernel: an empty one for NoStatic (WorldTable, pfb_aviary.cuh)
+template <bool INJECT, bool CONTACT>
+pfb::NoStaticTable world_table(AviaryVariant<INJECT, CONTACT, pfb::NoStatic>) { return {}; }
+template <bool INJECT, bool CONTACT>
+const pfb::StaticWorld& world_table(AviaryVariant<INJECT, CONTACT, pfb::StaticCtx> v) { return v.sb->world; }
+
+template <bool INJECT, bool CONTACT, class Launch>
+int aviary_step_world(const StaticBodies* sb, Launch& launch) {
+  return sb ? launch(AviaryVariant<INJECT, CONTACT, pfb::StaticCtx>{sb}) : launch(AviaryVariant<INJECT, CONTACT, pfb::NoStatic>{nullptr});
+}
+template <class Launch>
+int aviary_step_launch(PfbContext* h, const float* noise, Launch&& launch) {
+  const StaticBodies* sb = step_statics(h);
+  int rc;
+  if (aviary_contact_response(h)) rc = noise ? aviary_step_world<true, true>(sb, launch) : aviary_step_world<false, true>(sb, launch);
+  else rc = noise ? aviary_step_world<true, false>(sb, launch) : aviary_step_world<false, false>(sb, launch);
+  if (rc) return rc;
+  LAUNCH_CHECK(h);
+  return 0;
+}
+
 // `reset(grid)` launches the kind's reset kernel over every env and returns 0 or the result of fail()
 template <class Reset, class Launch>
 int tail_env_reset(PfbContext* h, const uint8_t* mask, cudaStream_t s, Reset&& reset, Launch&& launch) {

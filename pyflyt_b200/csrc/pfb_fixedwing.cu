@@ -49,62 +49,40 @@ __global__ void __launch_bounds__(kBlock) k_fw_get_base_state(const __grid_const
   fw_get_base_drone(st, ist, N, i, i, o);
 }
 
-// CONTACT: the ground pushes back (Aviary handles with contact_response)
-template <int MODE, bool INJECT, bool CONTACT>
+// n_steps x Aviary.step() in flight mode MODE, or MODE = kModePerDrone: drone i in modes[i] (pfb_set_modes; only the command
+// mapping branches on it).  CONTACT: the ground pushes back (Aviary handles with contact_response).  World = StaticCtx: against
+// the static bodies of each drone's world (pfb_add_static_body), bits[i] = what drone i touched during its last Aviary step.
+// Per-drone modes and static bodies exist on Aviary handles only, whose setpoints are 6 wide; one uniform mode reads sp_dim floats
+// (4 behind Fixedwing-Waypoints).
+template <int MODE, bool INJECT, bool CONTACT, class World>
 __global__ void __launch_bounds__(kBlock, kMinBlocks)
-    k_fw_aviary_step(const __grid_constant__ FixedwingParams p, const __grid_constant__ RngParams rng, float* __restrict__ st,
-                     int32_t* __restrict__ ist, const float* __restrict__ setpoint, const float* __restrict__ noise,
-                     int n_steps, uint32_t seq, int sp_dim, int64_t N) {
+    k_fw_aviary_step(const __grid_constant__ FixedwingParams p, const __grid_constant__ RngParams rng, const __grid_constant__ typename WorldTable<World>::T world,
+                     const float* __restrict__ pose, uint32_t* __restrict__ bits, float* __restrict__ st, int32_t* __restrict__ ist,
+                     const float* __restrict__ setpoint, const int8_t* __restrict__ modes, const float* __restrict__ noise, int n_steps,
+                     uint32_t seq, int sp_dim, int64_t N) {
   int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= N) return;
+  constexpr bool kPerDrone = MODE == kModePerDrone;
+  World w{&world, pose, N, i, 0u};
+  int mode = MODE;
+  if constexpr (kPerDrone && !World::kOn) mode = modes[i];  // where the mode is read steers ptxas' schedule (DESIGN.md §4h)
   FixedwingRegs s;
   fixedwing_load(st, ist, N, i, s);
+  if constexpr (kPerDrone || World::kOn) {
+    load_setpoint<6, 6>(setpoint, i, s.sp);
+  } else {
 #pragma unroll
-  for (int k = 0; k < 6; ++k) s.sp[k] = k < sp_dim ? __ldg(setpoint + (int64_t)sp_dim * i + k) : 0.0f;
+    for (int k = 0; k < 6; ++k) s.sp[k] = k < sp_dim ? __ldg(setpoint + (int64_t)sp_dim * i + k) : 0.0f;
+  }
+  if constexpr (kPerDrone && World::kOn) mode = modes[i];
   auto nz = make_noise<INJECT>(noise, N, i, rng, seq, TAG_AVIARY, p.noise_loc, p.ratio);
   if (fixedwing_full_model(p)) {  // launch-uniform: all surfaces, no wind -> the one-basic-block substep (pfb_fixedwing.cuh)
-    for (int k = 0; k < n_steps; ++k) fixedwing_aviary_step<MODE, true, CONTACT>(p, s, nz);
-  } else {
-    for (int k = 0; k < n_steps; ++k) fixedwing_aviary_step<MODE, false, CONTACT>(p, s, nz);
-  }
-  fixedwing_store(st, ist, N, i, s);
-}
-
-// n_steps x Aviary.step() against the static bodies of each drone's world (pfb_add_static_body; Aviary handles, 6-wide setpoints):
-// one flight mode MODE, or MODE = kStaticPerDrone = drone i in modes[i].  bits[i]: what drone i touched during its last Aviary step.
-constexpr int kStaticPerDrone = 1;
-template <int MODE, bool INJECT, bool CONTACT>
-__global__ void __launch_bounds__(kBlock, kMinBlocks)
-    k_fw_aviary_step_static(const __grid_constant__ FixedwingParams p, const __grid_constant__ RngParams rng, const __grid_constant__ StaticWorld world,
-                            const float* __restrict__ pose, uint32_t* __restrict__ bits, float* __restrict__ st, int32_t* __restrict__ ist,
-                            const float* __restrict__ setpoint, const int8_t* __restrict__ modes, const float* __restrict__ noise, int n_steps,
-                            uint32_t seq, int64_t N) {
-  int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
-  if (i >= N) return;
-  StaticCtx w{&world, pose, N, i, 0u};
-  FixedwingRegs s;
-  fixedwing_load(st, ist, N, i, s);
-  load_setpoint<6, 6>(setpoint, i, s.sp);
-  const int mode = MODE == kStaticPerDrone ? modes[i] : MODE;
-  auto nz = make_noise<INJECT>(noise, N, i, rng, seq, TAG_AVIARY, p.noise_loc, p.ratio);
-  if (fixedwing_full_model(p)) {
     for (int k = 0; k < n_steps; ++k) fixedwing_aviary_step_any<true, CONTACT>(p, s, mode, nz, &w);
   } else {
     for (int k = 0; k < n_steps; ++k) fixedwing_aviary_step_any<false, CONTACT>(p, s, mode, nz, &w);
   }
   fixedwing_store(st, ist, N, i, s);
-  bits[i] = w.bits;
-}
-
-// k_fw_aviary_step with drone i in flight mode modes[i] (pfb_set_modes; step body fixedwing_aviary_step_any)
-template <bool INJECT, bool CONTACT>
-__global__ void __launch_bounds__(kBlock, kMinBlocks)
-    k_fw_aviary_step_modes(const __grid_constant__ FixedwingParams p, const __grid_constant__ RngParams rng, float* __restrict__ st,
-                           int32_t* __restrict__ ist, const float* __restrict__ setpoint, const int8_t* __restrict__ modes,
-                           const float* __restrict__ noise, int n_steps, uint32_t seq, int64_t N) {
-  int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
-  if (i >= N) return;
-  fw_aviary_step_drone<INJECT, CONTACT, 6>(p, rng, st, ist, N, i, modes, setpoint, noise, N, i, n_steps, seq);  // Aviary handles: 6-wide setpoints
+  if constexpr (World::kOn) bits[i] = w.bits;
 }
 
 __global__ void __launch_bounds__(kBlock) k_fw_observe(const float* __restrict__ st, const int32_t* __restrict__ ist,
@@ -423,53 +401,17 @@ static int fw_set_modes(PfbContext* h, const int8_t*, cudaStream_t s) {
 
 int fw_aviary_step(PfbContext* h, int n_steps, const float* noise, cudaStream_t s) {
   const uint32_t seq = (uint32_t)h->aviary_seq++;
-  const int g = grid_for(h->n);
-  const bool contact = aviary_contact_response(h);
-  if (const StaticBodies* sb = step_statics(h)) {  // Aviary handles only (6-wide setpoints)
-#define FWS_ARGS h->fw, h->rng, sb->world, sb->d_pose, sb->d_bits, h->buf.state, h->buf.istate, h->buf.setpoint, h->d_modes, noise, n_steps, seq, h->n
-#define FWS_LAUNCH(M) \
-    if (contact) { if (noise) k_fw_aviary_step_static<M, true, true><<<g, kBlock, 0, s>>>(FWS_ARGS); else k_fw_aviary_step_static<M, false, true><<<g, kBlock, 0, s>>>(FWS_ARGS); } \
-    else { if (noise) k_fw_aviary_step_static<M, true, false><<<g, kBlock, 0, s>>>(FWS_ARGS); else k_fw_aviary_step_static<M, false, false><<<g, kBlock, 0, s>>>(FWS_ARGS); }
-    if (h->mode == kModePerDrone) { FWS_LAUNCH(kStaticPerDrone) }
-    else if (h->mode == 0) { FWS_LAUNCH(0) }
-    else { FWS_LAUNCH(-1) }
-#undef FWS_LAUNCH
-#undef FWS_ARGS
-    LAUNCH_CHECK(h);
-    return 0;
-  }
-  if (h->mode == kModePerDrone) {  // pfb_set_modes: Aviary handles only (6-wide setpoints)
-#define FWM_ARGS h->fw, h->rng, h->buf.state, h->buf.istate, h->buf.setpoint, h->d_modes, noise, n_steps, seq, h->n
-    if (contact) {
-      if (noise) k_fw_aviary_step_modes<true, true><<<g, kBlock, 0, s>>>(FWM_ARGS);
-      else k_fw_aviary_step_modes<false, true><<<g, kBlock, 0, s>>>(FWM_ARGS);
-    } else {
-      if (noise) k_fw_aviary_step_modes<true, false><<<g, kBlock, 0, s>>>(FWM_ARGS);
-      else k_fw_aviary_step_modes<false, false><<<g, kBlock, 0, s>>>(FWM_ARGS);
-    }
-#undef FWM_ARGS
-    LAUNCH_CHECK(h);
-    return 0;
-  }
-#define FW_ARGS h->fw, h->rng, h->buf.state, h->buf.istate, h->buf.setpoint, noise, n_steps, seq, fw_setpoint_dim(h), h->n
-  if (contact) {
-    if (h->mode == 0) {
-      if (noise) k_fw_aviary_step<0, true, true><<<g, kBlock, 0, s>>>(FW_ARGS);
-      else k_fw_aviary_step<0, false, true><<<g, kBlock, 0, s>>>(FW_ARGS);
-    } else {
-      if (noise) k_fw_aviary_step<-1, true, true><<<g, kBlock, 0, s>>>(FW_ARGS);
-      else k_fw_aviary_step<-1, false, true><<<g, kBlock, 0, s>>>(FW_ARGS);
-    }
-  } else if (h->mode == 0) {
-    if (noise) k_fw_aviary_step<0, true, false><<<g, kBlock, 0, s>>>(FW_ARGS);
-    else k_fw_aviary_step<0, false, false><<<g, kBlock, 0, s>>>(FW_ARGS);
-  } else {
-    if (noise) k_fw_aviary_step<-1, true, false><<<g, kBlock, 0, s>>>(FW_ARGS);
-    else k_fw_aviary_step<-1, false, false><<<g, kBlock, 0, s>>>(FW_ARGS);
-  }
-#undef FW_ARGS
-  LAUNCH_CHECK(h);
-  return 0;
+  return aviary_step_launch(h, noise, [&](auto v) {
+    using V = decltype(v);
+    auto launch = [&](auto mode) {
+      k_fw_aviary_step<decltype(mode)::value, V::inject, V::contact, typename V::world><<<grid_for(h->n), kBlock, 0, s>>>(
+          h->fw, h->rng, world_table(v), v.pose(), v.bits(), h->buf.state, h->buf.istate, h->buf.setpoint, h->d_modes, noise, n_steps, seq,
+          fw_setpoint_dim(h), h->n);
+      return 0;
+    };
+    if (h->mode == kModePerDrone) return launch(std::integral_constant<int, kModePerDrone>{});
+    return h->mode == 0 ? launch(std::integral_constant<int, 0>{}) : launch(std::integral_constant<int, -1>{});
+  });
 }
 
 static int fw_set_base_state(PfbContext* h, const BaseStateIn& a, cudaStream_t s) {

@@ -101,17 +101,22 @@ static_assert(sizeof(MixedStep<QuadXModelSet>) <= 32764, "the mixed step's __gri
 // drone's trajectory is bit-equal to the one it flies in a uniform handle with the same seed.  CONTACT: the floor pushes back.
 // RATES (a handle whose drones run at several control rates): every drone runs the handle's U substeps per Aviary step and
 // its control tick on the substeps that are multiples of its slot's ratio; its noise is keyed with U, whatever its own ratio.
-// The branches spell out the step bodies of pfb_aviary.cuh rather than call them: called, their pointers and counts are held
-// in registers across the step loop instead of being read from the parameter bank where they are used, and the kernel needs
-// more stack.
-template <bool INJECT, bool CONTACT, bool RATES, class PS>
-__global__ void __launch_bounds__(kBlock, kMinBlocks) k_mixed_aviary_step(const __grid_constant__ MixedStep<PS> a) {
+// World = StaticCtx: against the static bodies of drone u's world (pfb_add_static_body), bits[u] = what drone u touched during
+// its last Aviary step.
+// The branches spell out the step bodies of the single-kind step kernels rather than share them: shared, their pointers and
+// counts are held in registers across the step loop instead of being read from the parameter bank where they are used, and the
+// kernel needs more stack.  The floor-only path hands the substeps a null world, as the kernel did before it had a World: a
+// pointer to its unused NoStatic changes the schedule of 8 of the 16 floor-only instantiations (DESIGN.md §4h).
+template <bool INJECT, bool CONTACT, bool RATES, class PS, class World>
+__device__ __forceinline__ void mixed_aviary_step(const MixedStep<PS>& a, const typename WorldTable<World>::T* world, const float* pose,
+                                                  uint32_t* bits) {
   const MixedRows& r = a.r;
   const int b = blockIdx.x;
   if (b < r.cta_qx) {
     const int64_t j = (int64_t)b * kBlock + threadIdx.x;
     if (j >= r.n_qx) return;
     const int64_t u = r.slot_user[j];
+    World w{world, pose, a.n, u, 0u};
     const QuadXParams& p = qx_model(a.qx, j);
     const int mode = a.slot_mode[j];
     QuadXRegs s;
@@ -123,16 +128,18 @@ __global__ void __launch_bounds__(kBlock, kMinBlocks) k_mixed_aviary_step(const 
     if constexpr (RATES) {
       const int ratio = a.slot_ratio[j];
       auto nz = make_noise<INJECT>(a.noise, a.n, u, a.rng, a.seq, TAG_AVIARY, qx_model0(a.qx).noise_loc, a.U);
-      for (int k = 0; k < a.n_steps; ++k) quadx_aviary_step_rates<CONTACT>(p, s, mode, ratio, a.U, nz);
+      for (int k = 0; k < a.n_steps; ++k) quadx_aviary_step_rates<CONTACT>(p, s, mode, ratio, a.U, nz, World::kOn ? &w : nullptr);
     } else {
       auto nz = make_noise<INJECT>(a.noise, a.n, u, a.rng, a.seq, TAG_AVIARY, qx_model0(a.qx).noise_loc, qx_model0(a.qx).ratio);
-      for (int k = 0; k < a.n_steps; ++k) quadx_aviary_step_any<CONTACT>(p, s, mode, nz);
+      for (int k = 0; k < a.n_steps; ++k) quadx_aviary_step_any<CONTACT>(p, s, mode, nz, World::kOn ? &w : nullptr);
     }
     quadx_store_tile<7, kTileGroupStride>(r.qx_st + qx_tile_base(j, QX_ROWS), s, step_count);
+    if constexpr (World::kOn) bits[u] = w.bits;
   } else if (b < r.cta_qx + r.cta_fw) {
     const int64_t j = (int64_t)(b - r.cta_qx) * kBlock + threadIdx.x;
     if (j >= r.n_fw) return;
     const int64_t u = r.slot_user[r.n_qx + j];
+    World w{world, pose, a.n, u, 0u};
     const int mode = a.slot_mode[r.n_qx + j];
     const FixedwingParams& p = a.fw;
     FixedwingRegs s;
@@ -143,23 +150,25 @@ __global__ void __launch_bounds__(kBlock, kMinBlocks) k_mixed_aviary_step(const 
       const int ratio = a.slot_ratio[r.n_qx + j];
       auto nz = make_noise<INJECT>(a.noise, a.n, u, a.rng, a.seq, TAG_AVIARY, p.noise_loc, a.U);
       if (fixedwing_full_model(p)) {
-        for (int k = 0; k < a.n_steps; ++k) fixedwing_aviary_step_rates<true, CONTACT>(p, s, mode, ratio, a.U, nz);
+        for (int k = 0; k < a.n_steps; ++k) fixedwing_aviary_step_rates<true, CONTACT>(p, s, mode, ratio, a.U, nz, World::kOn ? &w : nullptr);
       } else {
-        for (int k = 0; k < a.n_steps; ++k) fixedwing_aviary_step_rates<false, CONTACT>(p, s, mode, ratio, a.U, nz);
+        for (int k = 0; k < a.n_steps; ++k) fixedwing_aviary_step_rates<false, CONTACT>(p, s, mode, ratio, a.U, nz, World::kOn ? &w : nullptr);
       }
     } else {
       auto nz = make_noise<INJECT>(a.noise, a.n, u, a.rng, a.seq, TAG_AVIARY, p.noise_loc, p.ratio);
       if (fixedwing_full_model(p)) {
-        for (int k = 0; k < a.n_steps; ++k) fixedwing_aviary_step_any<true, CONTACT>(p, s, mode, nz);
+        for (int k = 0; k < a.n_steps; ++k) fixedwing_aviary_step_any<true, CONTACT>(p, s, mode, nz, World::kOn ? &w : nullptr);
       } else {
-        for (int k = 0; k < a.n_steps; ++k) fixedwing_aviary_step_any<false, CONTACT>(p, s, mode, nz);
+        for (int k = 0; k < a.n_steps; ++k) fixedwing_aviary_step_any<false, CONTACT>(p, s, mode, nz, World::kOn ? &w : nullptr);
       }
     }
     fixedwing_store(r.fw_st, r.fw_ist, r.n_fw, j, s);
+    if constexpr (World::kOn) bits[u] = w.bits;
   } else {
     const int64_t j = (int64_t)(b - r.cta_qx - r.cta_fw) * kBlock + threadIdx.x;
     if (j >= r.n_rk) return;
     const int64_t u = r.slot_user[r.n_qx + r.n_fw + j];
+    World w{world, pose, a.n, u, 0u};
     const RocketParams& p = a.rk;
     RocketRegs s;
     rocket_load(r.rk_st, r.rk_ist, r.n_rk, j, s);
@@ -168,103 +177,21 @@ __global__ void __launch_bounds__(kBlock, kMinBlocks) k_mixed_aviary_step(const 
     if constexpr (RATES) {
       const int ratio = a.slot_ratio[r.n_qx + r.n_fw + j];
       auto nz = make_noise<INJECT>(a.noise, a.n, u, a.rng, a.seq, TAG_AVIARY, p.noise_loc, a.U);
-      for (int k = 0; k < a.n_steps; ++k) rocket_aviary_step_rates(p, s, ratio, a.U, nz);
+      for (int k = 0; k < a.n_steps; ++k) rocket_aviary_step_rates(p, s, ratio, a.U, nz, World::kOn ? &w : nullptr);
     } else {
       auto nz = make_noise<INJECT>(a.noise, a.n, u, a.rng, a.seq, TAG_AVIARY, p.noise_loc, p.ratio);
-      for (int k = 0; k < a.n_steps; ++k) rocket_aviary_step(p, s, nz, false);
+      for (int k = 0; k < a.n_steps; ++k) rocket_aviary_step(p, s, nz, false, World::kOn ? &w : nullptr);
     }
     rocket_store(r.rk_st, r.rk_ist, r.n_rk, j, s);
+    if constexpr (World::kOn) bits[u] = w.bits;
   }
 }
 
-// The body of k_mixed_aviary_step with the static bodies of drone u's world, whose bits go to bits[u].  A
-// copy rather than a shared body, so that k_mixed_aviary_step stays the code it was.
-template <bool INJECT, bool CONTACT, bool RATES, class PS>
-__device__ __forceinline__ void mixed_aviary_step_static(const MixedStep<PS>& a, const StaticWorld* world, const float* pose, uint32_t* bits) {
-  const MixedRows& r = a.r;
-  const int b = blockIdx.x;
-  if (b < r.cta_qx) {
-    const int64_t j = (int64_t)b * kBlock + threadIdx.x;
-    if (j >= r.n_qx) return;
-    const int64_t u = r.slot_user[j];
-    StaticCtx w{world, pose, a.n, u, 0u};
-    const QuadXParams& p = qx_model(a.qx, j);
-    const int mode = a.slot_mode[j];
-    QuadXRegs s;
-    int step_count;
-    quadx_load_tile<7, kTileGroupStride>(r.qx_st + qx_tile_base(j, QX_ROWS), s, step_count);
-    quadx_mask_pid(s, mode);
-#pragma unroll
-    for (int c = 0; c < 4; ++c) s.sp[c] = __ldg(a.setpoint + kMixedSetpointDim * u + c);
-    if constexpr (RATES) {
-      const int ratio = a.slot_ratio[j];
-      auto nz = make_noise<INJECT>(a.noise, a.n, u, a.rng, a.seq, TAG_AVIARY, qx_model0(a.qx).noise_loc, a.U);
-      for (int k = 0; k < a.n_steps; ++k) quadx_aviary_step_rates<CONTACT>(p, s, mode, ratio, a.U, nz, &w);
-    } else {
-      auto nz = make_noise<INJECT>(a.noise, a.n, u, a.rng, a.seq, TAG_AVIARY, qx_model0(a.qx).noise_loc, qx_model0(a.qx).ratio);
-      for (int k = 0; k < a.n_steps; ++k) quadx_aviary_step_any<CONTACT>(p, s, mode, nz, &w);
-    }
-    quadx_store_tile<7, kTileGroupStride>(r.qx_st + qx_tile_base(j, QX_ROWS), s, step_count);
-    bits[u] = w.bits;
-  } else if (b < r.cta_qx + r.cta_fw) {
-    const int64_t j = (int64_t)(b - r.cta_qx) * kBlock + threadIdx.x;
-    if (j >= r.n_fw) return;
-    const int64_t u = r.slot_user[r.n_qx + j];
-    StaticCtx w{world, pose, a.n, u, 0u};
-    const int mode = a.slot_mode[r.n_qx + j];
-    const FixedwingParams& p = a.fw;
-    FixedwingRegs s;
-    fixedwing_load(r.fw_st, r.fw_ist, r.n_fw, j, s);
-#pragma unroll
-    for (int c = 0; c < 6; ++c) s.sp[c] = __ldg(a.setpoint + kMixedSetpointDim * u + c);
-    if constexpr (RATES) {
-      const int ratio = a.slot_ratio[r.n_qx + j];
-      auto nz = make_noise<INJECT>(a.noise, a.n, u, a.rng, a.seq, TAG_AVIARY, p.noise_loc, a.U);
-      if (fixedwing_full_model(p)) {
-        for (int k = 0; k < a.n_steps; ++k) fixedwing_aviary_step_rates<true, CONTACT>(p, s, mode, ratio, a.U, nz, &w);
-      } else {
-        for (int k = 0; k < a.n_steps; ++k) fixedwing_aviary_step_rates<false, CONTACT>(p, s, mode, ratio, a.U, nz, &w);
-      }
-    } else {
-      auto nz = make_noise<INJECT>(a.noise, a.n, u, a.rng, a.seq, TAG_AVIARY, p.noise_loc, p.ratio);
-      if (fixedwing_full_model(p)) {
-        for (int k = 0; k < a.n_steps; ++k) fixedwing_aviary_step_any<true, CONTACT>(p, s, mode, nz, &w);
-      } else {
-        for (int k = 0; k < a.n_steps; ++k) fixedwing_aviary_step_any<false, CONTACT>(p, s, mode, nz, &w);
-      }
-    }
-    fixedwing_store(r.fw_st, r.fw_ist, r.n_fw, j, s);
-    bits[u] = w.bits;
-  } else {
-    const int64_t j = (int64_t)(b - r.cta_qx - r.cta_fw) * kBlock + threadIdx.x;
-    if (j >= r.n_rk) return;
-    const int64_t u = r.slot_user[r.n_qx + r.n_fw + j];
-    StaticCtx w{world, pose, a.n, u, 0u};
-    const RocketParams& p = a.rk;
-    RocketRegs s;
-    rocket_load(r.rk_st, r.rk_ist, r.n_rk, j, s);
-#pragma unroll
-    for (int c = 0; c < 7; ++c) s.sp[c] = __ldg(a.setpoint + kMixedSetpointDim * u + c);
-    if constexpr (RATES) {
-      const int ratio = a.slot_ratio[r.n_qx + r.n_fw + j];
-      auto nz = make_noise<INJECT>(a.noise, a.n, u, a.rng, a.seq, TAG_AVIARY, p.noise_loc, a.U);
-      for (int k = 0; k < a.n_steps; ++k) rocket_aviary_step_rates(p, s, ratio, a.U, nz, &w);
-    } else {
-      auto nz = make_noise<INJECT>(a.noise, a.n, u, a.rng, a.seq, TAG_AVIARY, p.noise_loc, p.ratio);
-      for (int k = 0; k < a.n_steps; ++k) rocket_aviary_step(p, s, nz, false, &w);
-    }
-    rocket_store(r.rk_st, r.rk_ist, r.n_rk, j, s);
-    bits[u] = w.bits;
-  }
-}
-
-// k_mixed_aviary_step against the static bodies of each drone's world (pfb_add_static_body); bits[u]: what drone u touched during
-// its last Aviary step
-template <bool INJECT, bool CONTACT, bool RATES, class PS>
+template <bool INJECT, bool CONTACT, bool RATES, class PS, class World>
 __global__ void __launch_bounds__(kBlock, kMinBlocks)
-    k_mixed_aviary_step_static(const __grid_constant__ MixedStep<PS> a, const __grid_constant__ StaticWorld world, const float* __restrict__ pose,
-                               uint32_t* __restrict__ bits) {
-  mixed_aviary_step_static<INJECT, CONTACT, RATES, PS>(a, &world, pose, bits);
+    k_mixed_aviary_step(const __grid_constant__ MixedStep<PS> a, const __grid_constant__ typename WorldTable<World>::T world,
+                        const float* __restrict__ pose, uint32_t* __restrict__ bits) {
+  mixed_aviary_step<INJECT, CONTACT, RATES, PS, World>(a, &world, pose, bits);
 }
 
 struct MixedObserve {
@@ -462,8 +389,9 @@ static int mx_set_modes(PfbContext* h, const int8_t* modes, cudaStream_t s) {
   return set_slot_modes(h, s);
 }
 
-template <bool INJECT, bool CONTACT, bool RATES, class PS>
-static void launch_step(const PfbContext* h, const PS& ps, const float* noise, int n_steps, uint32_t seq, cudaStream_t s) {
+// the launch-uniform arguments of k_mixed_aviary_step
+template <class PS>
+static MixedStep<PS> mixed_step(const PfbContext* h, const PS& ps, const float* noise, int n_steps, uint32_t seq) {
   const MixedKinds* m = h->mixed;
   MixedStep<PS> a;
   memset(&a, 0, sizeof(a));
@@ -480,26 +408,20 @@ static void launch_step(const PfbContext* h, const PS& ps, const float* noise, i
   a.seq = seq;
   a.slot_ratio = m->d_slot_ratio;
   a.U = m->U;
-  if (const StaticBodies* sb = step_statics(h))
-    k_mixed_aviary_step_static<INJECT, CONTACT, RATES, PS><<<grid_all(m), kBlock, 0, s>>>(a, sb->world, sb->d_pose, sb->d_bits);
-  else
-    k_mixed_aviary_step<INJECT, CONTACT, RATES, PS><<<grid_all(m), kBlock, 0, s>>>(a);
-}
-
-// RATES: several control rates (d_slot_ratio set), chosen by the handle and uniform over the launch
-template <bool RATES>
-static void launch_steps(const PfbContext* h, const float* noise, int n_steps, uint32_t seq, cudaStream_t s) {
-  const bool contact = h->env.contact_response != 0;
-  QX_PARAMS_SWITCH(h, (contact ? (noise ? launch_step<true, true, RATES>(h, ps, noise, n_steps, seq, s) : launch_step<false, true, RATES>(h, ps, noise, n_steps, seq, s))
-                                : (noise ? launch_step<true, false, RATES>(h, ps, noise, n_steps, seq, s) : launch_step<false, false, RATES>(h, ps, noise, n_steps, seq, s))));
+  return a;
 }
 
 static int mx_aviary_step(PfbContext* h, int n_steps, const float* noise, cudaStream_t s) {
   const uint32_t seq = (uint32_t)h->aviary_seq++;
-  if (h->mixed->d_slot_ratio) launch_steps<true>(h, noise, n_steps, seq, s);
-  else launch_steps<false>(h, noise, n_steps, seq, s);
-  LAUNCH_CHECK(h);
-  return 0;
+  return aviary_step_launch(h, noise, [&](auto v) {
+    using V = decltype(v);
+    auto launch = [&](auto rates) {  // RATES: several control rates (d_slot_ratio set), chosen by the handle
+      QX_PARAMS_SWITCH(h, (k_mixed_aviary_step<V::inject, V::contact, decltype(rates)::value, PS, typename V::world><<<grid_all(h->mixed), kBlock, 0, s>>>(
+                              mixed_step(h, ps, noise, n_steps, seq), world_table(v), v.pose(), v.bits())));
+      return 0;
+    };
+    return h->mixed->d_slot_ratio ? launch(std::true_type{}) : launch(std::false_type{});
+  });
 }
 
 static int mx_observe(PfbContext* h, cudaStream_t s) {

@@ -41,23 +41,39 @@ __global__ void __launch_bounds__(kBlock) k_quadx_set_mode(float* __restrict__ s
   reinterpret_cast<float4*>(setpoint)[i] = make_float4(s.sp[0], s.sp[1], s.sp[2], s.sp[3]);
 }
 
-// n_steps x Aviary.step() (aviary.py:480-531); CONTACT: the floor pushes back (Aviary handles with contact_response)
-template <int MODE, bool INJECT, bool TILED, class PS, bool CONTACT>
+// n_steps x Aviary.step() (aviary.py:480-531) in flight mode MODE, or MODE = kModePerDrone: drone i in modes[i] (pfb_set_modes).
+// Per-drone modes move every PID row (the mode-7 set); quadx_mask_pid gives each drone the PID memory the uniform kernel of its
+// mode would load, so both store the same words.  CONTACT: the floor pushes back (Aviary handles with contact_response).
+// World = StaticCtx: against the static bodies of each drone's world (pfb_add_static_body), bits[i] = what drone i touched
+// during its last Aviary step.  TILED = false (field-major state) is QuadX-Waypoints' layout, which has none of the three.
+template <int MODE, bool INJECT, bool TILED, class PS, bool CONTACT, class World>
 __global__ void __launch_bounds__(kBlock, kMinBlocks)
-    k_quadx_aviary_step(const __grid_constant__ PS ps, const __grid_constant__ RngParams rng,
-                        float* __restrict__ st, int32_t* __restrict__ ist, int rows, const float* __restrict__ setpoint,
-                        const float* __restrict__ noise, int n_steps, uint32_t seq, int64_t N) {
+    k_quadx_aviary_step(const __grid_constant__ PS ps, const __grid_constant__ RngParams rng, const __grid_constant__ typename WorldTable<World>::T world,
+                        const float* __restrict__ pose, uint32_t* __restrict__ bits, float* __restrict__ st, int32_t* __restrict__ ist, int rows,
+                        const float* __restrict__ setpoint, const int8_t* __restrict__ modes, const float* __restrict__ noise, int n_steps,
+                        uint32_t seq, int64_t N) {
   int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= N) return;
+  constexpr bool kPerDrone = MODE == kModePerDrone;
+  constexpr int LM = kPerDrone ? 7 : MODE;  // the PID rows moved
   const QuadXParams& p = qx_model(ps, i);
+  World w{&world, pose, N, i, 0u};
+  int mode = MODE;
+  if constexpr (kPerDrone && !World::kOn) mode = modes[i];  // where the mode is read steers ptxas' schedule (DESIGN.md §4h)
   QuadXRegs s;
   int step_count;
-  qx_load_any<MODE, TILED>(st, ist, rows, N, i, s, step_count);
+  qx_load_any<LM, TILED>(st, ist, rows, N, i, s, step_count);
+  if constexpr (kPerDrone && World::kOn) mode = modes[i];
+  if constexpr (kPerDrone) quadx_mask_pid(s, mode);
   float4 sp = __ldg(reinterpret_cast<const float4*>(setpoint) + i);
   s.sp[0] = sp.x; s.sp[1] = sp.y; s.sp[2] = sp.z; s.sp[3] = sp.w;
   auto nz = make_noise<INJECT>(noise, N, i, rng, seq, TAG_AVIARY, qx_model0(ps).noise_loc, qx_model0(ps).ratio);
-  for (int k = 0; k < n_steps; ++k) quadx_aviary_step<MODE, CONTACT>(p, s, nz);
-  qx_store_any<MODE, TILED>(st, ist, rows, N, i, s, step_count);
+  for (int k = 0; k < n_steps; ++k) {
+    if constexpr (kPerDrone) quadx_aviary_step_any<CONTACT>(p, s, mode, nz, &w);
+    else quadx_aviary_step<MODE, CONTACT>(p, s, nz, &w);
+  }
+  qx_store_any<LM, TILED>(st, ist, rows, N, i, s, step_count);
+  if constexpr (World::kOn) bits[i] = w.bits;
 }
 
 // ---- one flight mode per drone (pfb_set_modes; Aviary handles, warp-tiled) ----------------------------------------------
@@ -67,49 +83,6 @@ __global__ void __launch_bounds__(kBlock) k_quadx_set_modes(float* __restrict__ 
   int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= N) return;
   qx_set_mode_drone<4>(st, rows, i, modes, setpoint, i);
-}
-
-// n_steps x Aviary.step() with drone i in flight mode modes[i].  Every PID row is moved (the mode-7 set); quadx_mask_pid
-// gives each drone the PID memory the uniform kernel of its mode would load, so both store the same words.
-template <bool INJECT, class PS, bool CONTACT>
-__global__ void __launch_bounds__(kBlock, kMinBlocks)
-    k_quadx_aviary_step_modes(const __grid_constant__ PS ps, const __grid_constant__ RngParams rng, float* __restrict__ st, int rows,
-                              const float* __restrict__ setpoint, const int8_t* __restrict__ modes, const float* __restrict__ noise,
-                              int n_steps, uint32_t seq, int64_t N) {
-  int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
-  if (i >= N) return;
-  qx_aviary_step_drone<INJECT, CONTACT, 4>(ps, rng, st, rows, i, modes, setpoint, noise, N, i, n_steps, seq);
-}
-
-// n_steps x Aviary.step() against the static bodies of each drone's world (pfb_add_static_body; Aviary handles, warp-tiled): one
-// flight mode MODE, or MODE = kStaticPerDrone = drone i in modes[i] as k_quadx_aviary_step_modes.  bits[i]: what drone i touched
-// during its last Aviary step.
-constexpr int kStaticPerDrone = 8;
-template <int MODE, bool INJECT, class PS, bool CONTACT>
-__global__ void __launch_bounds__(kBlock, kMinBlocks)
-    k_quadx_aviary_step_static(const __grid_constant__ PS ps, const __grid_constant__ RngParams rng, const __grid_constant__ StaticWorld world,
-                               const float* __restrict__ pose, uint32_t* __restrict__ bits, float* __restrict__ st, int rows,
-                               const float* __restrict__ setpoint, const int8_t* __restrict__ modes, const float* __restrict__ noise,
-                               int n_steps, uint32_t seq, int64_t N) {
-  int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
-  if (i >= N) return;
-  constexpr int LM = MODE == kStaticPerDrone ? 7 : MODE;  // the rows moved: every PID row for per-drone modes
-  const QuadXParams& p = qx_model(ps, i);
-  StaticCtx w{&world, pose, N, i, 0u};
-  QuadXRegs s;
-  int step_count;
-  quadx_load_tile<LM, kTileGroupStride>(st + qx_tile_base(i, rows), s, step_count);
-  const int mode = MODE == kStaticPerDrone ? modes[i] : MODE;
-  if (MODE == kStaticPerDrone) quadx_mask_pid(s, mode);
-  float4 sp = __ldg(reinterpret_cast<const float4*>(setpoint) + i);
-  s.sp[0] = sp.x; s.sp[1] = sp.y; s.sp[2] = sp.z; s.sp[3] = sp.w;
-  auto nz = make_noise<INJECT>(noise, N, i, rng, seq, TAG_AVIARY, qx_model0(ps).noise_loc, qx_model0(ps).ratio);
-  for (int k = 0; k < n_steps; ++k) {
-    if constexpr (MODE == kStaticPerDrone) quadx_aviary_step_any<CONTACT>(p, s, mode, nz, &w);
-    else quadx_aviary_step<MODE, CONTACT>(p, s, nz, &w);
-  }
-  quadx_store_tile<LM, kTileGroupStride>(st + qx_tile_base(i, rows), s, step_count);
-  bits[i] = w.bits;
 }
 
 // Aviary.state(i) / aux_state(i) / contact_array  -> row-major API buffers
@@ -1011,54 +984,30 @@ static int qx_set_modes(PfbContext* h, const int8_t*, cudaStream_t s) {
   return 0;
 }
 
+template <int MODE, bool TILED, class V>
+static void qx_launch_step(PfbContext* h, V v, int n_steps, const float* noise, uint32_t seq, cudaStream_t s) {
+  QX_PARAMS_SWITCH(h, (k_quadx_aviary_step<MODE, V::inject, TILED, PS, V::contact, typename V::world><<<grid_for(h->n), kBlock, 0, s>>>(
+                          ps, h->rng, world_table(v), v.pose(), v.bits(), h->buf.state, h->buf.istate, qx_rows(h), h->buf.setpoint, h->d_modes,
+                          noise, n_steps, seq, h->n)));
+}
+
 int qx_aviary_step(PfbContext* h, int n_steps, const float* noise, cudaStream_t s) {
   const int mode = h->mode;
   const uint32_t seq = (uint32_t)h->aviary_seq++;
-  const int g = grid_for(h->n);
-  const bool contact = aviary_contact_response(h);
-  if (const StaticBodies* sb = step_statics(h)) {  // Aviary handles only, so always warp-tiled
-#define AVS_ARGS ps, h->rng, sb->world, sb->d_pose, sb->d_bits, h->buf.state, qx_rows(h), h->buf.setpoint, h->d_modes, noise, n_steps, seq, h->n
-#define AVS_LAUNCH(M, INJ, CT) QX_PARAMS_SWITCH(h, (k_quadx_aviary_step_static<M, INJ, PS, CT><<<g, kBlock, 0, s>>>(AVS_ARGS)))
+  return aviary_step_launch(h, noise, [&](auto v) {
+    using V = decltype(v);
+    // per-drone modes, static bodies and the contact response exist on Aviary handles only, which are warp-tiled
     if (mode == kModePerDrone) {
-      if (contact) { if (noise) { AVS_LAUNCH(kStaticPerDrone, true, true); } else { AVS_LAUNCH(kStaticPerDrone, false, true); } }
-      else { if (noise) { AVS_LAUNCH(kStaticPerDrone, true, false); } else { AVS_LAUNCH(kStaticPerDrone, false, false); } }
-    } else if (contact) {
-      if (noise) { PFB_MODE_SWITCH(mode, AVS_LAUNCH(MODE, true, true)); } else { PFB_MODE_SWITCH(mode, AVS_LAUNCH(MODE, false, true)); }
+      qx_launch_step<kModePerDrone, true>(h, v, n_steps, noise, seq, s);
+    } else if constexpr (V::contact || V::world::kOn) {
+      PFB_MODE_SWITCH(mode, (qx_launch_step<MODE, true>(h, v, n_steps, noise, seq, s)));
+    } else if (qx_tiled(h)) {
+      PFB_MODE_SWITCH(mode, (qx_launch_step<MODE, true>(h, v, n_steps, noise, seq, s)));
     } else {
-      if (noise) { PFB_MODE_SWITCH(mode, AVS_LAUNCH(MODE, true, false)); } else { PFB_MODE_SWITCH(mode, AVS_LAUNCH(MODE, false, false)); }
+      PFB_MODE_SWITCH(mode, (qx_launch_step<MODE, false>(h, v, n_steps, noise, seq, s)));
     }
-#undef AVS_LAUNCH
-#undef AVS_ARGS
-    LAUNCH_CHECK(h);
     return 0;
-  }
-  if (mode == kModePerDrone) {  // pfb_set_modes: Aviary handles only, so always warp-tiled
-#define AVM_ARGS ps, h->rng, h->buf.state, qx_rows(h), h->buf.setpoint, h->d_modes, noise, n_steps, seq, h->n
-    if (contact) {
-      if (noise) { QX_PARAMS_SWITCH(h, (k_quadx_aviary_step_modes<true, PS, true><<<g, kBlock, 0, s>>>(AVM_ARGS))); }
-      else { QX_PARAMS_SWITCH(h, (k_quadx_aviary_step_modes<false, PS, true><<<g, kBlock, 0, s>>>(AVM_ARGS))); }
-    } else {
-      if (noise) { QX_PARAMS_SWITCH(h, (k_quadx_aviary_step_modes<true, PS, false><<<g, kBlock, 0, s>>>(AVM_ARGS))); }
-      else { QX_PARAMS_SWITCH(h, (k_quadx_aviary_step_modes<false, PS, false><<<g, kBlock, 0, s>>>(AVM_ARGS))); }
-    }
-#undef AVM_ARGS
-    LAUNCH_CHECK(h);
-    return 0;
-  }
-#define AV_ARGS ps, h->rng, h->buf.state, h->buf.istate, qx_rows(h), h->buf.setpoint, noise, n_steps, seq, h->n
-  if (contact) {  // Aviary handles only, so always warp-tiled
-    if (noise) { QX_PARAMS_SWITCH(h, PFB_MODE_SWITCH(mode, (k_quadx_aviary_step<MODE, true, true, PS, true><<<g, kBlock, 0, s>>>(AV_ARGS)))); }
-    else { QX_PARAMS_SWITCH(h, PFB_MODE_SWITCH(mode, (k_quadx_aviary_step<MODE, false, true, PS, true><<<g, kBlock, 0, s>>>(AV_ARGS)))); }
-  } else if (qx_tiled(h)) {
-    if (noise) { QX_PARAMS_SWITCH(h, PFB_MODE_SWITCH(mode, (k_quadx_aviary_step<MODE, true, true, PS, false><<<g, kBlock, 0, s>>>(AV_ARGS)))); }
-    else { QX_PARAMS_SWITCH(h, PFB_MODE_SWITCH(mode, (k_quadx_aviary_step<MODE, false, true, PS, false><<<g, kBlock, 0, s>>>(AV_ARGS)))); }
-  } else {
-    if (noise) { QX_PARAMS_SWITCH(h, PFB_MODE_SWITCH(mode, (k_quadx_aviary_step<MODE, true, false, PS, false><<<g, kBlock, 0, s>>>(AV_ARGS)))); }
-    else { QX_PARAMS_SWITCH(h, PFB_MODE_SWITCH(mode, (k_quadx_aviary_step<MODE, false, false, PS, false><<<g, kBlock, 0, s>>>(AV_ARGS)))); }
-  }
-#undef AV_ARGS
-  LAUNCH_CHECK(h);
-  return 0;
+  });
 }
 
 int qx_observe(PfbContext* h, cudaStream_t s) {

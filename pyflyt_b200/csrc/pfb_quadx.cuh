@@ -362,9 +362,13 @@ struct StaticWorld {
 };
 // The step bodies take a World: NoStatic (the floor only: the kernels every handle without static bodies launches) or
 // StaticCtx (the floor and the static bodies of drone i's world).  bits: what drone i touched during its current Aviary step,
-// bit 0 the floor, bit 1 + b static body b.
+// bit 0 the floor, bit 1 + b static body b.  A step kernel initialises either as World w{&table, pose, n, i, 0u}.
+struct NoStaticTable {};
 struct NoStatic {
   static constexpr bool kOn = false;
+  const NoStaticTable* w;  // StaticCtx's fields, never read
+  const float* pose;
+  int64_t n, i;
   uint32_t bits;
 };
 struct StaticCtx {

@@ -1,6 +1,6 @@
 // TEST HARNESS — the host simulator (hostsim.cpp) plus the contact RESPONSE of the Aviary steps: the CONTACT = true
-// instantiations that k_quadx_aviary_step, k_quadx_aviary_step_modes, k_fw_aviary_step and k_fw_aviary_step_modes
-// (pfb_quadx.cu, pfb_fixedwing.cu) run on an Aviary handle created with contact_response, over the field-major layout.
+// instantiations that k_quadx_aviary_step and k_fw_aviary_step, in one flight mode or per-drone modes
+// (pfb_quadx.cu, pfb_fixedwing.cu), run on an Aviary handle created with contact_response, over the field-major layout.
 // The rocket needs no new entry point: its parameter block carries the switch (hs_rk_aviary_step_contact sets it).
 #include "hostsim.cpp"
 

@@ -1,5 +1,5 @@
 // TEST HARNESS — the host simulator (hostsim.cpp) plus one flight mode per drone: the glue of k_quadx_set_modes and
-// k_quadx_aviary_step_modes (pfb_quadx.cu) over the field-major layout, through the same PFB_HD dispatch helpers
+// k_quadx_aviary_step<kModePerDrone, ...> (pfb_quadx.cu) over the field-major layout, through the same PFB_HD dispatch helpers
 // (quadx_set_mode_any, quadx_aviary_step_any), so that the per-drone control path also runs on the CPU.
 #include "hostsim.cpp"
 

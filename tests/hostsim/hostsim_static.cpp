@@ -1,6 +1,6 @@
 // TEST HARNESS — the host simulator (hostsim.cpp) plus the static bodies of an Aviary handle (DESIGN.md §4h): the static_surface
 // helper on its own, and the QuadX Aviary step with the static bodies of each drone's world (StaticCtx, the World of
-// k_quadx_aviary_step_static) over the field-major layout.  The world comes in flat arrays in pfb::StaticWorld's layout.
+// the k_quadx_aviary_step<..., StaticCtx> instantiations) over the field-major layout.  The world comes in flat arrays in pfb::StaticWorld's layout.
 #include "hostsim.cpp"
 
 static int make_world(int n, const int* body, const int* kind, const float* at, const float* yaw_cs, const float* half, StaticWorld& w) {
