@@ -380,8 +380,9 @@ int pfb_observe_state(PfbHandle h, void* stream);
  * a cylinder's axis is vertical.  Every drone's world holds its own copy of each body.  A primitive is UNDER drone i when
  * its footprint holds the base's (x, y) and z + R_b >= its top (R_b: the model's contact reach); the contact flag of a body
  * is the drone's flag against the top of each primitive under it, and the contact response (contact_response) runs against
- * the highest surface under the drone (the floor, z = 0, or a top).  Side faces are not solid.  pfb_reset with mask = NULL
- * removes every static body (Aviary.reset calls resetSimulation).                                                        */
+ * the highest surface under the drone (the floor, z = 0, or a top).  This top-face rule is the default: side faces are not
+ * solid unless pfb_set_static_solid turns on the solid rule.  pfb_reset with mask = NULL removes every static body
+ * (Aviary.reset calls resetSimulation).                                                                                  */
 typedef PfbShape PfbStaticShape;
 /* Reads the collision primitives of a URDF (fixed joints; boxes, cylinders, spheres) in its base link frame, scaled by
  * global_scaling, and the origin of the base link's inertial frame in that frame (which may be offset, not rotated).
@@ -401,6 +402,13 @@ int pfb_set_static_pose(PfbHandle h, int body, const double* pos, const double* 
 /* bits[i] (device [N]): what drone i touched during the last pfb_aviary_step, bit 0 the floor, bit 1 + k static body k;
  * zero from the first body added after a full pfb_reset until the next step.                                            */
 int pfb_get_static_contacts(PfbHandle h, uint32_t* bits, void* stream);
+/* solid = 1: every static primitive is a solid on all of its faces, edges and corners (DESIGN.md §4h, "solid static
+ * bodies").  Each candidate point of the drone's collision primitives (8 per box or cylinder) takes the deepest of the floor
+ * and the primitives that hold it, with that face's normal, for the contact response; bit 1 + k is set when a candidate point
+ * lies inside a primitive of body k grown on every face by the contact threshold.  solid = 0 (the default): the top-face rule
+ * above.  A property of the handle: pfb_reset keeps it, and it takes effect at the next pfb_aviary_step.  Aviary handles only;
+ * solid must be 0 or 1.  Nothing is enqueued on `stream`.                                                                */
+int pfb_set_static_solid(PfbHandle h, int solid, void* stream);
 
 /* ---- gymnasium-env surface ----------------------------------------------------------------------- */
 /* env.reset(): begin_reset + end_reset (quadx_base_env.py:149-212): pose reset, set_mode, warm-up

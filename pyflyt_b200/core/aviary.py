@@ -42,7 +42,9 @@ Static bodies: ``loadURDF(fileName, basePosition, baseOrientation, useFixedBase=
 for script compatibility) puts a landing pad, a helipad or a rooftop into every drone's world, as the reference's
 ``aviary.loadURDF`` does; ``set_static_pose`` moves a body in the worlds of a mask of drones, and ``contact_bodies()`` says
 which body each drone touched.  Up to ``MAX_STATIC_BODIES`` bodies of ``MAX_STATIC_SHAPES`` boxes and cylinders in all,
-upright; only their top faces are solid (DESIGN.md §4h).  ``reset()`` removes them, as the reference's ``resetSimulation`` does.
+upright.  By default only their top faces are solid; ``solid_static_bodies=True`` makes every face, edge and corner solid, so
+that walls, pillars and towers stop and flag a drone that flies into them (DESIGN.md §4h).  ``reset()`` removes the bodies, as
+the reference's ``resetSimulation`` does, and keeps ``solid_static_bodies``.
 
 All state is held in caller-visible ``torch`` tensors; the CUDA library (libpyflyt_b200.so) only sees
 raw device pointers.  There is no CPU path.
@@ -111,6 +113,7 @@ class BatchedAviary:
         env_offset: int = 0,
         contact_response: bool = False,
         mixed_control_hz: bool = False,
+        solid_static_bodies: bool = False,
     ):
         """``contact_response``: the floor pushes back (contact impulses + Coulomb friction) instead of only raising
         ``contact_array``.  The reference always responds, since every ``Aviary`` is a PyBullet world; here it is opt-in so
@@ -120,7 +123,12 @@ class BatchedAviary:
         ``mixed_control_hz``: the drones' ``drone_options`` may differ in ``control_hz``, as in the reference's
         tests/test_core.py::test_multi_spawn (DESIGN.md §4e).  An Aviary step is then ``physics_hz / min(control_hz)`` physics
         steps, and each drone runs its controller every ``physics_hz / control_hz`` of them.  Opt-in so that a batch built
-        without it keeps refusing different rates.  Aviary handles only: an env flies one drone at one rate."""
+        without it keeps refusing different rates.  Aviary handles only: an env flies one drone at one rate.
+
+        ``solid_static_bodies``: the static bodies of ``loadURDF`` are solid on all of their faces, edges and corners, as in
+        PyBullet: a drone that flies into a wall or a pillar is flagged in ``contact_bodies()`` and, with ``contact_response``,
+        stopped by it.  Off, only their top faces are (DESIGN.md §4h): the rule of scripts and fixtures written before the
+        option, which it keeps bit for bit.  Aviary handles only: an env handle has no static bodies."""
         start_pos = np.asarray(start_pos, dtype=np.float32)
         start_orn = np.asarray(start_orn, dtype=np.float32)
         # shape checks with the reference's messages (aviary.py:120-131)
@@ -128,6 +136,8 @@ class BatchedAviary:
             raise AviaryInitException(f"start_pos must be shape (n, 3), currently {start_pos.shape}.")
         if start_orn.shape != start_pos.shape:
             raise AviaryInitException(f"start_orn must be same shape as start_pos, currently {start_orn.shape}.")
+        if solid_static_bodies and env_config is not None:
+            raise AviaryInitException("solid_static_bodies is an Aviary-handle option; an env handle (env_config) has no static bodies.")
         if mixed_control_hz and env_config is not None:
             raise AviaryInitException("mixed_control_hz is an Aviary-handle option; an env handle (env_config) flies one drone at one control_hz.")
         kinds = None  # one vehicle kind per drone (a list that holds more than one kind), else None
@@ -209,6 +219,9 @@ class BatchedAviary:
         else:
             _lib.check(L.pfb_create(C.byref(self.model), C.byref(env_config) if env_config is not None else None, self.num_drones, dev_index, self.seed, C.byref(self._h)))
         _lib.check(L.pfb_set_env_offset(self._h, int(env_offset)))
+        if solid_static_bodies:
+            _lib.check(L.pfb_set_static_solid(self._h, 1, None))
+        self._solid_static_bodies = bool(solid_static_bodies)
         n, dev = self.num_drones, self.device
         if kinds is None and len(self.models) > 1:  # drone i flies self.models[model_index[i]]; one table keeps the handle as pfb_create made it
             tables = (PfbModel * len(models))(*models)
@@ -255,6 +268,11 @@ class BatchedAviary:
         self._state_fresh = False
         self.static_bodies: list[str] = []  # the URDF of each static body (loadURDF), by body index
         self.reset()
+
+    @property
+    def solid_static_bodies(self) -> bool:
+        """Whether static bodies are solid on every face (the constructor's ``solid_static_bodies``), not only on their tops."""
+        return self._solid_static_bodies
 
     # ------------------------------------------------------------------ lifecycle
     def __del__(self):
@@ -410,8 +428,8 @@ class BatchedAviary:
         """The reference's ``aviary.loadURDF`` of a fixed-base body (a landing pad, a helipad, a rooftop), placed in every drone's
         world with its base link frame at ``basePosition`` / ``baseOrientation`` (x, y, z, w; None = identity).  Returns the
         body index ``k``: column ``1 + k`` of ``contact_bodies()``.  The body must be boxes and cylinders joined by fixed joints,
-        upright once posed (a yaw only); spheres, meshes, tilted poses and ``useFixedBase=False`` are refused.  Aviary handles
-        only."""
+        upright once posed (a yaw only); spheres, meshes, tilted poses and ``useFixedBase=False`` are refused.  Its top faces
+        are solid, or every face with ``solid_static_bodies=True``.  Aviary handles only."""
         if self.env_config is not None and self.env_config.env_kind != 0:
             raise AviaryInitException("static bodies are for Aviary handles; an env handle (env_config) keeps its own floor and pad.")
         if not useFixedBase:
@@ -472,7 +490,10 @@ class BatchedAviary:
 
     def contact_bodies(self) -> torch.Tensor:
         """(N, 1 + M) bool, M = static bodies loaded: column 0 the floor, column 1 + k static body k, touched during the last
-        ``step()`` — the reference's ``contact_array[drone.Id, body_id]``.  ``contact_array`` is their ``any``."""
+        ``step()`` — the reference's ``contact_array[drone.Id, body_id]``.  ``contact_array`` is their ``any``.  Top-face rule
+        (the default): a body's column is the drone's floor flag against the top of each of its primitives under the base.
+        ``solid_static_bodies=True``: it is set when a corner or rim point of the drone's collision primitives lies inside one
+        of the body's primitives grown by the contact threshold, whichever face it came through."""
         if not self.static_bodies:
             return self.contact_array.reshape(-1, 1)
         bits = torch.empty((self.num_drones,), dtype=torch.int32, device=self.device)

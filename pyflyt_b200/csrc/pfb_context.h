@@ -113,6 +113,8 @@ struct PfbContext {
   const struct HandleOps* ops;  // what the handle's kind runs, set once at creation
   // static bodies of an Aviary handle (pfb_add_static_body, pfb_static.cu); nullptr until the first one is added
   struct StaticBodies* statics;
+  // pfb_set_static_solid: the static bodies are solid on every face (SolidCtx), not top faces only; kept by pfb_reset
+  bool static_solid;
 };
 
 // ---- static bodies (pfb_static.cu; DESIGN.md §4h) ----------------------------------------------------------------------------
@@ -329,8 +331,8 @@ int tail_env_step(PfbContext* h, const float* noise, bool randact, cudaStream_t 
 // ---- host side of the Aviary step (pfb_aviary_step) of every vehicle kind and of the mixed-kind handle ----
 // Each kind passes one generic lambda `launch(AviaryVariant<INJECT, CONTACT, World>{sb})` that launches its step kernel and
 // returns 0 or the result of fail().  INJECT: injected noise; CONTACT: aviary_contact_response(h); World: pfb::StaticCtx with
-// the handle's static bodies `sb` (step_statics), or pfb::NoStatic with sb = nullptr.  The kernel takes world_table(v),
-// v.pose() and v.bits().
+// the handle's static bodies `sb` (step_statics), pfb::SolidCtx with them on a handle with pfb_set_static_solid, or
+// pfb::NoStatic with sb = nullptr.  The kernel takes world_table(v), v.pose() and v.bits().
 template <bool INJECT, bool CONTACT, class World>
 struct AviaryVariant {
   static constexpr bool inject = INJECT, contact = CONTACT;
@@ -345,17 +347,21 @@ template <bool INJECT, bool CONTACT>
 pfb::NoStaticTable world_table(AviaryVariant<INJECT, CONTACT, pfb::NoStatic>) { return {}; }
 template <bool INJECT, bool CONTACT>
 const pfb::StaticWorld& world_table(AviaryVariant<INJECT, CONTACT, pfb::StaticCtx> v) { return v.sb->world; }
+template <bool INJECT, bool CONTACT>
+const pfb::StaticWorld& world_table(AviaryVariant<INJECT, CONTACT, pfb::SolidCtx> v) { return v.sb->world; }
 
 template <bool INJECT, bool CONTACT, class Launch>
-int aviary_step_world(const StaticBodies* sb, Launch& launch) {
-  return sb ? launch(AviaryVariant<INJECT, CONTACT, pfb::StaticCtx>{sb}) : launch(AviaryVariant<INJECT, CONTACT, pfb::NoStatic>{nullptr});
+int aviary_step_world(const StaticBodies* sb, bool solid, Launch& launch) {
+  if (!sb) return launch(AviaryVariant<INJECT, CONTACT, pfb::NoStatic>{nullptr});
+  return solid ? launch(AviaryVariant<INJECT, CONTACT, pfb::SolidCtx>{sb}) : launch(AviaryVariant<INJECT, CONTACT, pfb::StaticCtx>{sb});
 }
 template <class Launch>
 int aviary_step_launch(PfbContext* h, const float* noise, Launch&& launch) {
   const StaticBodies* sb = step_statics(h);
+  const bool solid = h->static_solid;
   int rc;
-  if (aviary_contact_response(h)) rc = noise ? aviary_step_world<true, true>(sb, launch) : aviary_step_world<false, true>(sb, launch);
-  else rc = noise ? aviary_step_world<true, false>(sb, launch) : aviary_step_world<false, false>(sb, launch);
+  if (aviary_contact_response(h)) rc = noise ? aviary_step_world<true, true>(sb, solid, launch) : aviary_step_world<false, true>(sb, solid, launch);
+  else rc = noise ? aviary_step_world<true, false>(sb, solid, launch) : aviary_step_world<false, false>(sb, solid, launch);
   if (rc) return rc;
   LAUNCH_CHECK(h);
   return 0;

@@ -209,7 +209,8 @@ PFB_HD bool ground_contact(const ContactParams& cp, float pz, float r20, float r
 // the drone when its footprint (a disc, or a yawed rectangle) holds (px, py) and pz + reach >= its top, reach = the model's
 // contact reach about its base origin (contact_zmax / ContactParams::zmax).  The surface is the highest of the floor (0) and
 // the tops under the drone; touch(top) is the drone's contact flag against the plane z = top, bit 0 = touch(0), bit 1 + b =
-// touch(top) against any primitive of body b under the drone.  Side faces are not solid.
+// touch(top) against any primitive of body b under the drone.  This is the top-face rule: side faces are not solid here
+// (the solid rule, SolidCtx, is below).
 template <class Touch>
 PFB_HD float static_surface(const StaticWorld& w, const float* pose, int64_t n, int64_t i, float px, float py, float pz, float reach,
                             Touch&& touch, uint32_t& bits) {
@@ -266,16 +267,140 @@ PFB_HD Vec3 contact_point(const QuadXParams& p, int k, float lx, float ly, float
   return Vec3{p.shape_at[k][0] + lx, p.shape_at[k][1] + ly, p.shape_at[k][2] + lz};
 }
 
-// Tag: NoStatic, or StaticCtx on the static-body path, which passes a surface height that varies; its own copy of the solver
-// keeps the floor-only kernels' copy, into which the compiler may fold their constant height 0, as it was.
-template <class Tag = NoStatic, class Shapes>
+PFB_HD float contact_thr(const ContactParams& c, int k) { return c.thr[k]; }
+PFB_HD float contact_thr(const QuadXParams& p, int k) { return p.shape_thr[k]; }
+
+// candidate point j (0..7) of collision primitive sh (kind 0: a box corner; kind 1: a cylinder rim point), in the base frame
+template <class Shapes>
+PFB_HD Vec3 contact_candidate(const Shapes* cp, int sh, int kind, const float* dims, int j) {
+  const float sz = (j & 4) ? 1.0f : -1.0f;
+  float lx, ly, lz;
+  if (kind == 0) {
+    lx = ((j & 1) ? 1.0f : -1.0f) * dims[0]; ly = ((j & 2) ? 1.0f : -1.0f) * dims[1]; lz = sz * dims[2];
+  } else {
+    const int a = j & 3;
+    lx = dims[0] * (a == 0 ? 1.0f : (a == 2 ? -1.0f : 0.0f)); ly = dims[0] * (a == 1 ? 1.0f : (a == 3 ? -1.0f : 0.0f));
+    lz = sz * dims[1];
+  }
+  return contact_point(*cp, sh, lx, ly, lz);
+}
+
+// ---- the solid rule (SolidCtx: pfb_set_static_solid; DESIGN.md §4h) ----------------------------------------------------------
+// Every static primitive is a solid on all of its faces: a box yawed about z, or a vertical cylinder.  A point is tested in the
+// primitive's own frame: centre at `at` of the posed body, yaw = body yaw + primitive yaw.
+struct SolidFrame { float cx, cy, cz, c, s; };
+PFB_HD SolidFrame solid_frame(const StaticWorld& w, const float* pose, int64_t n, int64_t i, int k) {
+  const float* q = pose + (int64_t)kStaticPoseRows * w.body[k] * n + i;
+  const float bx = q[0], by = q[n], bz = q[2 * n], c = q[3 * n], sn = q[4 * n];
+  return SolidFrame{bx + c * w.at[k][0] - sn * w.at[k][1], by + sn * w.at[k][0] + c * w.at[k][1], bz + w.at[k][2],
+                    c * w.cyaw[k] - sn * w.syaw[k], sn * w.cyaw[k] + c * w.syaw[k]};
+}
+PFB_HD Vec3 solid_local(const SolidFrame& f, float x, float y, float z) {
+  const float dx = x - f.cx, dy = y - f.cy;
+  return Vec3{f.c * dx + f.s * dy, f.c * dy - f.s * dx, z - f.cz};
+}
+// world point of base-frame point pb
+PFB_HD Vec3 solid_point(const SolidBase& b, Vec3 pb) {
+  return Vec3{b.px + dot(Vec3{b.r[0], b.r[1], b.r[2]}, pb), b.py + dot(Vec3{b.r[3], b.r[4], b.r[5]}, pb), b.pz + dot(Vec3{b.r[6], b.r[7], b.r[8]}, pb)};
+}
+
+// The cull: bit k set when the base is within `reach` (the model's contact reach, contact_zmax / ContactParams::zmax) of
+// primitive k's bounding box in its own frame (the box itself; the cylinder's square prism), along each of its axes.  reach
+// bounds |candidate point - base| + the contact threshold, so a culled primitive holds no candidate point, even grown.
+PFB_HD uint32_t solid_live(const StaticWorld& w, const float* pose, int64_t n, int64_t i, float px, float py, float pz, float reach) {
+  uint32_t live = 0u;
+#pragma unroll 1
+  for (int k = 0; k < w.n_shapes; ++k) {
+    const Vec3 l = solid_local(solid_frame(w, pose, n, i, k), px, py, pz);
+    if (fabsf(l.x) - w.half[k][0] <= reach && fabsf(l.y) - w.half[k][1] <= reach && fabsf(l.z) - w.half[k][2] <= reach) live |= 1u << k;
+  }
+  return live;
+}
+
+// Penetration of local point l into primitive k: false when l is outside; else the depth of the nearest face and its outward
+// normal in the primitive frame.  Box: the face of least half_a - |l_a|, ties to +z, then +-x, then +-y, then -z.  Cylinder:
+// the least of radial r - rho, top h - l_z and bottom h + l_z, ties to top, then radial, then bottom; the radial normal is
+// +x for rho < 1e-6.
+PFB_HD bool solid_penetration(const StaticWorld& w, int k, Vec3 l, float& depth, Vec3& nl) {
+  const float* h = w.half[k];
+  float d = h[2] - l.z;
+  Vec3 m = Vec3{0.0f, 0.0f, 1.0f};
+  if (w.kind[k] == 0) {
+    if (!(fabsf(l.x) <= h[0] && fabsf(l.y) <= h[1] && fabsf(l.z) <= h[2])) return false;
+    const float dx = h[0] - fabsf(l.x), dy = h[1] - fabsf(l.y);
+    if (dx < d) { d = dx; m = Vec3{l.x >= 0.0f ? 1.0f : -1.0f, 0.0f, 0.0f}; }
+    if (dy < d) { d = dy; m = Vec3{0.0f, l.y >= 0.0f ? 1.0f : -1.0f, 0.0f}; }
+  } else {
+    const float rho = sqrtf(l.x * l.x + l.y * l.y);
+    if (!(rho <= h[0] && fabsf(l.z) <= h[2])) return false;
+    const float dr = h[0] - rho;
+    if (dr < d) { d = dr; m = rho < 1e-6f ? Vec3{1.0f, 0.0f, 0.0f} : Vec3{l.x / rho, l.y / rho, 0.0f}; }
+  }
+  const float db = h[2] + l.z;
+  if (db < d) { d = db; m = Vec3{0.0f, 0.0f, -1.0f}; }
+  depth = d;
+  nl = m;
+  return true;
+}
+
+// The contact of world point (x, y, z): the deepest of the floor (depth -z, normal +z) and every primitive of `live` that holds
+// the point; ties go to the floor, then to the primitive first in table order.  The normal is in the world frame.
+struct SolidContact { float depth; Vec3 n; };
+PFB_HD SolidContact solid_point_contact(const StaticWorld& w, const float* pose, int64_t n, int64_t i, uint32_t live, float x, float y, float z) {
+  SolidContact r{-z, Vec3{0.0f, 0.0f, 1.0f}};
+#pragma unroll 1
+  for (int k = 0; k < w.n_shapes; ++k) {
+    if (!((live >> k) & 1u)) continue;
+    const SolidFrame f = solid_frame(w, pose, n, i, k);
+    float d;
+    Vec3 m;
+    if (!solid_penetration(w, k, solid_local(f, x, y, z), d, m) || !(d > r.depth)) continue;
+    r.depth = d;
+    r.n = Vec3{f.c * m.x - f.s * m.y, f.s * m.x + f.c * m.y, m.z};
+  }
+  return r;
+}
+
+// Bits 1 + b of the solid rule: a candidate point of the drone lies inside a primitive of body b grown on every face by the
+// contact threshold of that point's drone primitive (the floor's bit 0 is the caller's).  Only the primitives of `live`.
+// Out of line and by value: it runs only near a body, and inlined it would hold its state in registers of the hot loop.
+template <class Shapes>
 #if defined(__CUDACC__)
 static __host__ __device__ __noinline__
 #else
 inline
 #endif
-ContactVel solve_contacts(const Shapes* cp, float pz, float top, Vec3 n /* world z in the body frame = third row of R */, Vec3 vb,
-                          Vec3 w, float M, Vec3 c, float Ixx, float Ixy, float Ixz, float Iyy, float Iyz, float Izz, float dt) {
+uint32_t solid_bits(const StaticWorld* wp, const float* pose, int64_t n, int64_t i, uint32_t live, const Shapes* cp, SolidBase b) {
+  const StaticWorld& w = *wp;
+  uint32_t bits = 0u;
+#pragma unroll 1
+  for (int sh = 0; sh < contact_n_shapes(*cp); ++sh) {
+    const int kind = contact_kind(*cp, sh);
+    if (kind > 1) continue;  // boxes and cylinders, as the solver
+    const float* dims = contact_dims(*cp, sh);
+    const float t = contact_thr(*cp, sh);
+#pragma unroll 1
+    for (int j = 0; j < 8; ++j) {
+      const Vec3 pw = solid_point(b, contact_candidate(cp, sh, kind, dims, j));
+#pragma unroll 1
+      for (int k = 0; k < w.n_shapes; ++k) {
+        if (!((live >> k) & 1u)) continue;
+        const Vec3 l = solid_local(solid_frame(w, pose, n, i, k), pw.x, pw.y, pw.z);
+        const float* h = w.half[k];
+        const bool in = w.kind[k] == 0 ? (fabsf(l.x) <= h[0] + t && fabsf(l.y) <= h[1] + t)
+                                        : sqrtf(l.x * l.x + l.y * l.y) <= h[0] + t;
+        if (in && fabsf(l.z) <= h[2] + t) bits |= 2u << w.body[k];
+      }
+    }
+  }
+  return bits;
+}
+
+// kContactIterations sweeps of the sequential impulse over the candidate points; at(pb, n) returns the depth of base-frame
+// point pb and sets its contact normal n (body frame)
+template <class Shapes, class At>
+PFB_HD ContactVel contact_sweeps(const Shapes* cp, At&& at, Vec3 vb, Vec3 w, float M, Vec3 c, float Ixx, float Ixy, float Ixz, float Iyy,
+                                 float Iyz, float Izz, float dt) {
   // inverse of the symmetric central inertia (cofactors)
   const float c00 = Iyy * Izz - Iyz * Iyz, c01 = Ixz * Iyz - Ixy * Izz, c02 = Ixy * Iyz - Ixz * Iyy;
   const float c11 = Ixx * Izz - Ixz * Ixz, c12 = Ixy * Ixz - Ixx * Iyz, c22 = Ixx * Iyy - Ixy * Ixy;
@@ -289,17 +414,9 @@ ContactVel solve_contacts(const Shapes* cp, float pz, float top, Vec3 n /* world
       if (kind > 1) continue;  // boxes and cylinders
       const float* dims = contact_dims(*cp, sh);
       for (int j = 0; j < 8; ++j) {
-        const float sz = (j & 4) ? 1.0f : -1.0f;
-        float lx, ly, lz;
-        if (kind == 0) {
-          lx = ((j & 1) ? 1.0f : -1.0f) * dims[0]; ly = ((j & 2) ? 1.0f : -1.0f) * dims[1]; lz = sz * dims[2];
-        } else {
-          const int a = j & 3;
-          lx = dims[0] * (a == 0 ? 1.0f : (a == 2 ? -1.0f : 0.0f)); ly = dims[0] * (a == 1 ? 1.0f : (a == 3 ? -1.0f : 0.0f));
-          lz = sz * dims[1];
-        }
-        const Vec3 pb = contact_point(*cp, sh, lx, ly, lz);
-        const float depth = top - (pz + dot(n, pb));
+        const Vec3 pb = contact_candidate(cp, sh, kind, dims, j);
+        Vec3 n;
+        const float depth = at(pb, n);
         if (depth <= 0.0f) continue;
         touched = 1;
         const Vec3 r = pb - c;
@@ -329,17 +446,48 @@ ContactVel solve_contacts(const Shapes* cp, float pz, float top, Vec3 n /* world
   return ContactVel{vo.x, vo.y, vo.z, w.x, w.y, w.z, touched};
 }
 
+// Tag: NoStatic, or StaticCtx on the static-body path, which passes a surface height that varies; its own copy of the solver
+// keeps the floor-only kernels' copy, into which the compiler may fold their constant height 0, as it was.
+template <class Tag = NoStatic, class Shapes>
+#if defined(__CUDACC__)
+static __host__ __device__ __noinline__
+#else
+inline
+#endif
+ContactVel solve_contacts(const Shapes* cp, float pz, float top, Vec3 n /* world z in the body frame = third row of R */, Vec3 vb,
+                          Vec3 w, float M, Vec3 c, float Ixx, float Ixy, float Ixz, float Iyy, float Iyz, float Izz, float dt) {
+  return contact_sweeps(cp, [&](Vec3 pb, Vec3& pn) { pn = n; return top - (pz + dot(n, pb)); }, vb, w, M, c, Ixx, Ixy, Ixz, Iyy, Iyz, Izz, dt);
+}
+
+// The solver of the solid rule: each candidate point takes its contact from solid_point_contact (the floor and the solids of
+// `live`), its normal rotated into the body frame.  b: the pose at the start of the substep.
+template <class Shapes>
+#if defined(__CUDACC__)
+static __host__ __device__ __noinline__
+#else
+inline
+#endif
+ContactVel solve_contacts_solid(const Shapes* cp, SolidCtx world, uint32_t live, SolidBase b, Vec3 vb, Vec3 w, float M, Vec3 c, float Ixx,
+                                float Ixy, float Ixz, float Iyy, float Iyz, float Izz, float dt) {
+  return contact_sweeps(cp, [&](Vec3 pb, Vec3& pn) {
+    const Vec3 pw = solid_point(b, pb);
+    const SolidContact k = solid_point_contact(*world.w, world.pose, world.n, world.i, live, pw.x, pw.y, pw.z);
+    pn = Vec3{b.r[0] * k.n.x + b.r[3] * k.n.y + b.r[6] * k.n.z, b.r[1] * k.n.x + b.r[4] * k.n.y + b.r[7] * k.n.z,
+              b.r[2] * k.n.x + b.r[5] * k.n.y + b.r[8] * k.n.z};
+    return k.depth;
+  }, vb, w, M, c, Ixx, Ixy, Ixz, Iyy, Iyz, Izz, dt);
+}
+
 // Contact impulses on the predicted velocities of `s` (world linear velocity, body angular velocity), before its pose is
-// integrated: the solve runs in the body frame of the pose at the START of the substep (rotation s.R, base altitude pz0).
-// M, c, I..: mass, COM offset and inertia about the COM (base frame).
-template <class Tag, class Shapes, class Regs>
-PFB_HD void apply_contact_impulses(const Shapes* cp, Regs& s, float pz0, float top, float M, Vec3 c, float Ixx, float Ixy, float Ixz,
-                                   float Iyy, float Iyz, float Izz, float dt) {
+// integrated: the solve runs in the body frame of the pose at the START of the substep (rotation s.R).  solve(n, vb, w) returns
+// the solved velocities in the body frame; n = world z in the body frame, vb = the body-frame linear velocity.
+template <class Regs, class Solve>
+PFB_HD void contact_impulses_with(Regs& s, Solve&& solve) {
   const float m00 = (float)s.R.m00, m01 = (float)s.R.m01, m02 = (float)s.R.m02, m10 = (float)s.R.m10, m11 = (float)s.R.m11,
               m12 = (float)s.R.m12, m20 = (float)s.R.m20, m21 = (float)s.R.m21, m22 = (float)s.R.m22;
   const float vwx = (float)s.vx, vwy = (float)s.vy, vwz = (float)s.vz;
   const Vec3 vbn = Vec3{m00 * vwx + m10 * vwy + m20 * vwz, m01 * vwx + m11 * vwy + m21 * vwz, m02 * vwx + m12 * vwy + m22 * vwz};
-  const ContactVel cv = solve_contacts<Tag>(cp, pz0, top, Vec3{m20, m21, m22}, vbn, Vec3{s.wx, s.wy, s.wz}, M, c, Ixx, Ixy, Ixz, Iyy, Iyz, Izz, dt);
+  const ContactVel cv = solve(Vec3{m20, m21, m22}, vbn, Vec3{s.wx, s.wy, s.wz});
   if (cv.touched) {
     s.vx = (vreal)(m00 * cv.vx + m01 * cv.vy + m02 * cv.vz);
     s.vy = (vreal)(m10 * cv.vx + m11 * cv.vy + m12 * cv.vz);
@@ -347,6 +495,27 @@ PFB_HD void apply_contact_impulses(const Shapes* cp, Regs& s, float pz0, float t
     s.wx = cv.wx; s.wy = cv.wy; s.wz = cv.wz;
   }
 }
+// against the plane z = top, base altitude pz0 at the start of the substep.  M, c, I..: mass, COM offset and inertia about the
+// COM (base frame).
+template <class Tag, class Shapes, class Regs>
+PFB_HD void apply_contact_impulses(const Shapes* cp, Regs& s, float pz0, float top, float M, Vec3 c, float Ixx, float Ixy, float Ixz,
+                                   float Iyy, float Iyz, float Izz, float dt) {
+  contact_impulses_with(s, [&](Vec3 n, Vec3 vbn, Vec3 w) { return solve_contacts<Tag>(cp, pz0, top, n, vbn, w, M, c, Ixx, Ixy, Ixz, Iyy, Iyz, Izz, dt); });
+}
+// against the floor and the solids of `live` (the solid rule), from the pose of `s`, which is still that of the start of the
+// substep
+template <class Shapes, class Regs>
+PFB_HD void apply_solid_impulses(const Shapes* cp, Regs& s, const SolidCtx& world, uint32_t live, float M, Vec3 c, float Ixx, float Ixy, float Ixz,
+                                 float Iyy, float Iyz, float Izz, float dt) {
+  const SolidBase b = solid_base(s);
+  contact_impulses_with(s, [&](Vec3, Vec3 vbn, Vec3 w) { return solve_contacts_solid(cp, world, live, b, vbn, w, M, c, Ixx, Ixy, Ixz, Iyy, Iyz, Izz, dt); });
+}
+
+// what the solid rule's response runs against (rigid_step's `top` with Tag = SolidCtx)
+struct SolidSurface {
+  const SolidCtx* world;
+  uint32_t live;
+};
 
 // Bullet free-body step for a composite body with COM offset c and full inertia I_O (SURVEY §A.3):
 //   F = M (a_O + wdot x c + w x (w x c)),   T_O = I_O wdot + w x I_O w + M c x a_O
@@ -354,10 +523,11 @@ PFB_HD void apply_contact_impulses(const Shapes* cp, Regs& s, float pz0, float t
 // same semi-implicit Euler + body-frame exp-map as the quad.
 // CONTACT: contact impulses over `cp` on the predicted velocities when `touching` (the substep's contact flag), before the
 // pose is integrated.
-// Tag: as solve_contacts (`top`: the surface height of the response).
-template <bool CONTACT = false, class Tag = NoStatic, typename Regs>
+// Tag: as solve_contacts (`top`: the surface height of the response), or SolidCtx (`top`: a SolidSurface, the solids the
+// response runs against).
+template <bool CONTACT = false, class Tag = NoStatic, typename Regs, class Surf = float>
 PFB_HD void rigid_step(const RigidParams& rb, float gravity, float dt_f, float vmax_f, Regs& s, Vec3 F, Vec3 T,
-                       const ContactParams* cp = nullptr, bool touching = false, float top = 0.0f) {
+                       const ContactParams* cp = nullptr, bool touching = false, Surf top = Surf()) {
   typedef decltype(s.R.m00) RT;  // the body's rotation-matrix precision (fwreal for aircraft, rreal for the rocket)
   const Rot<RT>& R = s.R;
   const float r20 = (float)R.m20, r21 = (float)R.m21, r22 = (float)R.m22;
@@ -412,8 +582,12 @@ PFB_HD void rigid_step(const RigidParams& rb, float gravity, float dt_f, float v
       const float M = rb.mass, iM = 1.0f / M;
       const Vec3 c = Vec3{rb.mc[0] * iM, rb.mc[1] * iM, rb.mc[2] * iM};
       const float c2 = dot(c, c);
-      apply_contact_impulses<Tag>(cp, s, (float)s.pz, top, M, c, rb.I[0] - M * (c2 - c.x * c.x), rb.I[1] + M * c.x * c.y, rb.I[2] + M * c.x * c.z,
+      if constexpr (Tag::kSolid)
+        apply_solid_impulses(cp, s, *top.world, top.live, M, c, rb.I[0] - M * (c2 - c.x * c.x), rb.I[1] + M * c.x * c.y, rb.I[2] + M * c.x * c.z,
                              rb.I[4] - M * (c2 - c.y * c.y), rb.I[5] + M * c.y * c.z, rb.I[8] - M * (c2 - c.z * c.z), dt_f);
+      else
+        apply_contact_impulses<Tag>(cp, s, (float)s.pz, top, M, c, rb.I[0] - M * (c2 - c.x * c.x), rb.I[1] + M * c.x * c.y, rb.I[2] + M * c.x * c.z,
+                               rb.I[4] - M * (c2 - c.y * c.y), rb.I[5] + M * c.y * c.z, rb.I[8] - M * (c2 - c.z * c.z), dt_f);
     }
     s.px += (xreal)(s.vx * dt);
     s.py += (xreal)(s.vy * dt);
@@ -530,7 +704,7 @@ PFB_HD void fixedwing_command(const FixedwingRegs& s, float* cmd) {
 // at the batch sizes these vehicles run at (16 384 envs) instruction-level parallelism is the only latency hiding there is:
 // FULL removes the tests at compile time, the surfaces land in ONE basic block and their chains interleave.
 // CONTACT = the ground pushes back (Aviary handles with contact_response): see rigid_step.
-// World: NoStatic or StaticCtx, as in quadx_substep.
+// World: NoStatic, StaticCtx or SolidCtx, as in quadx_substep.
 template <bool FULL = false, bool CONTACT = false, class World = NoStatic>
 PFB_HD void fixedwing_substep(const FixedwingParams& p, FixedwingRegs& s, const float* cmd, float xi, World* world = nullptr) {
   Vec3 F = Vec3{0.f, 0.f, 0.f}, T = Vec3{0.f, 0.f, 0.f};
@@ -556,7 +730,16 @@ PFB_HD void fixedwing_substep(const FixedwingParams& p, FixedwingRegs& s, const 
     F = F + Fm;
     T = T + cross(Vec3{p.motor_r[0], p.motor_r[1], p.motor_r[2]}, Fm) + Vec3{p.torque_k * a, 0.0f, 0.0f};
   }
-  if constexpr (World::kOn) {
+  if constexpr (World::kSolid) {
+    const float pz = (float)s.pz;
+    const uint32_t live = solid_live(*world->w, world->pose, world->n, world->i, (float)s.px, (float)s.py, pz, p.contact.zmax);
+    uint32_t b = ground_contact(p.contact, pz, (float)s.R.m20, (float)s.R.m21, (float)s.R.m22) ? 1u : 0u;
+    if (live) b |= solid_bits(world->w, world->pose, world->n, world->i, live, &p.contact, solid_base(s));
+    world->bits |= b;
+    const bool c = b != 0u;
+    s.flags = (s.flags & ~(uint32_t)FLAG_CONTACT_PREV) | (c ? (FLAG_CONTACT_PREV | FLAG_CONTACT_ARRAY) : 0u);
+    rigid_step<CONTACT, World>(p.rb, p.gravity, p.dt, p.vmax, s, F, T, &p.contact, c, SolidSurface{world, live});
+  } else if constexpr (World::kOn) {
     const float pz = (float)s.pz, r20 = (float)s.R.m20, r21 = (float)s.R.m21, r22 = (float)s.R.m22;
     uint32_t b;
     const float top = static_surface(*world->w, world->pose, world->n, world->i, (float)s.px, (float)s.py, pz, p.contact.zmax,

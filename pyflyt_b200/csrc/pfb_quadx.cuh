@@ -360,19 +360,27 @@ struct StaticWorld {
   float cyaw[kMaxStaticShapes], syaw[kMaxStaticShapes];  // yaw of the primitive in that frame
   float half[kMaxStaticShapes][3];    // box: half extents; cylinder: radius, radius, half length
 };
-// The step bodies take a World: NoStatic (the floor only: the kernels every handle without static bodies launches) or
-// StaticCtx (the floor and the static bodies of drone i's world).  bits: what drone i touched during its current Aviary step,
-// bit 0 the floor, bit 1 + b static body b.  A step kernel initialises either as World w{&table, pose, n, i, 0u}.
+// The step bodies take a World: NoStatic (the floor only: the kernels every handle without static bodies launches),
+// StaticCtx (the floor and the top faces of the static bodies of drone i's world) or SolidCtx (the floor and the static
+// bodies of drone i's world as solids: pfb_set_static_solid).  bits: what drone i touched during its current Aviary step,
+// bit 0 the floor, bit 1 + b static body b.  A step kernel initialises each as World w{&table, pose, n, i, 0u}.
 struct NoStaticTable {};
 struct NoStatic {
-  static constexpr bool kOn = false;
+  static constexpr bool kOn = false, kSolid = false;
   const NoStaticTable* w;  // StaticCtx's fields, never read
   const float* pose;
   int64_t n, i;
   uint32_t bits;
 };
 struct StaticCtx {
-  static constexpr bool kOn = true;
+  static constexpr bool kOn = true, kSolid = false;
+  const StaticWorld* w;
+  const float* pose;
+  int64_t n, i;
+  uint32_t bits;
+};
+struct SolidCtx {
+  static constexpr bool kOn = true, kSolid = true;
   const StaticWorld* w;
   const float* pose;
   int64_t n, i;
@@ -382,6 +390,26 @@ struct StaticCtx {
 template <class Touch>
 PFB_HD float static_surface(const StaticWorld& w, const float* pose, int64_t n, int64_t i, float px, float py, float pz, float reach,
                             Touch&& touch, uint32_t& bits);
+// pfb_fixedwing.cuh: the solid rule (SolidCtx) — the primitives within reach of the base, and the contact bits of the drone's
+// candidate points against them
+struct SolidBase { float px, py, pz, r[9]; };  // base position and body -> world rotation (row-major) at the start of the substep
+PFB_HD uint32_t solid_live(const StaticWorld& w, const float* pose, int64_t n, int64_t i, float px, float py, float pz, float reach);
+template <class Shapes>
+#if defined(__CUDACC__)
+static __host__ __device__ __noinline__
+#else
+inline
+#endif
+uint32_t solid_bits(const StaticWorld* w, const float* pose, int64_t n, int64_t i, uint32_t live, const Shapes* cp, SolidBase b);
+// the contact response against the floor and the solids of `live` (pfb_fixedwing.cuh)
+template <class Shapes, class Regs>
+PFB_HD void apply_solid_impulses(const Shapes* cp, Regs& s, const SolidCtx& world, uint32_t live, float M, Vec3 c, float Ixx, float Ixy, float Ixz,
+                                 float Iyy, float Iyz, float Izz, float dt);
+template <class Regs>
+PFB_HD SolidBase solid_base(const Regs& s) {
+  return SolidBase{(float)s.px, (float)s.py, (float)s.pz,
+                   {(float)s.R.m00, (float)s.R.m01, (float)s.R.m02, (float)s.R.m10, (float)s.R.m11, (float)s.R.m12, (float)s.R.m20, (float)s.R.m21, (float)s.R.m22}};
+}
 
 // Bullet clamps the WORLD angular-velocity coordinates to +-vmax; that can only bite when a body rate
 // exceeds vmax/sqrt(3), so the rotation to the world frame and back lives out of line (cold).  Everything
@@ -463,7 +491,14 @@ PFB_HD void quadx_substep(const QuadXParams& p, QuadXRegs& s, float xi, World* w
   //      integration inside stepSimulation); aviary.py:523-525
   bool c;
   float top = 0.0f;  // surface height under the drone
-  if constexpr (World::kOn) {
+  [[maybe_unused]] uint32_t live = 0u;  // SolidCtx: the primitives within reach of the base
+  if constexpr (World::kSolid) {
+    live = solid_live(*world->w, world->pose, world->n, world->i, (float)s.px, (float)s.py, (float)s.pz, p.contact_zmax);
+    uint32_t b = quadx_ground_contact(p, s) ? 1u : 0u;
+    if (live) b |= solid_bits(world->w, world->pose, world->n, world->i, live, &p, solid_base(s));
+    world->bits |= b;
+    c = b != 0u;
+  } else if constexpr (World::kOn) {
     uint32_t b;
     top = static_surface(*world->w, world->pose, world->n, world->i, (float)s.px, (float)s.py, (float)s.pz, p.contact_zmax,
                          [&](float t) { return quadx_ground_contact(p, s, t); }, b);
@@ -508,7 +543,11 @@ PFB_HD void quadx_substep(const QuadXParams& p, QuadXRegs& s, float xi, World* w
     s.wx = w.x; s.wy = w.y; s.wz = w.z;
   }
   if (CONTACT) {
-    if (c) apply_contact_impulses<World>(&p, s, (float)s.pz, top, 1.0f / p.inv_mass, Vec3{0.f, 0.f, 0.f}, p.Ixx, 0.0f, 0.0f, p.Iyy, 0.0f, p.Izz, p.dt);
+    if constexpr (World::kSolid) {
+      if (c) apply_solid_impulses(&p, s, *world, live, 1.0f / p.inv_mass, Vec3{0.f, 0.f, 0.f}, p.Ixx, 0.0f, 0.0f, p.Iyy, 0.0f, p.Izz, p.dt);
+    } else {
+      if (c) apply_contact_impulses<World>(&p, s, (float)s.pz, top, 1.0f / p.inv_mass, Vec3{0.f, 0.f, 0.f}, p.Ixx, 0.0f, 0.0f, p.Iyy, 0.0f, p.Izz, p.dt);
+    }
     s.px += (xreal)(s.vx * dt);
     s.py += (xreal)(s.vy * dt);
     s.pz += (xreal)(s.vz * dt);

@@ -90,7 +90,7 @@ PFB_HD void rocket_command(const RocketRegs& s, float* cmd) {
 }
 
 // one physics substep: update_physics (rocket.py:280-298) + stepSimulation + update_state
-// World: NoStatic or StaticCtx (Aviary handles, with_pad = false), as in quadx_substep.
+// World: NoStatic, StaticCtx or SolidCtx (Aviary handles, with_pad = false), as in quadx_substep.
 template <class World = NoStatic>
 PFB_HD void rocket_substep(const RocketParams& p, RocketRegs& s, const float* cmd, float xi, bool with_pad, World* world = nullptr) {
   Vec3 F = Vec3{0.f, 0.f, 0.f}, T = Vec3{0.f, 0.f, 0.f};
@@ -140,7 +140,16 @@ PFB_HD void rocket_substep(const RocketParams& p, RocketRegs& s, const float* cm
   bool touching = false, over_pad = false;
   float top = 0.0f;  // static bodies: the surface height under the drone
   const float pz0 = (float)s.pz;  // altitude at the START of the substep (the contact solver's pose)
-  if constexpr (World::kOn) {
+  [[maybe_unused]] uint32_t live = 0u;  // SolidCtx: the primitives within reach of the base
+  if constexpr (World::kSolid) {
+    live = solid_live(*world->w, world->pose, world->n, world->i, (float)s.px, (float)s.py, pz0, p.contact.zmax);
+    uint32_t b = ground_contact(p.contact, pz0, (float)s.R.m20, (float)s.R.m21, (float)s.R.m22, 0.0f) ? 1u : 0u;
+    if (live) b |= solid_bits(world->w, world->pose, world->n, world->i, live, &p.contact, solid_base(s));
+    world->bits |= b;
+    touching = b != 0u;
+    s.flags = (s.flags & ~(uint32_t)FLAG_CONTACT_PREV) | (touching ? (FLAG_CONTACT_PREV | FLAG_CONTACT_ARRAY) : 0u) |
+              ((b & 1u) ? FLAG_CONTACT_GROUND : 0u);
+  } else if constexpr (World::kOn) {
     const float pz = (float)s.pz, r20 = (float)s.R.m20, r21 = (float)s.R.m21, r22 = (float)s.R.m22;
     uint32_t b;
     top = static_surface(*world->w, world->pose, world->n, world->i, (float)s.px, (float)s.py, pz, p.contact.zmax,
@@ -205,7 +214,11 @@ PFB_HD void rocket_substep(const RocketParams& p, RocketRegs& s, const float* cm
     Vec3 wc = quadx_clamp_world_rates(p.vmax, Rf, Vec3{s.wx, s.wy, s.wz});
     s.wx = wc.x; s.wy = wc.y; s.wz = wc.z;
   }
-  if (p.contact_response && touching)  // contact impulses on the predicted velocities, before the pose is integrated (cold path)
+  if constexpr (World::kSolid) {
+    if (p.contact_response && touching)
+      apply_solid_impulses(&p.contact, s, *world, live, M, c, Ixx - M * (c2 - c.x * c.x), Ixy + M * c.x * c.y, Ixz + M * c.x * c.z,
+                           Iyy - M * (c2 - c.y * c.y), Iyz + M * c.y * c.z, Izz - M * (c2 - c.z * c.z), p.dt);
+  } else if (p.contact_response && touching)  // contact impulses on the predicted velocities, before the pose is integrated (cold path)
     apply_contact_impulses<World>(&p.contact, s, pz0, World::kOn ? top : (over_pad ? kPadTop : 0.0f), M, c, Ixx - M * (c2 - c.x * c.x), Ixy + M * c.x * c.y, Ixz + M * c.x * c.z,
                            Iyy - M * (c2 - c.y * c.y), Iyz + M * c.y * c.z, Izz - M * (c2 - c.z * c.z), p.dt);
   s.px += (xreal)(s.vx * dt); s.py += (xreal)(s.vy * dt); s.pz += (xreal)(s.vz * dt);

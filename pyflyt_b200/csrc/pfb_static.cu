@@ -184,3 +184,10 @@ extern "C" int pfb_get_static_contacts(PfbHandle h, uint32_t* bits, void* stream
   CUDA_OK(cudaMemcpyAsync(bits, h->statics->d_bits, (size_t)h->n * sizeof(uint32_t), cudaMemcpyDeviceToDevice, (cudaStream_t)stream));
   return 0;
 }
+
+extern "C" int pfb_set_static_solid(PfbHandle h, int solid, void*) {
+  if (require_aviary_statics(h, "pfb_set_static_solid")) return -1;
+  if (solid != 0 && solid != 1) return fail("pfb_set_static_solid: solid must be 0 (top faces) or 1 (every face), got %d", solid);
+  h->static_solid = solid == 1;
+  return 0;
+}

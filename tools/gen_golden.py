@@ -1411,6 +1411,189 @@ def static_fixtures():
                    {0: {i: [starts[i][0], starts[i][1], 0.0, 0.3] for i in range(3)}}, 600, seed=406, poses=poses)
 
 
+# ---- solid static bodies (DESIGN.md §4h, "solid static bodies") --------------------------------------------------------
+def _solid_prims(s):
+    """(kind, centre, world rotation, half sizes) of every collision primitive of the fixed-base body s; a cylinder's half sizes
+    are (radius, radius, half length)"""
+    Rs = s.R()
+    out = []
+    for lk in s.links:
+        for kind, dims, cr, cR in lk.shapes:
+            if kind not in ("box", "cylinder"):
+                raise ValueError(f"static body {s.path}: a {kind} (boxes and cylinders only)")
+            half = 0.5 * np.asarray(dims, dtype=np.float64) if kind == "box" else np.array([dims[0], dims[0], 0.5 * dims[1]])
+            out.append((kind, s.pos + Rs @ cr, Rs @ cR, half))
+    return out
+
+
+def _solid_points(b):
+    """the candidate points of free body b (8 per box or cylinder, in the solver's order) in the world frame, each with the
+    contact threshold of its primitive"""
+    Rb = b.R()
+    out = []
+    for lk in b.links:
+        for kind, dims, cr, cR in lk.shapes:
+            if kind == "box":
+                h = 0.5 * np.asarray(dims)
+                loc = [(sx * h[0], sy * h[1], sz * h[2]) for sz in (-1, 1) for sy in (-1, 1) for sx in (-1, 1)]
+                disc = float(np.linalg.norm(h))
+            elif kind == "cylinder":
+                rad, half = dims[0], 0.5 * dims[1]
+                loc = [(rad * cx, rad * cy, sz * half) for sz in (-1, 1) for cx, cy in ((1, 0), (0, 1), (-1, 0), (0, -1))]
+                disc = float(np.hypot(rad, half))
+            else:
+                continue
+            for q in loc:
+                out.append((b.pos + Rb @ (cr + cR @ np.asarray(q, dtype=np.float64)), 0.02 * disc))
+    return out
+
+
+def _solid_penetration(kind, centre, Rw, half, p):
+    """None outside; else (depth, world normal) of the nearest face: box ties +z, +-x, +-y, -z; cylinder ties top, radial,
+    bottom, the radial normal +x of the primitive on its axis"""
+    l = Rw.T @ (p - centre)
+    if kind == "box":
+        if not all(abs(l[a]) <= half[a] for a in range(3)):
+            return None
+        faces = [(half[2] - l[2], (0.0, 0.0, 1.0)), (half[0] - abs(l[0]), (1.0 if l[0] >= 0 else -1.0, 0.0, 0.0)),
+                 (half[1] - abs(l[1]), (0.0, 1.0 if l[1] >= 0 else -1.0, 0.0)), (half[2] + l[2], (0.0, 0.0, -1.0))]
+    else:
+        rho = float(np.hypot(l[0], l[1]))
+        if not (rho <= half[0] and abs(l[2]) <= half[2]):
+            return None
+        radial = (1.0, 0.0, 0.0) if rho < 1e-6 else (l[0] / rho, l[1] / rho, 0.0)
+        faces = [(half[2] - l[2], (0.0, 0.0, 1.0)), (half[0] - rho, radial), (half[2] + l[2], (0.0, 0.0, -1.0))]
+    d, nl = faces[0]
+    for fd, fn in faces[1:]:
+        if fd < d:
+            d, nl = fd, fn
+    return d, Rw @ np.asarray(nl)
+
+
+class solid_rule:
+    """The fake client's contact detection and response with the solid rule of DESIGN.md §4h (every face, edge and corner of a
+    static primitive solid; one contact per candidate point, the deepest of the floor and the primitives that hold it), for the
+    fixtures of this group only; oracle/fakebullet keeps its own rule for every other fixture."""
+
+    def __enter__(self):
+        import pybullet as fb
+
+        self.fb, self.saved = fb, (fb.World._detect_contacts, fb.World._solve_contacts)
+
+        def detect(world):
+            world.contacts = []
+            statics = [s for s in world.bodies.values() if s.fixed_base]
+            for b in world.bodies.values():
+                if b.fixed_base:
+                    continue
+                low = b.lowest_point_and_threshold()
+                if low is None:
+                    continue
+                pts = _solid_points(b)
+                for s in statics:
+                    if s.is_plane:
+                        hit = low[0] - s.pos[2] < low[1]
+                    else:
+                        hit = any(all(abs(l[a]) <= half[a] + thr for a in range(2)) if kind == "box" else float(np.hypot(l[0], l[1])) <= half[0] + thr
+                                  for kind, centre, Rw, half in _solid_prims(s) for p, thr in pts
+                                  for l in [Rw.T @ (p - centre)] if abs(l[2]) <= half[2] + thr)
+                    if hit:
+                        world.contacts.append((0, s.uid, b.uid, -1, -1))
+                        world.contacts.append((0, b.uid, s.uid, -1, -1))
+
+        def solve(world, b, Rb, M, c, I_O):
+            dt = world.dt
+            prims = [q for s in world.bodies.values() if s.fixed_base and not s.is_plane for q in _solid_prims(s)]
+            cw = Rb @ c
+            Ic = I_O - M * (np.dot(c, c) * np.eye(3) - np.outer(c, c))
+            Iinv = Rb @ np.linalg.inv(Ic) @ Rb.T
+            vc = b.v + np.cross(b.w, cw)
+            w = b.w.copy()
+            pts = [Rb @ p for p in world.contact_points(b.links)]
+            contacts = []  # per point: (depth, normal) of the deepest of the floor and the primitives holding it
+            for pw in pts:
+                x = b.pos + pw
+                depth, n = -x[2], np.array([0.0, 0.0, 1.0])
+                for q in prims:
+                    r = _solid_penetration(*q, x)
+                    if r is not None and r[0] > depth:
+                        depth, n = r
+                contacts.append((depth, n))
+            touched = False
+            for _ in range(world.CONTACT_ITERATIONS):
+                for pw, (depth, n) in zip(pts, contacts):
+                    if depth <= 0.0:
+                        continue
+                    touched = True
+                    r = pw - cw
+                    u = vc + np.cross(w, r)
+                    rn = np.cross(r, n)
+                    kn = 1.0 / M + np.dot(rn, Iinv @ rn)
+                    bias = world.CONTACT_ERP * max(depth - world.CONTACT_SLOP, 0.0) / dt
+                    jn = max(0.0, (bias - np.dot(u, n)) / kn)
+                    if jn > 0.0:
+                        vc = vc + (jn / M) * n
+                        w = w + Iinv @ (jn * rn)
+                        u = vc + np.cross(w, r)
+                        ut = u - np.dot(u, n) * n
+                        sp = float(np.linalg.norm(ut))
+                        if sp > 1e-12:
+                            t = ut / sp
+                            rt = np.cross(r, t)
+                            kt = 1.0 / M + np.dot(rt, Iinv @ rt)
+                            jt = min(sp / kt, world.CONTACT_FRICTION * jn)
+                            vc = vc - (jt / M) * t
+                            w = w - Iinv @ (jt * rt)
+            if touched:
+                b.w = w
+                b.v = vc - np.cross(w, cw)
+
+        fb.World._detect_contacts, fb.World._solve_contacts = detect, solve
+        fb.World.contact_response = True
+        return self
+
+    def __exit__(self, *exc):
+        self.fb.World._detect_contacts, self.fb.World._solve_contacts = self.saved
+        self.fb.World.contact_response = False
+
+
+def solid_fixtures():
+    """The unmodified reference Aviary with fixed-base bodies (loadURDF + register_all_new_bodies), read through
+    contact_array[drone.Id, body], on the fake client with the solid rule and the contact response (solid_rule)."""
+    cf2x = dict(drone_model="cf2x")
+    yaw30 = [0.0, 0.0, np.sin(np.pi / 12), np.cos(np.pi / 12)]
+    ident = [0.0, 0.0, 0.0, 1.0]
+    with solid_rule():
+        # cf2x in mode 7 sent 2.5 m past a wall 1.5 m ahead: flagged and stopped (the flight ends 0.25 s after the impact: pinned
+        # against the wall, the drone chatters, and its attitude then depends on rounding)
+        fly_static("solid_cf2x_wall", "quadx", cf2x, [[0.0, 0.0, 1.0]], [[0.0, 0.0, 0.0]], 7,
+                   [("wall_box.urdf", [1.5, 0.0, 0.0], ident)], {0: [4.0, 0.0, 0.0, 1.0]}, 220, seed=501)
+        # the same flight into the wall yawed 30 degrees
+        fly_static("solid_cf2x_wall_yawed", "quadx", cf2x, [[0.0, 0.3, 1.0]], [[0.0, 0.0, 0.0]], 7,
+                   [("wall_box.urdf", [1.5, 0.0, 0.0], yaw30)], {0: [4.0, 0.3, 0.0, 1.0]}, 220, seed=502)
+        # cf2x meeting a pillar off its centre line: the radial normal turns it, and it slides along the round side
+        fly_static("solid_cf2x_pillar_slide", "quadx", cf2x, [[0.0, 0.0, 1.0]], [[0.0, 0.0, 0.0]], 7,
+                   [("pillar_cylinder.urdf", [1.5, 0.2, 0.0], ident)], {0: [4.0, 0.0, 0.0, 1.0]}, 480, seed=503)
+        # the static_primitive_edge_drop drop under the solid rule: the body over the top meets the top and the edge
+        fly_static("solid_primitive_edge_drop", "quadx", dict(drone_model="primitive_drone"), [[1.0, 0.3, 2.2]], [[0.4, 0.2, 0.0]], -1,
+                   [("platform_box.urdf", [0.0, 0.0, 0.0], ident)], {0: [0.0, 0.0, 0.0, 0.0]}, 480, seed=504)
+        # cf2x landing across the 1 cm step of a slab's edge: floor and top contacts in one solve
+        fly_static("solid_cf2x_step_straddle", "quadx", cf2x, [[1.0, 0.0, 0.5]], [[0.0, 0.0, 0.0]], 7,
+                   [("slab_box.urdf", [0.0, 0.0, 0.0], ident)], {0: [1.0, 0.0, 0.0, -0.2]}, 480, seed=505)
+        # a fixed-wing in powered level flight into a 1 m thick wall
+        fly_static("solid_fixedwing_wall", "fixedwing", dict(drone_model="fixedwing"), [[0.0, 0.0, 5.0]], [[0.0, 0.0, 0.0]], 0,
+                   [("thick_wall.urdf", [20.0, 0.0, 0.0], ident)], {0: [0.0, 0.0, 0.0, 0.8]}, 360, seed=506)
+        # a rocket dropped beside a 1 m platform, its body over the side face, booster off
+        fly_static("solid_rocket_pad_side", "rocket", dict(drone_model="rocket"), [[1.08, 0.0, 5.5]], [[0.0, 0.0, 0.0]], 0,
+                   [("platform_box.urdf", [0.0, 0.0, 0.0], ident)], {0: [0, 0, 0, 0, 0, 0, 0]}, 240, seed=507)
+        # per-world poses: resetBasePositionAndOrientation moves the wall into the path in two worlds and out of it in the third
+        poses = [{0: ([1.2, 0.0, 1.5], [0.0, 0.0, np.sin(0.2), np.cos(0.2)])},
+                 {0: ([1.8, 0.5, 1.5], [0.0, 0.0, np.sin(-0.3), np.cos(-0.3)])},
+                 {0: ([1.5, 8.0, 1.5], ident)}]
+        fly_static("solid_cf2x_per_drone_poses", "quadx", cf2x, [[0.0, 0.0, 1.0]] * 3, [[0.0, 0.0, 0.0]] * 3, 7,
+                   [("wall_box.urdf", [50.0, 0.0, 0.0], ident)], {0: [4.0, 0.0, 0.0, 1.0]}, 220, seed=508, poses=poses)
+
+
 if __name__ == "__main__":
     os.makedirs(OUT, exist_ok=True)
     which = sys.argv[1] if len(sys.argv) > 1 else "all"
@@ -1446,3 +1629,5 @@ if __name__ == "__main__":
         base_state_fixtures()
     if which in ("all", "static"):
         static_fixtures()
+    if which in ("all", "solid"):
+        solid_fixtures()
