@@ -376,8 +376,8 @@ int pfb_observe_state(PfbHandle h, void* stream);
 
 /* ---- static bodies (DESIGN.md §4h): the reference's loadURDF(..., useFixedBase=True) of a landing pad, a helipad or a
  * rooftop.  Aviary handles only.  A body is 1..PFB_MAX_STATIC_SHAPES boxes and cylinders (PfbShape: `at` / `rot` in the
- * body's base link frame; box half extents, cylinder radius and half length), each upright once posed: a box may be yawed,
- * a cylinder's axis is vertical.  Every drone's world holds its own copy of each body.  A primitive is UNDER drone i when
+ * body's base link frame; box half extents, cylinder radius and half length), each upright once posed (a box may be yawed,
+ * a cylinder's axis is vertical) unless the handle is solid (pfb_set_static_solid), which takes any orientation.  Every drone's world holds its own copy of each body.  A primitive is UNDER drone i when
  * its footprint holds the base's (x, y) and z + R_b >= its top (R_b: the model's contact reach); the contact flag of a body
  * is the drone's flag against the top of each primitive under it, and the contact response (contact_response) runs against
  * the highest surface under the drone (the floor, z = 0, or a top).  This top-face rule is the default: side faces are not
@@ -390,14 +390,15 @@ typedef PfbShape PfbStaticShape;
 int pfb_static_shapes_from_urdf(const char* urdf_path, double global_scaling, PfbStaticShape* out, int cap, int* n_shapes,
                                 double inertial_origin[3]);
 /* loadURDF(useFixedBase=True): adds body *body_id = 0, 1, ... to every drone's world with its base LINK frame at pos[3],
- * quat[4] (x, y, z, w; host fp64; upright).  inertial_origin[3] (NULL = 0): the base inertial frame in the link frame, which
+ * quat[4] (x, y, z, w; host fp64; upright, or any unit quaternion on a solid handle).  inertial_origin[3] (NULL = 0): the base inertial frame in the link frame, which
  * pfb_set_static_pose places.                                                                                           */
 int pfb_add_static_body(PfbHandle h, const PfbStaticShape* shapes, int n_shapes, const double pos[3], const double quat[4],
                         const double inertial_origin[3], int* body_id, void* stream);
 /* resetBasePositionAndOrientation of static body `body` in the worlds of the drones of `mask` ([N], NULL = all): device fp64
  * pos [N][3], quat [N][4] (x, y, z, w) of its base INERTIAL frame, as PyBullet's reset places it.  Every quaternion of a
- * drone in the mask must be upright (a yaw about z: 1 - R22 <= 1e-9), else the call fails and changes nothing.  The check
- * reads the quaternions back to the host: this call synchronises `stream`.                                              */
+ * drone in the mask must be upright (a yaw about z: 1 - R22 <= 1e-9), else the call fails and changes nothing; a solid handle
+ * takes any unit quaternion (the link frame is at pos - R o, R the full rotation).  The check reads the quaternions back to
+ * the host: this call synchronises `stream`.                                              */
 int pfb_set_static_pose(PfbHandle h, int body, const double* pos, const double* quat, const uint8_t* mask, void* stream);
 /* bits[i] (device [N]): what drone i touched during the last pfb_aviary_step, bit 0 the floor, bit 1 + k static body k;
  * zero from the first body added after a full pfb_reset until the next step.                                            */
@@ -407,7 +408,9 @@ int pfb_get_static_contacts(PfbHandle h, uint32_t* bits, void* stream);
  * and the primitives that hold it, with that face's normal, for the contact response; bit 1 + k is set when a candidate point
  * lies inside a primitive of body k grown on every face by the contact threshold.  solid = 0 (the default): the top-face rule
  * above.  A property of the handle: pfb_reset keeps it, and it takes effect at the next pfb_aviary_step.  Aviary handles only;
- * solid must be 0 or 1.  Nothing is enqueued on `stream`.                                                                */
+ * solid must be 0 or 1.  A solid handle takes tilted bodies, primitives and poses (pfb_add_static_body, pfb_set_static_pose);
+ * solid = 0 fails while it holds one (until a full pfb_reset).  solid = 1 on a handle that already holds bodies enqueues the
+ * fill of their full poses on `stream`.                                                                                   */
 int pfb_set_static_solid(PfbHandle h, int solid, void* stream);
 
 /* ---- gymnasium-env surface ----------------------------------------------------------------------- */

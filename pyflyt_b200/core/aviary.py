@@ -43,7 +43,8 @@ for script compatibility) puts a landing pad, a helipad or a rooftop into every 
 ``aviary.loadURDF`` does; ``set_static_pose`` moves a body in the worlds of a mask of drones, and ``contact_bodies()`` says
 which body each drone touched.  Up to ``MAX_STATIC_BODIES`` bodies of ``MAX_STATIC_SHAPES`` boxes and cylinders in all,
 upright.  By default only their top faces are solid; ``solid_static_bodies=True`` makes every face, edge and corner solid, so
-that walls, pillars and towers stop and flag a drone that flies into them (DESIGN.md §4h).  ``reset()`` removes the bodies, as
+that walls, pillars and towers stop and flag a drone that flies into them, and lets bodies take any orientation: ramps, race
+gates and bars, tilted by ``baseOrientation``, by ``set_static_pose`` or by the ``rpy`` of their URDF (DESIGN.md §4h).  ``reset()`` removes the bodies, as
 the reference's ``resetSimulation`` does, and keeps ``solid_static_bodies``.
 
 All state is held in caller-visible ``torch`` tensors; the CUDA library (libpyflyt_b200.so) only sees
@@ -427,9 +428,11 @@ class BatchedAviary:
                  globalScaling: float = 1.0) -> int:
         """The reference's ``aviary.loadURDF`` of a fixed-base body (a landing pad, a helipad, a rooftop), placed in every drone's
         world with its base link frame at ``basePosition`` / ``baseOrientation`` (x, y, z, w; None = identity).  Returns the
-        body index ``k``: column ``1 + k`` of ``contact_bodies()``.  The body must be boxes and cylinders joined by fixed joints,
-        upright once posed (a yaw only); spheres, meshes, tilted poses and ``useFixedBase=False`` are refused.  Its top faces
-        are solid, or every face with ``solid_static_bodies=True``.  Aviary handles only."""
+        body index ``k``: column ``1 + k`` of ``contact_bodies()``.  The body must be boxes and cylinders joined by fixed joints;
+        spheres, meshes and ``useFixedBase=False`` are refused.  By default its top faces are solid and it must be upright once
+        posed (a yaw only: a tilted ``baseOrientation`` or collision ``rpy`` is refused).  With ``solid_static_bodies=True``
+        every face is solid and any unit quaternion and any collision ``rpy`` are taken (a ramp, a race gate, a bar).  Aviary
+        handles only."""
         if self.env_config is not None and self.env_config.env_kind != 0:
             raise AviaryInitException("static bodies are for Aviary handles; an env handle (env_config) keeps its own floor and pad.")
         if not useFixedBase:
@@ -460,9 +463,10 @@ class BatchedAviary:
 
     def set_static_pose(self, body: int, pos, quat=None, mask=None) -> None:
         """``resetBasePositionAndOrientation`` of static body ``body`` in the worlds of the drones of ``mask`` ([N] bool; None =
-        every drone): ``pos`` [N, 3] or [3], ``quat`` [N, 4] or [4] (x, y, z, w; None = identity), fp64, upright (a yaw only).
-        As in PyBullet, the pose is that of the body's base INERTIAL frame (``loadURDF``'s ``basePosition`` places its base link
-        frame; the two differ by the inertial origin of the URDF's base link).  Each drone's world keeps its own pose, so every
+        every drone): ``pos`` [N, 3] or [3], ``quat`` [N, 4] or [4] (x, y, z, w; None = identity), fp64; upright (a yaw only)
+        unless the handle has ``solid_static_bodies=True``, which takes any unit quaternion.  As in PyBullet, the pose is that of
+        the body's base INERTIAL frame (``loadURDF``'s ``basePosition`` places its base link frame at ``pos - R o``, R the
+        rotation of ``quat`` and o the inertial origin of the URDF's base link).  Each drone's world keeps its own pose, so every
         drone may get a different one (randomised pads)."""
         n = self.num_drones
         if not 0 <= int(body) < len(self.static_bodies):
@@ -475,8 +479,9 @@ class BatchedAviary:
         err = float(np.max(np.abs(np.linalg.norm(q, axis=1) - 1.0))) if n else 0.0
         if not err <= 1e-6:
             raise ValueError(f"quat must be unit quaternions (x, y, z, w): a norm differs from 1 by {err:.3g} (> 1e-6).")
-        if not _upright_error(q) <= 1e-9:
-            raise ValueError("static bodies stay upright: quat must be a yaw about the world z axis (tilted static bodies are not modelled).")
+        if not self._solid_static_bodies and not _upright_error(q) <= 1e-9:
+            raise ValueError("static bodies stay upright: quat must be a yaw about the world z axis (tilted static bodies are not modelled "
+                             "under the top-face rule).  A handle built with solid_static_bodies=True takes any orientation.")
         pt = torch.as_tensor(np.ascontiguousarray(p), device=self.device)
         qt = torch.as_tensor(np.ascontiguousarray(q), device=self.device)
         m = None

@@ -46,7 +46,7 @@ __device__ __forceinline__ void load_setpoint(const float* setpoint, int64_t u, 
   }
 }
 
-// ---- the world an Aviary step kernel flies its drones in (World = NoStatic, StaticCtx or SolidCtx, pfb_quadx.cuh) -----------
+// ---- the world an Aviary step kernel flies its drones in (World = NoStatic, StaticCtx, SolidCtx or TiltedCtx, pfb_quadx.cuh)
 // The static-body table is the kernel's __grid_constant__ parameter of type WorldTable<World>::T: an empty struct on the
 // floor-only path, so that its parameter bank does not carry the StaticWorld.  The kernel binds drone i's world to it in place,
 // World w{&table, pose, n, i, 0u}; returned by a helper instead, it moves instructions in some kernels (DESIGN.md §4h).  A
@@ -62,6 +62,10 @@ struct WorldTable<StaticCtx> {
 template <>
 struct WorldTable<SolidCtx> {
   using T = StaticWorld;
+};
+template <>
+struct WorldTable<TiltedCtx> {
+  using T = TiltedWorld;
 };
 
 // ---- Aviary.state(i) / aux_state(i) / contact_array of the drone in row j, and the hi / lo words of its position ------------

@@ -125,6 +125,12 @@ struct StaticBodies {
   double inertial[pfb::kMaxStaticBodies][3];  // each body's base inertial origin in its link frame (pfb_set_static_pose places it)
   float* d_pose;           // [kStaticPoseRows * kMaxStaticBodies][n]: x, y, z, cos yaw, sin yaw of body b in drone i's world
   uint32_t* d_bits;        // [n], user order: bit 0 the floor, bit 1 + b body b, touched during the last Aviary step
+  // solid handles (pfb_set_static_solid): the table and the poses of the rule with full rotation frames (pfb::TiltedCtx).
+  // d_full: [kTiltedPoseRows * kMaxStaticBodies][n], x, y, z and the row-major base link -> world rotation of body b in drone
+  // i's world; written with d_pose for every body, so that the handle can change path at any step.
+  pfb::TiltedWorld tworld;
+  float* d_full;
+  bool tilted;             // a tilted body, primitive or masked pose since the last reset: the step launches TiltedCtx
 };
 // The static bodies an Aviary step launch flies against; nullptr = none: the handle launches the kernels it launched before
 // static bodies existed
@@ -331,14 +337,17 @@ int tail_env_step(PfbContext* h, const float* noise, bool randact, cudaStream_t 
 // ---- host side of the Aviary step (pfb_aviary_step) of every vehicle kind and of the mixed-kind handle ----
 // Each kind passes one generic lambda `launch(AviaryVariant<INJECT, CONTACT, World>{sb})` that launches its step kernel and
 // returns 0 or the result of fail().  INJECT: injected noise; CONTACT: aviary_contact_response(h); World: pfb::StaticCtx with
-// the handle's static bodies `sb` (step_statics), pfb::SolidCtx with them on a handle with pfb_set_static_solid, or
-// pfb::NoStatic with sb = nullptr.  The kernel takes world_table(v), v.pose() and v.bits().
+// the handle's static bodies `sb` (step_statics), pfb::SolidCtx with them on a handle with pfb_set_static_solid
+// (pfb::TiltedCtx once it holds a tilted body), or pfb::NoStatic with sb = nullptr.  The kernel takes world_table(v), v.pose() and v.bits().
 template <bool INJECT, bool CONTACT, class World>
 struct AviaryVariant {
   static constexpr bool inject = INJECT, contact = CONTACT;
   using world = World;
   const StaticBodies* sb;
-  const float* pose() const { return sb ? sb->d_pose : nullptr; }
+  const float* pose() const {
+    if constexpr (std::is_same<World, pfb::TiltedCtx>::value) return sb->d_full;
+    return sb ? sb->d_pose : nullptr;
+  }
   uint32_t* bits() const { return sb ? sb->d_bits : nullptr; }
 };
 
@@ -349,10 +358,15 @@ template <bool INJECT, bool CONTACT>
 const pfb::StaticWorld& world_table(AviaryVariant<INJECT, CONTACT, pfb::StaticCtx> v) { return v.sb->world; }
 template <bool INJECT, bool CONTACT>
 const pfb::StaticWorld& world_table(AviaryVariant<INJECT, CONTACT, pfb::SolidCtx> v) { return v.sb->world; }
+template <bool INJECT, bool CONTACT>
+const pfb::TiltedWorld& world_table(AviaryVariant<INJECT, CONTACT, pfb::TiltedCtx> v) { return v.sb->tworld; }
 
+// A solid handle runs the yaw frames of SolidCtx while every body, primitive and pose since its last reset is upright, so that
+// upright scenes keep their bits and their cheaper cull (5 pose words per primitive); TiltedCtx once one is tilted.
 template <bool INJECT, bool CONTACT, class Launch>
 int aviary_step_world(const StaticBodies* sb, bool solid, Launch& launch) {
   if (!sb) return launch(AviaryVariant<INJECT, CONTACT, pfb::NoStatic>{nullptr});
+  if (solid && sb->tilted) return launch(AviaryVariant<INJECT, CONTACT, pfb::TiltedCtx>{sb});
   return solid ? launch(AviaryVariant<INJECT, CONTACT, pfb::SolidCtx>{sb}) : launch(AviaryVariant<INJECT, CONTACT, pfb::StaticCtx>{sb});
 }
 template <class Launch>

@@ -286,8 +286,8 @@ PFB_HD Vec3 contact_candidate(const Shapes* cp, int sh, int kind, const float* d
 }
 
 // ---- the solid rule (SolidCtx: pfb_set_static_solid; DESIGN.md §4h) ----------------------------------------------------------
-// Every static primitive is a solid on all of its faces: a box yawed about z, or a vertical cylinder.  A point is tested in the
-// primitive's own frame: centre at `at` of the posed body, yaw = body yaw + primitive yaw.
+// Every static primitive is a solid on all of its faces.  A point is tested in the primitive's own frame: centre at `at` of the
+// posed body; SolidCtx: a box yawed about z or a vertical cylinder, yaw = body yaw + primitive yaw; TiltedCtx: any rotation.
 struct SolidFrame { float cx, cy, cz, c, s; };
 PFB_HD SolidFrame solid_frame(const StaticWorld& w, const float* pose, int64_t n, int64_t i, int k) {
   const float* q = pose + (int64_t)kStaticPoseRows * w.body[k] * n + i;
@@ -299,6 +299,36 @@ PFB_HD Vec3 solid_local(const SolidFrame& f, float x, float y, float z) {
   const float dx = x - f.cx, dy = y - f.cy;
   return Vec3{f.c * dx + f.s * dy, f.c * dy - f.s * dx, z - f.cz};
 }
+// primitive-frame direction m in the world frame
+PFB_HD Vec3 solid_to_world(const SolidFrame& f, Vec3 m) { return Vec3{f.c * m.x - f.s * m.y, f.s * m.x + f.c * m.y, m.z}; }
+// TiltedCtx: the same with a full rotation r (row-major, primitive -> world) = body rotation x primitive rotation, centre =
+// body origin + body rotation x `at`
+struct TiltFrame { float cx, cy, cz, r[9]; };
+PFB_HD TiltFrame solid_frame(const TiltedWorld& w, const float* pose, int64_t n, int64_t i, int k) {
+  const float* q = pose + (int64_t)kTiltedPoseRows * w.body[k] * n + i;
+  float b[9];
+#pragma unroll
+  for (int e = 0; e < 9; ++e) b[e] = q[(3 + e) * n];
+  const float* a = w.at[k];
+  const float* p = w.rot[k];
+  TiltFrame f;
+  f.cx = q[0] + b[0] * a[0] + b[1] * a[1] + b[2] * a[2];
+  f.cy = q[n] + b[3] * a[0] + b[4] * a[1] + b[5] * a[2];
+  f.cz = q[2 * n] + b[6] * a[0] + b[7] * a[1] + b[8] * a[2];
+#pragma unroll
+  for (int r = 0; r < 3; ++r)
+#pragma unroll
+    for (int c = 0; c < 3; ++c) f.r[3 * r + c] = b[3 * r] * p[c] + b[3 * r + 1] * p[3 + c] + b[3 * r + 2] * p[6 + c];
+  return f;
+}
+// R^T (p - c)
+PFB_HD Vec3 solid_local(const TiltFrame& f, float x, float y, float z) {
+  const float dx = x - f.cx, dy = y - f.cy, dz = z - f.cz;
+  return Vec3{f.r[0] * dx + f.r[3] * dy + f.r[6] * dz, f.r[1] * dx + f.r[4] * dy + f.r[7] * dz, f.r[2] * dx + f.r[5] * dy + f.r[8] * dz};
+}
+PFB_HD Vec3 solid_to_world(const TiltFrame& f, Vec3 m) {
+  return Vec3{f.r[0] * m.x + f.r[1] * m.y + f.r[2] * m.z, f.r[3] * m.x + f.r[4] * m.y + f.r[5] * m.z, f.r[6] * m.x + f.r[7] * m.y + f.r[8] * m.z};
+}
 // world point of base-frame point pb
 PFB_HD Vec3 solid_point(const SolidBase& b, Vec3 pb) {
   return Vec3{b.px + dot(Vec3{b.r[0], b.r[1], b.r[2]}, pb), b.py + dot(Vec3{b.r[3], b.r[4], b.r[5]}, pb), b.pz + dot(Vec3{b.r[6], b.r[7], b.r[8]}, pb)};
@@ -307,7 +337,8 @@ PFB_HD Vec3 solid_point(const SolidBase& b, Vec3 pb) {
 // The cull: bit k set when the base is within `reach` (the model's contact reach, contact_zmax / ContactParams::zmax) of
 // primitive k's bounding box in its own frame (the box itself; the cylinder's square prism), along each of its axes.  reach
 // bounds |candidate point - base| + the contact threshold, so a culled primitive holds no candidate point, even grown.
-PFB_HD uint32_t solid_live(const StaticWorld& w, const float* pose, int64_t n, int64_t i, float px, float py, float pz, float reach) {
+template <class W>
+PFB_HD uint32_t solid_live(const W& w, const float* pose, int64_t n, int64_t i, float px, float py, float pz, float reach) {
   uint32_t live = 0u;
 #pragma unroll 1
   for (int k = 0; k < w.n_shapes; ++k) {
@@ -321,7 +352,8 @@ PFB_HD uint32_t solid_live(const StaticWorld& w, const float* pose, int64_t n, i
 // normal in the primitive frame.  Box: the face of least half_a - |l_a|, ties to +z, then +-x, then +-y, then -z.  Cylinder:
 // the least of radial r - rho, top h - l_z and bottom h + l_z, ties to top, then radial, then bottom; the radial normal is
 // +x for rho < 1e-6.
-PFB_HD bool solid_penetration(const StaticWorld& w, int k, Vec3 l, float& depth, Vec3& nl) {
+template <class W>
+PFB_HD bool solid_penetration(const W& w, int k, Vec3 l, float& depth, Vec3& nl) {
   const float* h = w.half[k];
   float d = h[2] - l.z;
   Vec3 m = Vec3{0.0f, 0.0f, 1.0f};
@@ -345,33 +377,30 @@ PFB_HD bool solid_penetration(const StaticWorld& w, int k, Vec3 l, float& depth,
 
 // The contact of world point (x, y, z): the deepest of the floor (depth -z, normal +z) and every primitive of `live` that holds
 // the point; ties go to the floor, then to the primitive first in table order.  The normal is in the world frame.
+// W: StaticWorld (SolidCtx: yaw frames) or TiltedWorld (TiltedCtx: rotation frames), as for every helper of the rule.
 struct SolidContact { float depth; Vec3 n; };
-PFB_HD SolidContact solid_point_contact(const StaticWorld& w, const float* pose, int64_t n, int64_t i, uint32_t live, float x, float y, float z) {
+template <class W>
+PFB_HD SolidContact solid_point_contact(const W& w, const float* pose, int64_t n, int64_t i, uint32_t live, float x, float y, float z) {
   SolidContact r{-z, Vec3{0.0f, 0.0f, 1.0f}};
 #pragma unroll 1
   for (int k = 0; k < w.n_shapes; ++k) {
     if (!((live >> k) & 1u)) continue;
-    const SolidFrame f = solid_frame(w, pose, n, i, k);
+    const auto f = solid_frame(w, pose, n, i, k);
     float d;
     Vec3 m;
     if (!solid_penetration(w, k, solid_local(f, x, y, z), d, m) || !(d > r.depth)) continue;
     r.depth = d;
-    r.n = Vec3{f.c * m.x - f.s * m.y, f.s * m.x + f.c * m.y, m.z};
+    r.n = solid_to_world(f, m);
   }
   return r;
 }
 
 // Bits 1 + b of the solid rule: a candidate point of the drone lies inside a primitive of body b grown on every face by the
 // contact threshold of that point's drone primitive (the floor's bit 0 is the caller's).  Only the primitives of `live`.
-// Out of line and by value: it runs only near a body, and inlined it would hold its state in registers of the hot loop.
-template <class Shapes>
-#if defined(__CUDACC__)
-static __host__ __device__ __noinline__
-#else
-inline
-#endif
-uint32_t solid_bits(const StaticWorld* wp, const float* pose, int64_t n, int64_t i, uint32_t live, const Shapes* cp, SolidBase b) {
-  const StaticWorld& w = *wp;
+// Out of line and by value: it runs only near a body, and inlined it would hold its state in registers of the hot loop.  One
+// body for both frames (solid_bits_in); each World has its own out-of-line copy.
+template <class W, class Shapes>
+PFB_HD uint32_t solid_bits_in(const W& w, const float* pose, int64_t n, int64_t i, uint32_t live, const Shapes* cp, SolidBase b) {
   uint32_t bits = 0u;
 #pragma unroll 1
   for (int sh = 0; sh < contact_n_shapes(*cp); ++sh) {
@@ -394,6 +423,24 @@ uint32_t solid_bits(const StaticWorld* wp, const float* pose, int64_t n, int64_t
     }
   }
   return bits;
+}
+template <class Shapes>
+#if defined(__CUDACC__)
+static __host__ __device__ __noinline__
+#else
+inline
+#endif
+uint32_t solid_bits(const StaticWorld* wp, const float* pose, int64_t n, int64_t i, uint32_t live, const Shapes* cp, SolidBase b) {
+  return solid_bits_in(*wp, pose, n, i, live, cp, b);
+}
+template <class Shapes>
+#if defined(__CUDACC__)
+static __host__ __device__ __noinline__
+#else
+inline
+#endif
+uint32_t solid_bits(const TiltedWorld* wp, const float* pose, int64_t n, int64_t i, uint32_t live, const Shapes* cp, SolidBase b) {
+  return solid_bits_in(*wp, pose, n, i, live, cp, b);
 }
 
 // kContactIterations sweeps of the sequential impulse over the candidate points; at(pb, n) returns the depth of base-frame
@@ -460,7 +507,19 @@ ContactVel solve_contacts(const Shapes* cp, float pz, float top, Vec3 n /* world
 }
 
 // The solver of the solid rule: each candidate point takes its contact from solid_point_contact (the floor and the solids of
-// `live`), its normal rotated into the body frame.  b: the pose at the start of the substep.
+// `live`), its normal rotated into the body frame.  b: the pose at the start of the substep.  One body for both frames
+// (Ctx = SolidCtx or TiltedCtx); each has its own out-of-line copy.
+template <class Shapes, class Ctx>
+PFB_HD ContactVel solve_contacts_solid_in(const Shapes* cp, const Ctx& world, uint32_t live, SolidBase b, Vec3 vb, Vec3 w, float M, Vec3 c, float Ixx,
+                                          float Ixy, float Ixz, float Iyy, float Iyz, float Izz, float dt) {
+  return contact_sweeps(cp, [&](Vec3 pb, Vec3& pn) {
+    const Vec3 pw = solid_point(b, pb);
+    const SolidContact k = solid_point_contact(*world.w, world.pose, world.n, world.i, live, pw.x, pw.y, pw.z);
+    pn = Vec3{b.r[0] * k.n.x + b.r[3] * k.n.y + b.r[6] * k.n.z, b.r[1] * k.n.x + b.r[4] * k.n.y + b.r[7] * k.n.z,
+              b.r[2] * k.n.x + b.r[5] * k.n.y + b.r[8] * k.n.z};
+    return k.depth;
+  }, vb, w, M, c, Ixx, Ixy, Ixz, Iyy, Iyz, Izz, dt);
+}
 template <class Shapes>
 #if defined(__CUDACC__)
 static __host__ __device__ __noinline__
@@ -469,13 +528,17 @@ inline
 #endif
 ContactVel solve_contacts_solid(const Shapes* cp, SolidCtx world, uint32_t live, SolidBase b, Vec3 vb, Vec3 w, float M, Vec3 c, float Ixx,
                                 float Ixy, float Ixz, float Iyy, float Iyz, float Izz, float dt) {
-  return contact_sweeps(cp, [&](Vec3 pb, Vec3& pn) {
-    const Vec3 pw = solid_point(b, pb);
-    const SolidContact k = solid_point_contact(*world.w, world.pose, world.n, world.i, live, pw.x, pw.y, pw.z);
-    pn = Vec3{b.r[0] * k.n.x + b.r[3] * k.n.y + b.r[6] * k.n.z, b.r[1] * k.n.x + b.r[4] * k.n.y + b.r[7] * k.n.z,
-              b.r[2] * k.n.x + b.r[5] * k.n.y + b.r[8] * k.n.z};
-    return k.depth;
-  }, vb, w, M, c, Ixx, Ixy, Ixz, Iyy, Iyz, Izz, dt);
+  return solve_contacts_solid_in(cp, world, live, b, vb, w, M, c, Ixx, Ixy, Ixz, Iyy, Iyz, Izz, dt);
+}
+template <class Shapes>
+#if defined(__CUDACC__)
+static __host__ __device__ __noinline__
+#else
+inline
+#endif
+ContactVel solve_contacts_solid(const Shapes* cp, TiltedCtx world, uint32_t live, SolidBase b, Vec3 vb, Vec3 w, float M, Vec3 c, float Ixx,
+                                float Ixy, float Ixz, float Iyy, float Iyz, float Izz, float dt) {
+  return solve_contacts_solid_in(cp, world, live, b, vb, w, M, c, Ixx, Ixy, Ixz, Iyy, Iyz, Izz, dt);
 }
 
 // Contact impulses on the predicted velocities of `s` (world linear velocity, body angular velocity), before its pose is
@@ -504,16 +567,17 @@ PFB_HD void apply_contact_impulses(const Shapes* cp, Regs& s, float pz0, float t
 }
 // against the floor and the solids of `live` (the solid rule), from the pose of `s`, which is still that of the start of the
 // substep
-template <class Shapes, class Regs>
-PFB_HD void apply_solid_impulses(const Shapes* cp, Regs& s, const SolidCtx& world, uint32_t live, float M, Vec3 c, float Ixx, float Ixy, float Ixz,
+template <class Shapes, class Regs, class Ctx>
+PFB_HD void apply_solid_impulses(const Shapes* cp, Regs& s, const Ctx& world, uint32_t live, float M, Vec3 c, float Ixx, float Ixy, float Ixz,
                                  float Iyy, float Iyz, float Izz, float dt) {
   const SolidBase b = solid_base(s);
   contact_impulses_with(s, [&](Vec3, Vec3 vbn, Vec3 w) { return solve_contacts_solid(cp, world, live, b, vbn, w, M, c, Ixx, Ixy, Ixz, Iyy, Iyz, Izz, dt); });
 }
 
-// what the solid rule's response runs against (rigid_step's `top` with Tag = SolidCtx)
+// what the solid rule's response runs against (rigid_step's `top` with Tag = SolidCtx or TiltedCtx)
+template <class Ctx>
 struct SolidSurface {
-  const SolidCtx* world;
+  const Ctx* world;
   uint32_t live;
 };
 
@@ -738,7 +802,7 @@ PFB_HD void fixedwing_substep(const FixedwingParams& p, FixedwingRegs& s, const 
     world->bits |= b;
     const bool c = b != 0u;
     s.flags = (s.flags & ~(uint32_t)FLAG_CONTACT_PREV) | (c ? (FLAG_CONTACT_PREV | FLAG_CONTACT_ARRAY) : 0u);
-    rigid_step<CONTACT, World>(p.rb, p.gravity, p.dt, p.vmax, s, F, T, &p.contact, c, SolidSurface{world, live});
+    rigid_step<CONTACT, World>(p.rb, p.gravity, p.dt, p.vmax, s, F, T, &p.contact, c, SolidSurface<World>{world, live});
   } else if constexpr (World::kOn) {
     const float pz = (float)s.pz, r20 = (float)s.R.m20, r21 = (float)s.R.m21, r22 = (float)s.R.m22;
     uint32_t b;

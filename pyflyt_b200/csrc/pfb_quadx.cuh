@@ -361,8 +361,8 @@ struct StaticWorld {
   float half[kMaxStaticShapes][3];    // box: half extents; cylinder: radius, radius, half length
 };
 // The step bodies take a World: NoStatic (the floor only: the kernels every handle without static bodies launches),
-// StaticCtx (the floor and the top faces of the static bodies of drone i's world) or SolidCtx (the floor and the static
-// bodies of drone i's world as solids: pfb_set_static_solid).  bits: what drone i touched during its current Aviary step,
+// StaticCtx (the floor and the top faces of the static bodies of drone i's world), SolidCtx (the floor and the static
+// bodies of drone i's world as solids: pfb_set_static_solid) or TiltedCtx (the same in full rotation frames, below).  bits: what drone i touched during its current Aviary step,
 // bit 0 the floor, bit 1 + b static body b.  A step kernel initialises each as World w{&table, pose, n, i, 0u}.
 struct NoStaticTable {};
 struct NoStatic {
@@ -386,6 +386,26 @@ struct SolidCtx {
   int64_t n, i;
   uint32_t bits;
 };
+// The solid rule with full rotation frames: tilted static bodies (pfb_static.cu: a solid handle that holds a tilted body,
+// primitive or pose since its last reset).  Its own table: each primitive's centre and rotation (row-major, primitive ->
+// body) in its body's base link frame; the pose of body b in drone i's world is rows 12 b .. 12 b + 11 (x, y, z, then the
+// row-major base link -> world rotation) of a field-major [12 * kMaxStaticBodies][n] buffer.
+constexpr int kTiltedPoseRows = 12;
+struct TiltedWorld {
+  int n_shapes;
+  int body[kMaxStaticShapes];
+  int kind[kMaxStaticShapes];
+  float at[kMaxStaticShapes][3];
+  float rot[kMaxStaticShapes][9];
+  float half[kMaxStaticShapes][3];
+};
+struct TiltedCtx {
+  static constexpr bool kOn = true, kSolid = true;
+  const TiltedWorld* w;
+  const float* pose;
+  int64_t n, i;
+  uint32_t bits;
+};
 // pfb_fixedwing.cuh: surface height under a drone and its contact bits
 template <class Touch>
 PFB_HD float static_surface(const StaticWorld& w, const float* pose, int64_t n, int64_t i, float px, float py, float pz, float reach,
@@ -393,7 +413,8 @@ PFB_HD float static_surface(const StaticWorld& w, const float* pose, int64_t n, 
 // pfb_fixedwing.cuh: the solid rule (SolidCtx) — the primitives within reach of the base, and the contact bits of the drone's
 // candidate points against them
 struct SolidBase { float px, py, pz, r[9]; };  // base position and body -> world rotation (row-major) at the start of the substep
-PFB_HD uint32_t solid_live(const StaticWorld& w, const float* pose, int64_t n, int64_t i, float px, float py, float pz, float reach);
+template <class W>
+PFB_HD uint32_t solid_live(const W& w, const float* pose, int64_t n, int64_t i, float px, float py, float pz, float reach);
 template <class Shapes>
 #if defined(__CUDACC__)
 static __host__ __device__ __noinline__
@@ -401,9 +422,16 @@ static __host__ __device__ __noinline__
 inline
 #endif
 uint32_t solid_bits(const StaticWorld* w, const float* pose, int64_t n, int64_t i, uint32_t live, const Shapes* cp, SolidBase b);
-// the contact response against the floor and the solids of `live` (pfb_fixedwing.cuh)
-template <class Shapes, class Regs>
-PFB_HD void apply_solid_impulses(const Shapes* cp, Regs& s, const SolidCtx& world, uint32_t live, float M, Vec3 c, float Ixx, float Ixy, float Ixz,
+template <class Shapes>
+#if defined(__CUDACC__)
+static __host__ __device__ __noinline__
+#else
+inline
+#endif
+uint32_t solid_bits(const TiltedWorld* w, const float* pose, int64_t n, int64_t i, uint32_t live, const Shapes* cp, SolidBase b);
+// the contact response against the floor and the solids of `live` (pfb_fixedwing.cuh); Ctx = SolidCtx or TiltedCtx
+template <class Shapes, class Regs, class Ctx>
+PFB_HD void apply_solid_impulses(const Shapes* cp, Regs& s, const Ctx& world, uint32_t live, float M, Vec3 c, float Ixx, float Ixy, float Ixz,
                                  float Iyy, float Iyz, float Izz, float dt);
 template <class Regs>
 PFB_HD SolidBase solid_base(const Regs& s) {

@@ -1,9 +1,11 @@
 // pfb_static.cu — static (fixed-base) bodies of an Aviary handle (DESIGN.md §4h): the reference's
 // loadURDF(..., useFixedBase=True) of a landing pad, a helipad or a rooftop, one copy in every drone's world.
 //
-// The primitive table (pfb::StaticWorld) is host-side here and travels to every step launch as a kernel parameter; the poses are
-// a field-major device buffer that only pfb_add_static_body and pfb_set_static_pose write.  The step kernels themselves live
-// with each vehicle kind (pfb_quadx.cu, pfb_fixedwing.cu, pfb_rocket.cu, pfb_mixed.cu) and run when step_statics(h) is set.
+// The primitive table (pfb::StaticWorld, and pfb::TiltedWorld on solid handles) is host-side here and travels to every step
+// launch as a kernel parameter; the poses are field-major device buffers (yaw poses, and full poses on solid handles) that
+// only pfb_add_static_body and pfb_set_static_pose write (and pfb_set_static_solid fills, for a handle made solid late).  The
+// step kernels themselves live with each vehicle kind (pfb_quadx.cu, pfb_fixedwing.cu, pfb_rocket.cu, pfb_mixed.cu) and run
+// when step_statics(h) is set.
 #include <cuda_runtime.h>
 
 #include <cmath>
@@ -44,11 +46,74 @@ static bool upright(const double* q) {
   return n > 0.0 && 2.0 * (q[0] * q[0] + q[1] * q[1]) / n <= 1e-9;
 }
 
+// ---- full poses of a solid handle (StaticBodies::d_full, read by TiltedCtx) -------------------------------------------------
+// the row-major rotation of quaternion (x, y, z, w), normalised
+PFB_HD void quat_rotation(double x, double y, double z, double w, double* r) {
+  const double d = 2.0 / (x * x + y * y + z * z + w * w);
+  r[0] = 1.0 - d * (y * y + z * z); r[1] = d * (x * y - z * w);       r[2] = d * (x * z + y * w);
+  r[3] = d * (x * y + z * w);       r[4] = 1.0 - d * (x * x + z * z); r[5] = d * (y * z - x * w);
+  r[6] = d * (x * z - y * w);       r[7] = d * (y * z + x * w);       r[8] = 1.0 - d * (x * x + y * y);
+}
+struct FullPose { float v[kTiltedPoseRows]; };  // x, y, z, row-major rotation
+
+// rows 12 b .. 12 b + 11 of every drone's world: the pose of body b
+__global__ void __launch_bounds__(kBlock) k_static_fill_full(float* __restrict__ full, int body, const __grid_constant__ FullPose p, int64_t N) {
+  int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= N) return;
+  float* q = full + (int64_t)kTiltedPoseRows * body * N + i;
+#pragma unroll
+  for (int e = 0; e < kTiltedPoseRows; ++e) q[e * N] = p.v[e];
+}
+
+// k_static_set_pose's reset with the full rotation R of each quaternion: the link frame is at pos - R (ox, oy, oz)
+__global__ void __launch_bounds__(kBlock) k_static_set_full_pose(float* __restrict__ full, int body, const double* __restrict__ pos,
+                                                                 const double* __restrict__ quat, const uint8_t* __restrict__ mask, double ox,
+                                                                 double oy, double oz, int64_t N) {
+  int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= N) return;
+  if (mask && !mask[i]) return;
+  double r[9];
+  quat_rotation(quat[4 * i], quat[4 * i + 1], quat[4 * i + 2], quat[4 * i + 3], r);
+  float* q = full + (int64_t)kTiltedPoseRows * body * N + i;
+  q[0] = (float)(pos[3 * i] - (r[0] * ox + r[1] * oy + r[2] * oz));
+  q[N] = (float)(pos[3 * i + 1] - (r[3] * ox + r[4] * oy + r[5] * oz));
+  q[2 * N] = (float)(pos[3 * i + 2] - (r[6] * ox + r[7] * oy + r[8] * oz));
+#pragma unroll
+  for (int e = 0; e < 9; ++e) q[(3 + e) * N] = (float)r[e];
+}
+
+// the full poses of bodies 0 .. n_bodies - 1 from their yaw poses (all upright): a handle that becomes solid after its first body
+__global__ void __launch_bounds__(kBlock) k_static_full_from_yaw(float* __restrict__ full, const float* __restrict__ pose, int n_bodies, int64_t N) {
+  int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= N) return;
+  for (int b = 0; b < n_bodies; ++b) {
+    const float* y = pose + (int64_t)kStaticPoseRows * b * N + i;
+    float* q = full + (int64_t)kTiltedPoseRows * b * N + i;
+    const float c = y[3 * N], sn = y[4 * N];
+    const float v[kTiltedPoseRows] = {y[0], y[N], y[2 * N], c, -sn, 0.0f, sn, c, 0.0f, 0.0f, 0.0f, 1.0f};
+#pragma unroll
+    for (int e = 0; e < kTiltedPoseRows; ++e) q[e * N] = v[e];
+  }
+}
+
+// the full-pose buffer of a solid handle with static-body buffers, filled from the yaw poses of the bodies it holds
+static int static_alloc_full(PfbContext* h, cudaStream_t st) {
+  StaticBodies* b = h->statics;
+  if (!b || b->d_full) return 0;
+  CUDA_OK(cudaMalloc(&b->d_full, (size_t)kTiltedPoseRows * kMaxStaticBodies * (size_t)h->n * sizeof(float)));
+  if (b->n_bodies > 0) {
+    k_static_full_from_yaw<<<grid_for(h->n), kBlock, 0, st>>>(b->d_full, b->d_pose, b->n_bodies, h->n);
+    LAUNCH_CHECK(h);
+  }
+  return 0;
+}
+
 void static_destroy(PfbContext* h) {
   StaticBodies* b = h->statics;
   if (!b) return;
   if (b->d_pose) cudaFree(b->d_pose);
   if (b->d_bits) cudaFree(b->d_bits);
+  if (b->d_full) cudaFree(b->d_full);
   delete b;
   h->statics = nullptr;
 }
@@ -58,6 +123,8 @@ void static_clear(PfbContext* h) {
   if (!h->statics) return;
   h->statics->n_bodies = 0;
   h->statics->world.n_shapes = 0;
+  h->statics->tworld.n_shapes = 0;
+  h->statics->tilted = false;
 }
 
 // Aviary handles only: an env handle keeps its own floor and pad policy
@@ -78,16 +145,25 @@ extern "C" int pfb_add_static_body(PfbHandle h, const PfbStaticShape* shapes, in
   if (have_shapes + n_shapes > kMaxStaticShapes)
     return fail("pfb_add_static_body: at most %d collision primitives over all static bodies of a handle (have %d, adding %d)", kMaxStaticShapes,
                 have_shapes, n_shapes);
-  if (!upright(quat))
-    return fail("pfb_add_static_body: the body must stay upright (only a yaw about the world z axis): tilted static bodies are not modelled");
-  // each primitive upright in the body frame: a box yawed about its z axis, a cylinder whose axis is z
+  // the top-face rule needs upright bodies and primitives; a solid handle takes any orientation (TiltedCtx once one is tilted)
+  const bool solid = h->static_solid;
+  bool tilted = !upright(quat);
+  if (tilted && !solid)
+    return fail("pfb_add_static_body: the body must stay upright (only a yaw about the world z axis): tilted static bodies are not modelled "
+                "under the top-face rule.  A solid handle (pfb_set_static_solid, solid_static_bodies=True) takes any orientation");
+  // each primitive upright in the body frame (a box yawed about its z axis, a cylinder whose axis is z), unless the handle is solid
   for (int k = 0; k < n_shapes; ++k) {
     const PfbStaticShape& s = shapes[k];
     if (s.kind != PFB_SHAPE_BOX && s.kind != PFB_SHAPE_CYLINDER)
       return fail("pfb_add_static_body: primitive %d is a %s; static bodies are boxes and cylinders", k, s.kind == PFB_SHAPE_SPHERE ? "sphere" : "mesh or unknown shape");
     const double* r = s.rot;
     const double tilt = fabs(r[2]) + fabs(r[5]) + fabs(r[6]) + fabs(r[7]) + fabs(r[8] - 1.0);
-    if (!(tilt <= 1e-9)) return fail("pfb_add_static_body: primitive %d is tilted in its body; only a yaw about the body's z axis is modelled", k);
+    if (!(tilt <= 1e-9)) {
+      if (!solid)
+        return fail("pfb_add_static_body: primitive %d is tilted in its body; only a yaw about the body's z axis is modelled under the top-face "
+                    "rule.  A solid handle (pfb_set_static_solid, solid_static_bodies=True) takes any orientation", k);
+      tilted = true;
+    }
     if (!(s.dims[0] > 0.0 && s.dims[1] > 0.0 && (s.kind == PFB_SHAPE_CYLINDER || s.dims[2] > 0.0)))
       return fail("pfb_add_static_body: primitive %d has a non-positive size", k);
   }
@@ -110,6 +186,7 @@ extern "C" int pfb_add_static_body(PfbHandle h, const PfbStaticShape* shapes, in
     h->statics = b;
   }
   StaticBodies* b = h->statics;
+  if (solid && static_alloc_full(h, st)) return -1;
   const int body = b->n_bodies;
   // the first body since creation or a full reset: no contact with a static body yet (resetSimulation empties contact_array)
   if (body == 0) CUDA_OK(cudaMemsetAsync(b->d_bits, 0, (size_t)h->n * sizeof(uint32_t), st));
@@ -122,20 +199,38 @@ extern "C" int pfb_add_static_body(PfbHandle h, const PfbStaticShape* shapes, in
     w.kind[j] = s.kind;
     for (int c = 0; c < 3; ++c) w.at[j][c] = (float)s.at[c];
     const double nrm = std::sqrt(s.rot[0] * s.rot[0] + s.rot[3] * s.rot[3]);  // first column = (cos, sin, 0) of the yaw
-    w.cyaw[j] = (float)(s.rot[0] / nrm);
-    w.syaw[j] = (float)(s.rot[3] / nrm);
+    w.cyaw[j] = nrm > 0.0 ? (float)(s.rot[0] / nrm) : 1.0f;  // a tilted primitive's yaw is never read (TiltedCtx)
+    w.syaw[j] = nrm > 0.0 ? (float)(s.rot[3] / nrm) : 0.0f;
+    TiltedWorld& t = b->tworld;
+    t.body[j] = body;
+    t.kind[j] = s.kind;
+    for (int c = 0; c < 3; ++c) t.at[j][c] = w.at[j][c];
+    for (int e = 0; e < 9; ++e) t.rot[j][e] = (float)s.rot[e];
     if (s.kind == PFB_SHAPE_BOX) {
       for (int c = 0; c < 3; ++c) w.half[j][c] = (float)s.dims[c];
     } else {
       w.half[j][0] = w.half[j][1] = (float)s.dims[0];
       w.half[j][2] = (float)s.dims[1];
     }
+    for (int c = 0; c < 3; ++c) t.half[j][c] = w.half[j][c];
   }
   const double z = quat[2], qw = quat[3], d = qw * qw + z * z;
-  k_static_fill<<<grid_for(h->n), kBlock, 0, st>>>(b->d_pose, body, (float)pos[0], (float)pos[1], (float)pos[2], (float)((qw * qw - z * z) / d),
-                                                   (float)(2.0 * qw * z / d), h->n);
+  // the yaw pose of a tilted body is never read (TiltedCtx); d = 0 (a half turn about a horizontal axis) keeps it finite
+  k_static_fill<<<grid_for(h->n), kBlock, 0, st>>>(b->d_pose, body, (float)pos[0], (float)pos[1], (float)pos[2], d > 0.0 ? (float)((qw * qw - z * z) / d) : 1.0f,
+                                                   d > 0.0 ? (float)(2.0 * qw * z / d) : 0.0f, h->n);
   LAUNCH_CHECK(h);
+  if (b->d_full) {
+    double r[9];
+    quat_rotation(quat[0], quat[1], quat[2], quat[3], r);
+    FullPose fp;
+    for (int c = 0; c < 3; ++c) fp.v[c] = (float)pos[c];
+    for (int e = 0; e < 9; ++e) fp.v[3 + e] = (float)r[e];
+    k_static_fill_full<<<grid_for(h->n), kBlock, 0, st>>>(b->d_full, body, fp, h->n);
+    LAUNCH_CHECK(h);
+  }
+  b->tilted = b->tilted || tilted;
   w.n_shapes += n_shapes;
+  b->tworld.n_shapes += n_shapes;
   b->n_bodies += 1;
   *body_id = body;
   return 0;
@@ -148,7 +243,8 @@ extern "C" int pfb_set_static_pose(PfbHandle h, int body, const double* pos, con
   if (body < 0 || body >= have) return fail("pfb_set_static_pose: no static body %d (the handle has %d)", body, have);
   CUDA_OK(cudaSetDevice(h->device));
   cudaStream_t st = (cudaStream_t)stream;
-  {  // every masked quaternion upright, checked in fp64 on the host before anything changes
+  bool tilted = false;
+  {  // every masked quaternion upright (or, on a solid handle, whether one is tilted), checked in fp64 on the host before anything changes
     const size_t n = (size_t)h->n;
     double* hq = new (std::nothrow) double[4 * n];
     uint8_t* hm = mask ? new (std::nothrow) uint8_t[n] : nullptr;
@@ -162,17 +258,27 @@ extern "C" int pfb_set_static_pose(PfbHandle h, int body, const double* pos, con
     if (e == cudaSuccess) e = cudaStreamSynchronize(st);
     int64_t bad = -1;
     for (int64_t i = 0; e == cudaSuccess && bad < 0 && i < h->n; ++i)
-      if ((!hm || hm[i]) && !upright(hq + 4 * i)) bad = i;
+      if ((!hm || hm[i]) && !upright(hq + 4 * i)) {
+        tilted = true;
+        if (!h->static_solid) bad = i;
+      }
     delete[] hq;
     delete[] hm;
     if (e != cudaSuccess) return fail("pfb_set_static_pose: reading the quaternions failed: %s", cudaGetErrorString(e));
     if (bad >= 0)
-      return fail("pfb_set_static_pose: quat[%lld] is not upright (only a yaw about the world z axis): tilted static bodies are not modelled",
+      return fail("pfb_set_static_pose: quat[%lld] is not upright (only a yaw about the world z axis): tilted static bodies are not modelled "
+                  "under the top-face rule.  A solid handle (pfb_set_static_solid, solid_static_bodies=True) takes any orientation",
                   (long long)bad);
   }
-  const double* o = h->statics->inertial[body];
-  k_static_set_pose<<<grid_for(h->n), kBlock, 0, st>>>(h->statics->d_pose, body, pos, quat, mask, o[0], o[1], o[2], h->n);
+  StaticBodies* b = h->statics;
+  const double* o = b->inertial[body];
+  k_static_set_pose<<<grid_for(h->n), kBlock, 0, st>>>(b->d_pose, body, pos, quat, mask, o[0], o[1], o[2], h->n);
   LAUNCH_CHECK(h);
+  if (b->d_full) {
+    k_static_set_full_pose<<<grid_for(h->n), kBlock, 0, st>>>(b->d_full, body, pos, quat, mask, o[0], o[1], o[2], h->n);
+    LAUNCH_CHECK(h);
+  }
+  b->tilted = b->tilted || tilted;
   return 0;
 }
 
@@ -185,9 +291,16 @@ extern "C" int pfb_get_static_contacts(PfbHandle h, uint32_t* bits, void* stream
   return 0;
 }
 
-extern "C" int pfb_set_static_solid(PfbHandle h, int solid, void*) {
+extern "C" int pfb_set_static_solid(PfbHandle h, int solid, void* stream) {
   if (require_aviary_statics(h, "pfb_set_static_solid")) return -1;
   if (solid != 0 && solid != 1) return fail("pfb_set_static_solid: solid must be 0 (top faces) or 1 (every face), got %d", solid);
+  if (solid == 0 && h->statics && h->statics->tilted)
+    return fail("pfb_set_static_solid: the handle holds a tilted static body, primitive or pose since its last reset, which the top-face rule "
+                "does not model; reset it first");
+  if (solid == 1) {
+    CUDA_OK(cudaSetDevice(h->device));
+    if (static_alloc_full(h, (cudaStream_t)stream)) return -1;
+  }
   h->static_solid = solid == 1;
   return 0;
 }

@@ -1594,6 +1594,63 @@ def solid_fixtures():
                    [("wall_box.urdf", [50.0, 0.0, 0.0], ident)], {0: [4.0, 0.0, 0.0, 1.0]}, 220, seed=508, poses=poses)
 
 
+# ---- tilted static bodies (DESIGN.md §4h, "tilted static bodies") ----------------------------------------------------------
+def _quat(roll, pitch, yaw):
+    """PyBullet's getQuaternionFromEuler (x, y, z, w)"""
+    cr, sr, cp, sp, cy, sy = np.cos(roll / 2), np.sin(roll / 2), np.cos(pitch / 2), np.sin(pitch / 2), np.cos(yaw / 2), np.sin(yaw / 2)
+    return [sr * cp * cy - cr * sp * sy, cr * sp * cy + sr * cp * sy, cr * cp * sy - sr * sp * cy, cr * cp * cy + sr * sp * sy]
+
+
+def _quat_matrix(q):
+    x, y, z, w = q
+    return np.array([[1 - 2 * (y * y + z * z), 2 * (x * y - z * w), 2 * (x * z + y * w)], [2 * (x * y + z * w), 1 - 2 * (x * x + z * z), 2 * (y * z - x * w)],
+                     [2 * (x * z - y * w), 2 * (y * z + x * w), 1 - 2 * (x * x + y * y)]])
+
+
+def tilted_fixtures():
+    """The unmodified reference Aviary with tilted fixed-base bodies (a ramp, a race gate, a bar, a rolled wall, a pad pitched in
+    its URDF), on the fake client with the solid rule (solid_rule, which works in each primitive's full world rotation)."""
+    cf2x = dict(drone_model="cf2x")
+    idle = {0: [0.0, 0.0, 0.0, 0.0]}
+    ident = [0.0, 0.0, 0.0, 1.0]
+    with solid_rule():
+        # cf2x, motors idle, dropped on a ramp pitched 0.35 rad (under the friction angle atan 0.5 = 0.46 rad): it rests on it
+        fly_static("tilted_cf2x_ramp_rest", "quadx", cf2x, [[0.0, 0.0, 1.4]], [[0.0, 0.0, 0.0]], -1,
+                   [("ramp_slab.urdf", [0.0, 0.0, 1.0], _quat(0.0, 0.35, 0.0))], idle, 360, seed=601)
+        # the same drop on a ramp pitched 0.6 rad (over the friction angle): it slides down
+        fly_static("tilted_cf2x_ramp_slide", "quadx", cf2x, [[0.0, 0.0, 1.4]], [[0.0, 0.0, 0.0]], -1,
+                   [("ramp_slab.urdf", [0.0, 0.0, 1.0], _quat(0.0, 0.6, 0.0))], idle, 360, seed=602)
+        # cf2x in mode 7 through the centre of a race gate pitched 0.3 rad and yawed 1.0 rad: no gate bit
+        gq = _quat(0.0, 0.3, 1.0)
+        G = _quat_matrix(gq)
+        gc = np.array([1.5, 1.0, 1.0])
+        # level flight along the gate's normal seen from above, aimed 0.17 m over its centre: the drone sags that much while it
+        # gathers speed, and crosses the gate's plane near its centre
+        h = np.array([np.cos(1.0), np.sin(1.0), 0.0])
+        a, b = gc - 1.5 * h + [0.0, 0.0, 0.17], gc + 1.5 * h + [0.0, 0.0, 0.17]
+        fly_static("tilted_cf2x_gate_pass", "quadx", cf2x, [a.tolist()], [[0.0, 0.0, 0.0]], 7, [("race_gate.urdf", gc.tolist(), gq)],
+                   {0: [b[0], b[1], 0.0, b[2]]}, 300, seed=603)
+        # the same level flight through the centre of the gate's top bar: the bit is set and the drone is deflected
+        a2, b2 = a + 0.225 * G[:, 2], b + 0.225 * G[:, 2]
+        fly_static("tilted_cf2x_gate_bar", "quadx", cf2x, [a2.tolist()], [[0.0, 0.0, 0.0]], 7, [("race_gate.urdf", gc.tolist(), gq)],
+                   {0: [b2[0], b2[1], 0.0, b2[2]]}, 240, seed=604)
+        # primitive_drone, motors idle, dropped onto a horizontal cylinder bar just off its axis: the radial normal turns it off
+        fly_static("tilted_primitive_bar_drop", "quadx", dict(drone_model="primitive_drone"), [[0.06, 0.0, 1.6]], [[0.0, 0.0, 0.0]], -1,
+                   [("bar_cylinder.urdf", [0.0, 0.0, 0.0], ident)], idle, 360, seed=605)
+        # a fixed-wing in powered level flight into a 1 m thick wall rolled 0.3 rad about x
+        fly_static("tilted_fixedwing_rolled_wall", "fixedwing", dict(drone_model="fixedwing"), [[0.0, 0.0, 5.0]], [[0.0, 0.0, 0.0]], 0,
+                   [("thick_wall.urdf", [20.0, 0.0, 0.0], _quat(0.3, 0.0, 0.0))], {0: [0.0, 0.0, 0.0, 0.8]}, 360, seed=606)
+        # a rocket lowered onto a pad pitched 0.08 rad in its URDF and rolled 0.05 rad by its pose, booster off
+        fly_static("tilted_rocket_pad", "rocket", dict(drone_model="rocket"), [[0.2, 0.1, 3.0]], [[0.0, 0.0, 0.0]], 0,
+                   [("tilted_pad.urdf", [0.0, 0.0, 0.0], _quat(0.05, 0.0, 0.0))], {0: [0, 0, 0, 0, 0, 0, 0]}, 240, seed=607)
+        # per-world poses: resetBasePositionAndOrientation tilts the wall into the path in two worlds and moves it away in the third
+        poses = [{0: ([1.5, 0.0, 1.5], _quat(0.0, 0.3, 0.2))},
+                 {0: ([1.6, 0.3, 1.5], _quat(0.4, -0.2, -0.3))},
+                 {0: ([1.5, 8.0, 1.5], _quat(0.2, 0.2, 0.0))}]
+        fly_static("tilted_cf2x_per_drone_poses", "quadx", cf2x, [[0.0, 0.0, 1.0]] * 3, [[0.0, 0.0, 0.0]] * 3, 7,
+                   [("wall_box.urdf", [50.0, 0.0, 0.0], ident)], {0: [4.0, 0.0, 0.0, 1.0]}, 220, seed=608, poses=poses)
+
+
 if __name__ == "__main__":
     os.makedirs(OUT, exist_ok=True)
     which = sys.argv[1] if len(sys.argv) > 1 else "all"
@@ -1631,3 +1688,5 @@ if __name__ == "__main__":
         static_fixtures()
     if which in ("all", "solid"):
         solid_fixtures()
+    if which in ("all", "tilted"):
+        tilted_fixtures()
